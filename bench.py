@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — utterances/sec of the TC-ResNet training step (MFCC front-end + fwd + bwd + SGD-momentum).
 
-  python bench.py --gpus N --steps K --warmup W                 # our sm_100a CUDA path (one rank per GPU under torchrun)
+  python bench.py --gpus N --steps K --warmup W                 # our sm_90a CUDA path (one rank per GPU under torchrun)
   python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path restated (oracle port)
 
 Prints ONE JSON line (rank 0).  A "step" = one pass of the hot path over one batch of synthetic 16 kHz 1 s
@@ -54,27 +54,37 @@ def parse_args():
                     help="train: the headline training step; dscnn: DS-CNN-S forward (BASELINE.json config 5, comparison point); "
                          "infer: evaluation-mode forward from wav (config 1 with --batch 1: latency); "
                          "augment: the device input stage (SURVEY.md 8f row 1), an HBM-bound elementwise pass")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its last step (the arrays its caller receives) "
+                         "as DIR/<name>.npy in float32; the inputs are seeded, so two builds can be compared output for output")
     return ap.parse_args()
+
+
+DUMP_MAX_ELEMS = 4 << 20        # per array: at most 16 MB of float32 (a fixed, seeded sample of a larger output)
+
+
+def dump_outputs(a, arrays):
+    """--dump-outputs DIR: DIR/<name>.npy (float32) for every array; an array of more than DUMP_MAX_ELEMS elements is replaced by
+    the elements at a fixed, seeded set of flat indices (the same on every run), so the files stay under 64 MB in all."""
+    if not a.dump_outputs:
+        return
+    import numpy as np
+    os.makedirs(a.dump_outputs, exist_ok=True)
+    for name, t in arrays.items():
+        x = t.detach().float().cpu().numpy().ravel() if hasattr(t, "detach") else np.asarray(t, np.float32).ravel()
+        if x.size > DUMP_MAX_ELEMS:
+            x = x[np.sort(np.random.default_rng(0).choice(x.size, DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(a.dump_outputs, name + ".npy"), x.astype(np.float32))
 
 
 def l2_policy(a, clip=16000):
     rot = max(1, a.rotate)
-    return f"inputs rotate over {rot} distinct batches ({rot * a.batch * clip * 4 / 1e6:.0f} MB > 126 MB L2)"
+    return f"inputs rotate over {rot} distinct batches ({rot * a.batch * clip * 4 / 1e6:.0f} MB; the H100's L2 is 50 MB)"
 
 
 def make_config(a, world, exchange):
     """The SAME keys in both arms (the driver compares them)."""
     return {"workload": workload_name(a), "global_batch": a.batch * world, "l2": l2_policy(a), "exchange": exchange}
-
-
-def sources_sha():
-    """Hash of the kernel sources: a committed ncu capture is only quoted while it describes THESE kernels."""
-    import glob
-    import hashlib
-    h = hashlib.sha1()
-    for f in sorted(glob.glob(os.path.join(ROOT, "tc-resnet_b200", "csrc", "*.cu*")) + glob.glob(os.path.join(ROOT, "tc-resnet_b200", "csrc", "*.h"))):
-        h.update(open(f, "rb").read())
-    return h.hexdigest()[:16]
 
 
 def pin_to_gpu_numa_node(dev_index):
@@ -106,7 +116,7 @@ def workload_name(a):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks (B200_PROFILING.md recipe)
+# clocks: nvidia-smi queried every 100 ms during the timed steps
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     def __init__(self, index: int):
@@ -171,9 +181,8 @@ def cpu_port_step_fn(a, batch, threads=None):
 
 
 def calibrate_cpu_threads(a):
-    """The tensors of this path are tiny: intra-op parallelism over all 128 host cores is SLOWER than over 16 (measured on the
-    B200 box: 7.6 s per step of 32 utterances at 128 threads).  Give the CPU arm its best thread count: time one step of 128
-    utterances at each candidate and keep the fastest."""
+    """The tensors of this path are tiny: on a many-core host, intra-op parallelism over all cores can be SLOWER than over 16.
+    Give the CPU arm its best thread count: time one step of 128 utterances at each candidate and keep the fastest."""
     global _CPU_THREADS
     if _CPU_THREADS is not None:
         return _CPU_THREADS
@@ -350,6 +359,8 @@ def run_ours(a):
     ms = float(ms.item())
     launches = eng.launch_count() - launches0
     clocks = sampler.stop() if sampler else None
+    if rank == 0:
+        dump_outputs(a, {"losses": losses, "params": params, "slots": slots, "moving": moving})
     final_loss = float(losses[0].item())
     value = n * world * a.steps / (ms * 1e-3)
 
@@ -399,7 +410,7 @@ def run_ours(a):
         from tcresnet_b200.engine import HostFeed
         h_wavs = [w.cpu().pin_memory() for w in wavs[:min(rot, 4)]]
         h_hots = [o.cpu().pin_memory() for o in onehots[:min(rot, 4)]]
-        esteps = max(100, min(a.steps, 200))            # never fewer than 100 timed steps, whatever --steps says
+        esteps = a.steps
 
         def e2e_run(host_wavs, host_clips=None, background=None):
             feed = HostFeed(eng, lag=2)
@@ -517,8 +528,8 @@ def run_ours(a):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet)"
         total_ms = sum(v[0] for v in stats.values())
         top = sorted(stats.items(), key=lambda kv: -kv[1][0])
         kernels = []
@@ -527,21 +538,6 @@ def run_ours(a):
             dur = tms / cnt * 1e-3
             kernels.append({"name": name, "us": dur * 1e6, "share": tms / total_ms, "GBps": b / dur / 1e9, "TFLOPs": f / dur / 1e12})
         dom = kernels[0]
-        # DRAM traffic of the dominant kernel from the committed ncu --set full capture (profiles/, same workload)
-        traffic, traffic_src = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic_tcresnet8_b512.json")))
-            if tj.get("kernels_sha") != sources_sha():           # a capture of OTHER kernels is not evidence for these
-                traffic_src = f"stale capture ignored ({tj.get('source')}: kernels_sha {tj.get('kernels_sha')} != {sources_sha()})"
-            elif a.model == "TCResNet8" and a.width == 1.0 and n == 512:
-                ncu_name = {"mfcc": ("mfcc_pair_kernel", "mfcc_kernel"), "dw_grouped": ("dw_grouped_kernel",), "head": ("head_kernel",),
-                            "resident_fwd": ("resident_fwd_kernel",), "resident_bwd": ("resident_bwd_kernel",),
-                            "resident_bwd_data": ("resident_bwd_kernel",)}.get(dom["name"])
-                for k, v in tj["bytes_per_launch"].items():
-                    if ncu_name and k.startswith(ncu_name):
-                        traffic, traffic_src = v, f"profiles/ncu_traffic_tcresnet8_b512.json ({tj['source']})"
-        except Exception:
-            pass
         alg_bytes, alg_flops = kernel_work(plan, dom["name"], n)
         # which pipe binds this kernel: the larger of its two floors (bytes / HBM peak, flops / fp32-FMA peak)
         t_hbm, t_fma = alg_bytes / (hbm_peak * 1e9), alg_flops / max(fp32_peak * 1e12, 1.0)
@@ -551,8 +547,8 @@ def run_ours(a):
                                    "the FMA pipe because single TF32 / BF16 products miss the 1e-4 logit bound (DESIGN.md)"}
         binding = fma_form if t_fma > t_hbm else hbm_form
         out["roofline"] = {"bound": "fp32-fma" if t_fma > t_hbm else "hbm", "kernel": dom["name"], "achieved": binding["achieved"],
-                           "peak": binding["peak"], "unit": binding["unit"], "frac": binding["frac"], "traffic": traffic,
-                           "traffic_source": traffic_src, "algorithmic_bytes_per_launch": alg_bytes,
+                           "peak": binding["peak"], "unit": binding["unit"], "frac": binding["frac"], "traffic": None,
+                           "algorithmic_bytes_per_launch": alg_bytes,
                            "algorithmic_flops_per_launch": alg_flops, "floors_us": {"hbm": t_hbm * 1e6, "fp32_fma": t_fma * 1e6},
                            "kernel_us": dom["us"], "kernel_share_of_step": dom["share"], "hbm": hbm_form, "fp32": fma_form,
                            "step": {"train_flops_per_utt": plan.train_flops(), "min_bytes_per_utt": plan.min_bytes(n),
@@ -600,7 +596,7 @@ def quick_train(torch, dev, model, width, batch, window_ms, stride_ms, fp32_peak
     value = batch / (ms * 1e-3)
     eng.close()
     return {"metric": f"utterances/sec (fwd+bwd+update) {model}-{width:g}", "value": value, "ms_per_step": ms, "batch": batch, "steps": steps,
-            "warmup": warmup, "l2": f"inputs rotate over {rot} resident batches ({rot * batch * plan.clip * 4 / 1e6:.0f} MB > 126 MB L2)",
+            "warmup": warmup, "l2": f"inputs rotate over {rot} resident batches ({rot * batch * plan.clip * 4 / 1e6:.0f} MB; the H100's L2 is 50 MB)",
             "final_total_loss": float(losses[0].item()), "train_flops_per_utt": plan.train_flops(),
             "fp32_frac": plan.train_flops() * value / 1e12 / max(fp32_peak, 1e-9)}
 
@@ -626,7 +622,7 @@ def quick_dscnn(torch, dev, n, steps=40, warmup=6, rot=8):
     ms = e0.elapsed_time(e1) / steps
     return {"metric": "utterances/sec (forward) DS-CNN-S", "value": n / (ms * 1e-3), "ms_per_step": ms, "batch": n, "steps": steps,
             "forward_flops_per_utt": net.forward_flops, "tflops": n / (ms * 1e-3) * net.forward_flops / 1e12,
-            "pointwise": "tcgen05 3xTF32 (csrc/tcr_dscnn.cu)" if os.environ.get("TCR_DSCNN_TC", "1") != "0" else "fp32 FMA"}
+            "pointwise": "wgmma 3xTF32 (csrc/tcr_dscnn.cu)" if os.environ.get("TCR_DSCNN_TC", "1") != "0" else "fp32 FMA"}
 
 
 def run_infer(a):
@@ -647,9 +643,10 @@ def run_infer(a):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(a.steps):
-        eng.forward(wavs[i % a.rotate], params, moving)
+        res = eng.forward(wavs[i % a.rotate], params, moving)
     e1.record()
     torch.cuda.synchronize()
+    dump_outputs(a, {"logits": res["logits"], "probs": res["probs"]})
     ms = e0.elapsed_time(e1) / a.steps
     h_wav = wavs[0].cpu().pin_memory()
     d_wav = torch.empty_like(wavs[0])
@@ -692,27 +689,28 @@ def run_augment(a):
         eng.augment(pcm[i % rot], clips[i % rot], background, out=outs[i % rot])
     e1.record()
     torch.cuda.synchronize()
+    dump_outputs(a, {"wav": outs[(a.steps - 1) % rot]})
     ms = e0.elapsed_time(e1) / a.steps
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     alg = n * clip * (2 + 4 + 4)                       # int16 read + background read + fp32 write per sample
     gbs = alg / (ms * 1e-3) / 1e9
     emit({"metric": "utterances/sec (device input stage: decode + shift + background mix + clip)", "value": n / (ms * 1e-3),
           "unit": "utterances/sec", "n_gpus": 1, "steps": a.steps, "warmup": max(a.warmup, 3), "ms_per_step": ms,
           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "impl": "ours",
           "config": {"workload": f"tcr_augment_pcm16, batch {n} clips of 16000 samples, 6 background recordings of 60 s",
-                     "l2": f"inputs/outputs rotate over {rot} buffers ({rot * alg / 1e6:.0f} MB > 126 MB L2)"},
+                     "l2": f"inputs/outputs rotate over {rot} buffers ({rot * alg / 1e6:.0f} MB; the H100's L2 is 50 MB)"},
           "roofline": {"bound": "hbm", "kernel": "augment", "achieved": gbs, "peak": hbm_peak, "unit": "GB/s", "frac": gbs / hbm_peak,
                        "traffic": None, "algorithmic_bytes_per_launch": alg},
           "gpu_launches": eng.launch_count()})
 
 
 def run_dscnn(a):
-    """Config 5: DS-CNN-S forward, MFCC 49x40 features resident in HBM, batch 512, one B200 (2-D-conv comparison point)."""
+    """Config 5: DS-CNN-S forward, MFCC 49x40 features resident in HBM, batch 512, one GPU (2-D-conv comparison point)."""
     import torch
     import tcresnet_b200  # noqa: F401
     from tcresnet_b200.dscnn import DsCnn
@@ -731,9 +729,10 @@ def run_dscnn(a):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for i in range(a.steps):
-        net.forward(feats[i % a.rotate], params)
+        res = net.forward(feats[i % a.rotate], params)
     e1.record()
     torch.cuda.synchronize()
+    dump_outputs(a, {"logits": res[0], "probs": res[1]})
     ms = e0.elapsed_time(e1)
     value = n * a.steps / (ms * 1e-3)
     # per-kernel durations (separate pass: the event brackets add overhead) and the roofline of the dominant kernel
@@ -770,22 +769,21 @@ def run_dscnn(a):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
     dom = kernels[0]
     alg_b, alg_f = work.get(dom["name"], (0, 0))
     roofline = {"bound": "hbm", "kernel": dom["name"], "achieved": dom["GBps"], "peak": hbm_peak, "unit": "GB/s",
                 "frac": dom["GBps"] / hbm_peak,
-                "peak_source": "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)",
+                "peak_source": "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 3350 GB/s (H100 SXM data sheet)",
                 "traffic": None, "algorithmic_bytes_per_launch": alg_b, "algorithmic_flops_per_launch": alg_f,
                 "kernel_us": dom["us"], "kernel_share_of_step": dom["share"],
-                "note": "activations in + out once per block (fp32 NHWC); the 1x1 conv runs on tcgen05 as three TF32 passes "
-                        "(6.3 GFLOP/launch incl. the split, a ~6 us floor at the tf32 peak), so HBM is the roofline; ncu shows the "
-                        "L1/shared-memory data pipe as the busiest unit (profiles/r02_dscnn_*.txt)"}
+                "note": "activations in + out once per block (fp32 NHWC); the 1x1 conv runs on wgmma as three TF32 passes "
+                        "(6.3 GFLOP/launch incl. the split, a ~13 us floor at the H100's dense TF32 data-sheet rate), so HBM is the roofline"}
     # end to end through the public call with HOST features: pinned host -> H2D -> forward -> D2H probabilities, every step
     h_feats = [f.cpu().pin_memory() for f in feats[:4]]
     d_in = torch.empty(n, 49, 40, device=dev)
     h_out = torch.empty(n, 12).pin_memory()
-    esteps = max(100, min(a.steps, 200))
+    esteps = a.steps
     for i in range(12):
         d_in.copy_(h_feats[i % 4], non_blocking=True)
         h_out.copy_(net.forward(d_in, params)[1], non_blocking=True)
@@ -801,9 +799,9 @@ def run_dscnn(a):
                       "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic", "impl": "ours",
                       "config": {"workload": f"DS-CNN-S forward (inference), MFCC 49x40 features resident in HBM, batch {n}",
                                  "global_batch": n, "l2": f"inputs rotate over {a.rotate} resident batches; every block streams "
-                                                          f"{2 * act / 1e6:.0f} MB of activations (> 126 MB L2 over a step)",
+                                                          f"{2 * act / 1e6:.0f} MB of activations (the H100's L2 is 50 MB)",
                                  "exchange": "none (1 GPU)", "forward_flops_per_utt": net.forward_flops,
-                                 "pointwise": "fp32 FMA" if os.environ.get("TCR_DSCNN_TC", "2") == "0" else "tcgen05 3xTF32"},
+                                 "pointwise": "fp32 FMA" if os.environ.get("TCR_DSCNN_TC", "2") == "0" else "wgmma 3xTF32"},
                       "fp32_tflops": value * net.forward_flops / 1e12, "roofline": roofline, "kernels": kernels,
                       "gpu_launches": int(sum(k["launches_per_step"] for k in kernels) * a.steps),
                       "e2e": {"value": e2e_v, "unit": "utterances/sec", "h2d_bytes_per_step": n * 49 * 40 * 4,

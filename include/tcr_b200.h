@@ -1,4 +1,4 @@
-/* tcr_b200.h — C ABI of the B200-native TC-ResNet hot path (libtcr_b200.so).
+/* tcr_b200.h — C ABI of the H100-native TC-ResNet hot path (libtcr_b200.so).
  *
  * The reference (hyperconnect/TC-ResNet) has no FFI: its "plugin API" is Python-level and the
  * arithmetic runs inside TensorFlow 1.13's Session.run.  This header is the boundary a maintainer

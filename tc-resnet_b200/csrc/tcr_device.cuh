@@ -1,4 +1,4 @@
-// tcr_device.cuh — device-side helpers shared by all kernels of libtcr_b200 (sm_100a).
+// tcr_device.cuh — device-side helpers shared by all kernels of libtcr_b200 (sm_90a).
 // The TCR_EMU branch only exists so tests/emu can run the same kernel logic on a CPU box;
 // the product library is always built by nvcc without TCR_EMU.
 #pragma once

@@ -1,4 +1,4 @@
-// tcr_dscnn.cu — DS-CNN (Hello-Edge) forward pass for sm_100a: the reference's 2-D-conv comparison model
+// tcr_dscnn.cu — DS-CNN (Hello-Edge) forward pass for sm_90a: the reference's 2-D-conv comparison model
 // (audio_nets/ds_cnn.py:20-118, BASELINE.json config 5), inference mode.
 //
 //   dscnn_conv_kernel      first layer: kh x kw conv from the single-channel feature map (+bias, BN, ReLU)
@@ -198,26 +198,77 @@ __global__ void __launch_bounds__(256) dscnn_dsblock_kernel(DsLayerDev L, int RH
   }
 }
 
-// ---- depthwise-separable block with the pointwise 1x1 conv on the 5th-generation tensor cores (tcgen05 / UMMA) ----
+// ---- depthwise-separable block with the pointwise 1x1 conv on the Hopper tensor cores (wgmma) ----
 // The pointwise conv IS a dense [positions, C] x [C, CO] contraction (audio_nets/ds_cnn.py:56-59), 77 % of DS-CNN-S's FLOPs.
-// Per CTA: 128 accumulator rows (RH output rows x wout positions, RH * wout <= 128) x CO columns in TMEM.
-//   * single TF32 products miss the 1e-4 logit bound (6.7e-4 relative on a K = 64 dot product, tools/ubench/umma_tf32.cu), so every
-//     operand is split x = hi + lo with hi = x truncated to TF32 (low 13 mantissa bits cleared, lo = x - hi exact) and three MMAs
-//     accumulate lo*hi + hi*lo + hi*hi in fp32: 4e-7 relative, the same as the FMA kernel;
-//   * operands sit in shared memory in UMMA's canonical K-major no-swizzle layout, element (row, k) at float offset
+// Per tile: 128 accumulator rows (RH output rows x wout positions, RH * wout <= 128) x CO columns, held in the registers of the
+// warpgroup(s) that issue the MMAs.
+//   * single TF32 products miss the 1e-4 logit bound (6.7e-4 relative on a K = 64 dot product), so every operand is split
+//     x = hi + lo with hi = x truncated to TF32 (low 13 mantissa bits cleared, lo = x - hi exact) and three MMAs accumulate
+//     lo*hi + hi*lo + hi*hi in fp32: 4e-7 relative, the same as the FMA kernel;
+//   * operands sit in shared memory in wgmma's K-major no-swizzle layout, element (row, k) at float offset
 //     (k / 4) * LBO + row * 4 + k % 4: an 8-row core matrix is 128 contiguous bytes, 8-row groups are 128 B apart (SBO) and the
 //     K-chunk stride LBO is padded by 16 B so that neither the depthwise stage's float4 stores nor the filter staging conflict;
-//   * one thread issues the 3 * C/8 tcgen05.mma (M = 128, N = CO, K = 8) and commits them to an mbarrier; all 8 warps then read
-//     their TMEM lane quarter (warp % 4) and column half (warp / 4) with tcgen05.ld, apply the folded BatchNorm + ReLU, store.
+//   * wgmma.mma_async m64nNk8 (TF32 operands, fp32 accumulators): one instruction covers 64 rows, K = 8 (two 4-wide chunks).
+//     Thread (warp w of the warpgroup, lane l) holds rows 16 w + l / 4 and 16 w + l / 4 + 8, columns 8 j + 2 (l % 4) and + 1:
+//     d[4 j + 2 h + e] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + e].
 // The input rows are staged channel-chunk-major ([C/4][rows*wp][4]) so that lanes walking positions read conflict-free float4s.
 #ifndef TCR_EMU
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// wgmma shared-memory matrix descriptor: start address >> 4 in bits [0,14), leading (K-chunk) byte offset >> 4 in [16,30),
+// stride (8-row group) byte offset >> 4 in [32,46); base offset 0 and layout type 0 (no swizzle) in the high bits.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);                  // start address >> 4, bits [0,14)
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;         // leading (K-chunk) byte offset >> 4, bits [16,30)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;         // stride (8-row group) byte offset >> 4, bits [32,46)
-  d |= (uint64_t)1 << 46;                                   // descriptor version 1 (sm_100); layout type 0 = no swizzle
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   return d;
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 64] += A[64 x 8] B[64 x 8]^T, both operands K-major TF32 in shared memory
+__device__ __forceinline__ void wgmma_m64n64k8_tf32(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db)
+      : "memory");
+}
+// D[64 x 32] += A[64 x 8] B[32 x 8]^T
+__device__ __forceinline__ void wgmma_m64n32k8_tf32(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db)
+      : "memory");
+}
+// Folded BatchNorm + ReLU of a warpgroup's accumulator fragment (NA instructions' worth of 64-row blocks, NJ 8-column groups)
+// and the NHWC store: accumulator row m -> out[(gbase + m) * CO + col0 + column], rows >= npos are not stored.
+template <int NA, int NJ>
+__device__ __forceinline__ void gmma_epilogue(const float (&acc)[NA][4 * NJ], int m0, int col0, int CO, int npos, const float* sc,
+                                              const float* sf, float* __restrict__ out, size_t gbase, int wtid) {
+  const int r0 = m0 + 16 * (wtid >> 5) + ((wtid & 31) >> 2), c = 2 * (wtid & 3);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int co = col0 + 8 * j + c;
+    const float2 s = ld2(sc + co), t = ld2(sf + co);
+#pragma unroll
+    for (int q = 0; q < 2 * NA; ++q) {                            // rows r0, r0 + 8, r0 + 64, r0 + 72
+      const int m = r0 + 8 * (q & 1) + 64 * (q >> 1);
+      if (m < npos) {
+        const float* a = &acc[q >> 1][4 * j + 2 * (q & 1)];
+        *reinterpret_cast<float2*>(out + (gbase + m) * CO + co) = make_float2(fmaxf(fmaf(a[0], s.x, t.x), 0.f), fmaxf(fmaf(a[1], s.y, t.y), 0.f));
+      }
+    }
+  }
 }
 __device__ __forceinline__ void tf32_split(float4 v, float4& hi, float4& lo) {
   hi = make_float4(__uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u),
@@ -230,24 +281,23 @@ __device__ __forceinline__ void cp_async16_zfill(float* dst_smem, const float* s
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes) : "memory");
 }
 
-// Persistent: a CTA keeps the split filter bank, the TMEM allocation and the per-channel tables for all its tiles
-// (tile = RH output rows of one utterance), and the next tile's input rows travel (cp.async) while the current tile is computed.
+// Persistent: a CTA keeps the split filter bank and the per-channel tables for all its tiles (tile = RH output rows of one
+// utterance), and the next tile's input rows travel (cp.async) while the current tile is computed.
 // Specialised for the 3x3 / stride-1 depthwise stage (every separable block of DS-CNN-S, audio_nets/ds_cnn.py:20-26):
 //   * depthwise: a thread owns (4 channels, one output column) and slides down the rows, so every input float4 is read once
 //     per thread (3 loads per output instead of 9) and the 9 taps stay in registers;
-//   * two TMEM accumulators: the MMAs of tile i run while the epilogue of tile i-1 drains the other one;
-//   * the UMMA descriptors are formed once; a k-step only adds its byte offset to the start-address field.
+//   * the four warpgroups then each issue the 3 * C/8 wgmma (m64, n = CO/2, k8) of one quarter of the accumulator
+//     (rows 64 (g % 2) .., columns (g / 2) CO/2 ..) and drain it from their registers;
+//   * the descriptors are formed once; a k-step only adds its byte offset to the start-address field.
 constexpr int kTcThreads = 512;
 template <int C, int CO>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
                                                                   const float* __restrict__ in, float* __restrict__ out, float eps) {
+  static_assert(CO == 64, "one m64n32k8 quarter per warpgroup");
   TCR_DYNAMIC_SMEM(smem_raw);
-  __shared__ uint64_t mma_bar[2];
-  __shared__ uint32_t tmem_base_s;
   float* smem = reinterpret_cast<float*>(smem_raw);
   constexpr int C4 = C / 4, KS = C / 8;
-  constexpr int TMEM_COLS = 2 * CO <= 32 ? 32 : (2 * CO <= 64 ? 64 : (2 * CO <= 128 ? 128 : 256));
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int hin_t = RH + 2;                                       // 3x3, stride 1
   const int wp = L.wout + 2;
   const int XP = hin_t * wp * 4 + 4;                              // floats per channel chunk of the input tile (+16 B against conflicts)
@@ -264,11 +314,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
   float* sf2 = sc2 + CO;
   const int tpu = (L.hout + RH - 1) / RH;                         // tiles per utterance
   const int ntiles = tpu * n_utt;
-  if (tid == 0) { mbar_init(&mma_bar[0], 1); mbar_init(&mma_bar[1], 1); }
-  if (warp == 0) {                                               // TMEM: two accumulators of 128 lanes x CO fp32 columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   // pointwise filters pw[ci][co] -> B operand [n = co][k = ci], hi / lo parts (params are caller-owned: independent of the producer)
   for (int i0 = tid; i0 < C * CO; i0 += kTcThreads * 8) {
     float v[8];
@@ -315,57 +360,19 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
       }
     }
   };
-  // epilogue of one tile: accumulator row m = 32 * (warp % 4) + lane, columns [(warp / 4) * CO / NG, + CO / NG), batches of 16
-  auto epilogue = [&](uint32_t tacc, int tile_e) {
-    const int n = tile_e / tpu, h0 = (tile_e - n * tpu) * RH, npos = imin(RH, L.hout - h0) * L.wout;
-    constexpr int NG = kTcThreads / 128;                           // column groups: every warp reads its TMEM lane quarter
-    const int m = 32 * (warp & 3) + lane, cbase = (warp >> 2) * (CO / NG);
-    const size_t gbase = ((size_t)n * L.hout + h0) * L.wout;
-#pragma unroll
-    for (int c0 = 0; c0 < CO / NG; c0 += 16) {
-      uint32_t r[16];
-      const uint32_t taddr = tacc + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)(cbase + c0);
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                   : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                     "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                   : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (m < npos) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const int co = cbase + c0 + j;
-          const float4 s = ld4(sc2 + co), t = ld4(sf2 + co);
-          st4(out + (gbase + m) * CO + co,
-              make_float4(fmaxf(fmaf(__uint_as_float(r[j]), s.x, t.x), 0.f), fmaxf(fmaf(__uint_as_float(r[j + 1]), s.y, t.y), 0.f),
-                          fmaxf(fmaf(__uint_as_float(r[j + 2]), s.z, t.z), 0.f), fmaxf(fmaf(__uint_as_float(r[j + 3]), s.w, t.w), 0.f)));
-        }
-      }
-    }
-  };
-  int tile = blockIdx.x, cur = 0, it = 0, prev_tile = -1;
-  uint32_t parity[2] = {0u, 0u};
+  // this warpgroup's quarter of the accumulator
+  const int g = warp >> 2, m0 = 64 * (g & 1), col0 = (g >> 1) * (CO / 2);
+  const uint64_t da_hi = gmma_desc(smem_u32(a_hi + 4 * m0), LBA * 4u, 128u), da_lo = gmma_desc(smem_u32(a_lo + 4 * m0), LBA * 4u, 128u);
+  const uint64_t db_hi = gmma_desc(smem_u32(b_hi + 4 * col0), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo + 4 * col0), LBB * 4u, 128u);
+  int tile = blockIdx.x, cur = 0;
   if (tile < ntiles) fetch_tile(tile, xs0);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base_s;
-  // instruction descriptor: D fp32 (bits 4-5 = 1), A and B TF32 (bits 7-9, 10-12 = 2), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-  constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(CO >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  const uint64_t da_hi = umma_desc(smem_u32(a_hi), LBA * 4u, 128u), da_lo = umma_desc(smem_u32(a_lo), LBA * 4u, 128u);
-  const uint64_t db_hi = umma_desc(smem_u32(b_hi), LBB * 4u, 128u), db_lo = umma_desc(smem_u32(b_lo), LBB * 4u, 128u);
-  for (; tile < ntiles; tile += gridDim.x, cur ^= 1, ++it) {
+  for (; tile < ntiles; tile += gridDim.x, cur ^= 1) {
     const int n = tile / tpu, h0 = (tile - n * tpu) * RH, rh = imin(RH, L.hout - h0);
-    (void)n;
     float* xs = xs0 + (size_t)cur * C4 * XP;
     asm volatile("cp.async.wait_all;" ::: "memory");
-    __syncthreads();                                             // this tile's rows have landed
+    // this tile's rows have landed, and every warpgroup has finished the previous tile's MMAs (the A tiles are free)
+    __syncthreads();
     if (tile + (int)gridDim.x < ntiles) fetch_tile(tile + gridDim.x, xs0 + (size_t)(cur ^ 1) * C4 * XP);
-    // the previous tile's MMAs read the A tiles: they must be done before the depthwise stage overwrites them
-    if (prev_tile >= 0) {
-      mbar_wait(&mma_bar[(it - 1) & 1], parity[(it - 1) & 1]);
-      parity[(it - 1) & 1] ^= 1u;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
     // depthwise 3x3 + folded BN + ReLU -> A operand (hi / lo): thread = (channel chunk, output column), sliding down the rows
     // row segments keep every thread busy: (segment, channel chunk, column) tasks, a segment re-reads its two halo rows
     const int ntask0 = C4 * L.wout;
@@ -405,129 +412,78 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
     }
     // accumulator rows past rh * wout are never stored, whatever the A rows there hold (each output row depends on its own A row only)
     fence_proxy_async();                                         // generic-proxy stores of the operands -> visible to the async proxy
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (tid == 0) {
-      const uint32_t tacc = tmem + (uint32_t)((it & 1) * CO);
+    float acc[1][CO / 8 * 2];
 #pragma unroll
-      for (int pass = 0; pass < 3; ++pass) {                     // lo*hi, hi*lo, hi*hi: the small terms first
-        const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
+    for (int i = 0; i < CO / 4; ++i) acc[0][i] = 0.f;
+    wgmma_fence();
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {                        // one MMA covers K = 8 = two 4-wide chunks
-          const uint64_t da = da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db = db0 + (uint64_t)((2 * ks * LBB * 4) >> 4);
-          const uint32_t accumulate = (pass | ks) ? 1u : 0u;
-          asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                       "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                       ::"r"(tacc), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-        }
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mma_bar[it & 1])) : "memory");
+    for (int pass = 0; pass < 3; ++pass) {                       // lo*hi, hi*lo, hi*hi: the small terms first
+      const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks)                            // one MMA covers K = 8 = two 4-wide chunks
+        wgmma_m64n32k8_tf32(acc[0], da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db0 + (uint64_t)((2 * ks * LBB * 4) >> 4));
     }
-    // while these MMAs run: drain the previous tile's accumulator (its MMAs were waited for above)
-    if (prev_tile >= 0) epilogue(tmem + (uint32_t)(((it - 1) & 1) * CO), prev_tile);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    prev_tile = tile;
+    wgmma_commit();
+    wgmma_wait_all();
+    gmma_epilogue<1, CO / 16>(acc, m0, col0, CO, rh * L.wout, sc2, sf2, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
   }
-  if (prev_tile >= 0) {
-    mbar_wait(&mma_bar[(it - 1) & 1], parity[(it - 1) & 1]);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    epilogue(tmem + (uint32_t)(((it - 1) & 1) * CO), prev_tile);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
 }
 
 // Warp-specialised version of the block above (the default): the stages of a tile run on different warps and meet on mbarriers,
-// so the input fetch, the depthwise stage, the MMAs and the epilogue of neighbouring tiles overlap instead of taking turns.
+// so the input fetch and the depthwise stage of the next tile overlap the MMAs and the epilogue of this one.
 //   warps 0-9   producers: TMA fetch of the tile two ahead (cp.async.bulk.tensor into the input buffer they have just left) and
 //               the depthwise stage, input tile -> A operand (hi / lo); both double-buffered
-//   warp  10    one elected thread issues the 3 * C/8 tcgen05.mma of a tile and commits them to `mma_done`
-//   warps 12-15 epilogue (TMEM lane quarter = warp % 4, all CO columns)
-// Barriers (index = tile parity): in_full (TMA complete_tx), a_full (producers), mma_done (tcgen05.commit),
-// tmem_empty (epilogue warps).  A rows are packed to the tile's own row count (rounded to 8): the M = 128 MMA then reads a few
-// rows of the next K chunk as rows >= npos, whose accumulator rows are never stored.
-constexpr int kWsProducerWarps = 10, kWsProducers = 32 * kWsProducerWarps, kWsFetchers = 128;
+//   warps 12-15 consumer warpgroup: the 3 * C/8 k-steps of a tile (two wgmma m64nCOk8 each: accumulator rows 0-63, 64-127),
+//               then the epilogue from its registers
+// Barriers (index = tile parity): in_full (TMA complete_tx), a_full (producers), mma_done (the consumer warpgroup, once its
+// MMAs have completed: the A buffer may be refilled).  A rows are packed to the tile's own row count (rounded to 8): the
+// 128-row MMA then reads a few rows of the next K chunk as rows >= npos, whose accumulator rows are never stored.
+constexpr int kWsProducerWarps = 10, kWsProducers = 32 * kWsProducerWarps, kWsConsumers = 128;
+constexpr int kWsConsumerWarp0 = kTcThreads / 32 - 4;
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {       // arrives when this thread's earlier cp.asyncs have landed
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// The MMA and epilogue roles of the warp-specialised kernels (shared by the separable block and the first conv).
-// MMA role, one thread: per tile 3 * K4/2 tcgen05.mma (M = 128, N = CO, K = 8) on A buffer it % 2 -> TMEM accumulator it % 2.
+// The consumer role of the warp-specialised kernels (shared by the separable block and the first conv), one warpgroup
+// (wtid = thread index within it): per tile 3 * K4/2 k-steps on A buffer it % 2, then the folded BatchNorm + ReLU and the
+// NHWC store of the tile's rows.
 template <int CO>
-__device__ __forceinline__ void ws_mma_role(int ntiles, int K4, int LBA, const float* a0, const float* b_hi, const float* b_lo, uint32_t tmem,
-                                            uint64_t* a_full, uint64_t* tmem_empty, uint64_t* mma_done) {
+__device__ __forceinline__ void ws_consumer_role(const DsLayerDev& L, int RH, int tpu, int ntiles, int K4, int LBA, const float* a0,
+                                                 const float* b_hi, const float* b_lo, const float* sc, const float* sf,
+                                                 float* __restrict__ out, uint64_t* a_full, uint64_t* mma_done, int wtid) {
+  static_assert(CO == 64, "one m64n64k8 per 64 accumulator rows");
   constexpr int LBB = CO * 4 + 4;
-  // instruction descriptor: D fp32 (bits 4-5 = 1), A and B TF32 (bits 7-9, 10-12 = 2), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-  constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(CO >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  const uint64_t db_hi = umma_desc(smem_u32(b_hi), LBB * 4u, 128u), db_lo = umma_desc(smem_u32(b_lo), LBB * 4u, 128u);
+  const uint64_t db_hi = gmma_desc(smem_u32(b_hi), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo), LBB * 4u, 128u);
   const int KS = K4 >> 1;
   int it = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
     const int b = it & 1, k = it >> 1;
     const float* a_hi = a0 + (size_t)b * 2 * K4 * LBA;
-    const uint64_t da_hi = umma_desc(smem_u32(a_hi), (uint32_t)LBA * 4u, 128u);
-    const uint64_t da_lo = umma_desc(smem_u32(a_hi + (size_t)K4 * LBA), (uint32_t)LBA * 4u, 128u);
+    const uint64_t da_hi = gmma_desc(smem_u32(a_hi), (uint32_t)LBA * 4u, 128u);
+    const uint64_t da_lo = gmma_desc(smem_u32(a_hi + (size_t)K4 * LBA), (uint32_t)LBA * 4u, 128u);
     mbar_wait(&a_full[b], (uint32_t)(k & 1));
-    if (it >= 2) mbar_wait(&tmem_empty[b], (uint32_t)((k - 1) & 1));              // the epilogue of tile it-2 has drained this accumulator
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tacc = tmem + (uint32_t)(b * CO);
+    float acc[2][CO / 2];
+#pragma unroll
+    for (int i = 0; i < CO / 2; ++i) { acc[0][i] = 0.f; acc[1][i] = 0.f; }
+    wgmma_fence();
 #pragma unroll
     for (int pass = 0; pass < 3; ++pass) {                       // lo*hi, hi*lo, hi*hi: the small terms first
       const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
 #pragma unroll 4
-      for (int ks = 0; ks < KS; ++ks) {                          // one MMA covers K = 8 = two 4-wide chunks
+      for (int ks = 0; ks < KS; ++ks) {                          // one k-step covers K = 8 = two 4-wide chunks
         const uint64_t da = da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db = db0 + (uint64_t)((2 * ks * LBB * 4) >> 4);
-        const uint32_t accumulate = (pass | ks) ? 1u : 0u;
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                     "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                     ::"r"(tacc), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
+        wgmma_m64n64k8_tf32(acc[0], da, db);
+        wgmma_m64n64k8_tf32(acc[1], da + (uint64_t)((64 * 16) >> 4), db);   // rows 64-127: eight 8-row groups further
       }
     }
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mma_done[b])) : "memory");
-  }
-}
-// Epilogue role, 4 warps: warp quarter q reads TMEM lanes [32 q, 32 q + 32) = accumulator rows, all CO columns in batches of 16,
-// applies the folded BatchNorm + ReLU and stores the NHWC row; then hands the accumulator back (tmem_empty).
-template <int CO>
-__device__ __forceinline__ void ws_epilogue_role(const DsLayerDev& L, int RH, int tpu, int ntiles, uint32_t tmem, const float* sc, const float* sf,
-                                                 float* __restrict__ out, uint64_t* mma_done, uint64_t* tmem_empty, int q, int lane) {
-  const int m = 32 * q + lane;
-  int it = 0;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-    const int b = it & 1, k = it >> 1;
-    mbar_wait(&mma_done[b], (uint32_t)(k & 1));
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    wgmma_commit();
+    wgmma_wait_all();
+    mbar_arrive(&mma_done[b]);                                   // the A buffer is free for the tile two ahead
     const int n = tile / tpu, h0 = (tile - n * tpu) * RH, npos = imin(RH, L.hout - h0) * L.wout;
-    const size_t gbase = ((size_t)n * L.hout + h0) * L.wout;
-    const uint32_t tacc = tmem + (uint32_t)(b * CO) + ((uint32_t)(32 * q) << 16);
-#pragma unroll
-    for (int c0 = 0; c0 < CO; c0 += 16) {
-      uint32_t r[16];
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                   : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                     "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                   : "r"(tacc + (uint32_t)c0));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (m < npos) {                                             // a lane owns a whole NHWC row: 32-byte stores (one full sector each)
-#pragma unroll
-        for (int j = 0; j < 16; j += 8) {
-          const int co = c0 + j;
-          const float4 s0 = ld4(sc + co), t0 = ld4(sf + co), s1 = ld4(sc + co + 4), t1 = ld4(sf + co + 4);
-          asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(out + (gbase + m) * CO + co),
-                       "f"(fmaxf(fmaf(__uint_as_float(r[j]), s0.x, t0.x), 0.f)), "f"(fmaxf(fmaf(__uint_as_float(r[j + 1]), s0.y, t0.y), 0.f)),
-                       "f"(fmaxf(fmaf(__uint_as_float(r[j + 2]), s0.z, t0.z), 0.f)), "f"(fmaxf(fmaf(__uint_as_float(r[j + 3]), s0.w, t0.w), 0.f)),
-                       "f"(fmaxf(fmaf(__uint_as_float(r[j + 4]), s1.x, t1.x), 0.f)), "f"(fmaxf(fmaf(__uint_as_float(r[j + 5]), s1.y, t1.y), 0.f)),
-                       "f"(fmaxf(fmaf(__uint_as_float(r[j + 6]), s1.z, t1.z), 0.f)), "f"(fmaxf(fmaf(__uint_as_float(r[j + 7]), s1.w, t1.w), 0.f))
-                       : "memory");
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    mbar_arrive(&tmem_empty[b]);
+    gmma_epilogue<2, CO / 8>(acc, 0, 0, CO, npos, sc, sf, out, ((size_t)n * L.hout + h0) * L.wout, wtid);
   }
 }
 
@@ -535,12 +491,10 @@ template <int C, int CO>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const __grid_constant__ CUtensorMap in_map, DsLayerDev L, int RH, int n_utt,
                                                                          const float* __restrict__ params, float* __restrict__ out, float eps) {
   TCR_DYNAMIC_SMEM(smem_raw);
-  __shared__ uint64_t in_full[2], a_full[2], mma_done[2], tmem_empty[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t in_full[2], a_full[2], mma_done[2];
   float* smem = reinterpret_cast<float*>(smem_raw);
-  constexpr int C4 = C / 4, KS = C / 8;
-  constexpr int TMEM_COLS = 2 * CO <= 32 ? 32 : (2 * CO <= 64 ? 64 : (2 * CO <= 128 ? 128 : 256));
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  constexpr int C4 = C / 4;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int hin_t = RH + 2, wp = L.wout + 2;
   constexpr int CH = C / 2, CH4 = CH / 4;                         // channels per TMA box: 32 fp32 = one 128-byte swizzle row
   static_assert(CH * 4 == 128, "the input halves are 128-byte rows (SWIZZLE_128B)");
@@ -562,13 +516,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
     for (int b = 0; b < 2; ++b) {
       mbar_init(&in_full[b], 1);
       mbar_init(&a_full[b], kWsProducers);
-      mbar_init(&mma_done[b], 1);
-      mbar_init(&tmem_empty[b], kWsFetchers);
+      mbar_init(&mma_done[b], kWsConsumers);
     }
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   for (int i0 = tid; i0 < C * CO; i0 += kTcThreads * 8) {
     float v[8];
@@ -591,10 +540,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
   for (int c = tid; c < CO; c += kTcThreads) fold_bn(params, L.pb, L.pbeta, L.pmm, L.pmv, c, eps, sc2, sf2);
   pdl_wait();
   fence_proxy_async();                                           // the B operand was written through the generic proxy
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base_s;
 
   if (warp < kWsProducerWarps) {
     // ---- input fetch (TMA) + depthwise 3x3 + folded BN + ReLU -> A operand ----
@@ -664,7 +610,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
           acc0 = acc1; acc1 = acc2; acc2 = make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
-      fence_proxy_async();                                       // operand stores -> visible to the async proxy (UMMA)
+      fence_proxy_async();                                       // operand stores -> visible to the async proxy (wgmma)
       mbar_arrive(&a_full[b]);
       const int nxt = tile + 2 * (int)gridDim.x;                  // refill this input buffer once every producer has left it
       if (nxt < ntiles) {
@@ -672,16 +618,9 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
         if (tid == 0) fetch_tile(nxt, xs, &in_full[b]);
       }
     }
-  } else if (warp == kWsProducerWarps) {
-    // ---- MMA issue: one thread ----
-    if (lane == 0) ws_mma_role<CO>(ntiles, C4, LBA, a0, b_hi, b_lo, tmem, a_full, tmem_empty, mma_done);
-  } else if (warp >= kTcThreads / 32 - 4) {
-    // ---- epilogue: 4 warps ----
-    ws_epilogue_role<CO>(L, RH, tpu, ntiles, tmem, sc2, sf2, out, mma_done, tmem_empty, warp & 3, lane);
+  } else if (warp >= kWsConsumerWarp0) {
+    ws_consumer_role<CO>(L, RH, tpu, ntiles, C4, LBA, a0, b_hi, b_lo, sc2, sf2, out, a_full, mma_done, tid - 32 * kWsConsumerWarp0);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
 }
 
 // First conv, warp-specialised (same roles and barriers as the block kernel): the producers copy the tile's input rows
@@ -691,11 +630,9 @@ template <int CO>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
                                                                       const float* __restrict__ in, float* __restrict__ out, float eps) {
   TCR_DYNAMIC_SMEM(smem_raw);
-  __shared__ uint64_t in_full[2], a_full[2], mma_done[2], tmem_empty[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t in_full[2], a_full[2], mma_done[2];
   float* smem = reinterpret_cast<float*>(smem_raw);
-  constexpr int TMEM_COLS = 2 * CO <= 32 ? 32 : (2 * CO <= 64 ? 64 : (2 * CO <= 128 ? 128 : 256));
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int K = L.kh * L.kw, K4 = K >> 2;
   const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
   const int XT = (hin_t * wp + 3) & ~3;
@@ -712,13 +649,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
     for (int b = 0; b < 2; ++b) {
       mbar_init(&in_full[b], kWsProducers);
       mbar_init(&a_full[b], kWsProducers);
-      mbar_init(&mma_done[b], 1);
-      mbar_init(&tmem_empty[b], kWsFetchers);
+      mbar_init(&mma_done[b], kWsConsumers);
     }
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
   }
   for (int i = tid; i < K * CO; i += kTcThreads) {                // filters w[k][co] -> B operand [n = co][k]
     const int k = i / CO, co = i - k * CO;
@@ -731,10 +663,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
   for (int c = tid; c < CO; c += kTcThreads) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc, sf);
   pdl_wait();
   fence_proxy_async();
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base_s;
 
   if (warp < kWsProducerWarps) {
     // the cells a thread copies and the (position, tap chunk) operands it gathers are the same for every tile: worked out once
@@ -809,28 +738,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
         cp_async_mbar_arrive(&in_full[b]);
       }
     }
-  } else if (warp == kWsProducerWarps) {
-    if (lane == 0) ws_mma_role<CO>(ntiles, K4, LBA, a0, b_hi, b_lo, tmem, a_full, tmem_empty, mma_done);
-  } else if (warp >= kTcThreads / 32 - 4) {
-    ws_epilogue_role<CO>(L, RH, tpu, ntiles, tmem, sc, sf, out, mma_done, tmem_empty, warp & 3, lane);
+  } else if (warp >= kWsConsumerWarp0) {
+    ws_consumer_role<CO>(L, RH, tpu, ntiles, K4, LBA, a0, b_hi, b_lo, sc, sf, out, a_full, mma_done, tid - 32 * kWsConsumerWarp0);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
 }
 
 // First layer (kh x kw conv from the single-channel feature map, audio_nets/ds_cnn.py:21 `conv_1`) as an implicit GEMM on
-// tcgen05: A[m][k] = x[oh*sh + k / kw, ow*sw + k % kw] is gathered from the staged input rows straight into the canonical
-// operand layout (hi / lo), B = the filter bank [co][k], K = kh * kw (40), same persistent / double-TMEM structure as above.
+// wgmma: A[m][k] = x[oh*sh + k / kw, ow*sw + k % kw] is gathered from the staged input rows straight into the canonical
+// operand layout (hi / lo), B = the filter bank [co][k], K = kh * kw (40), same persistent / quarter-per-warpgroup structure as
+// the lock-step block kernel above.
 template <int CO>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
                                                                       const float* __restrict__ in, float* __restrict__ out, float eps) {
+  static_assert(CO == 64, "one m64n32k8 quarter per warpgroup");
   TCR_DYNAMIC_SMEM(smem_raw);
-  __shared__ uint64_t mma_bar[2];
-  __shared__ uint32_t tmem_base_s;
   float* smem = reinterpret_cast<float*>(smem_raw);
-  constexpr int TMEM_COLS = 2 * CO <= 32 ? 32 : (2 * CO <= 64 ? 64 : (2 * CO <= 128 ? 128 : 256));
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int K = L.kh * L.kw, K4 = K >> 2, KS = K >> 3;
   const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
   const int XT = (hin_t * wp + 3) & ~3;
@@ -844,11 +767,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev
   float* sf = sc + CO;
   const int tpu = (L.hout + RH - 1) / RH;
   const int ntiles = tpu * n_utt;
-  if (tid == 0) { mbar_init(&mma_bar[0], 1); mbar_init(&mma_bar[1], 1); }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "n"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
   for (int i = tid; i < K * CO; i += kTcThreads) {                // filters w[k][co] -> B operand [n = co][k]
     const int k = i / CO, co = i - k * CO;
     const float x = __ldg(params + L.w + i);
@@ -896,54 +814,18 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev
     g_x23[j] = e[2] | (e[3] << 16);
     g_a[j] = ((kc * LBA + 4 * m) << 7) | m;
   }
-  auto epilogue = [&](uint32_t tacc, int tile_e) {
-    const int n = tile_e / tpu, h0 = (tile_e - n * tpu) * RH, npos = imin(RH, L.hout - h0) * L.wout;
-    constexpr int NG = kTcThreads / 128;
-    const int m = 32 * (warp & 3) + lane, cbase = (warp >> 2) * (CO / NG);
-    const size_t gbase = ((size_t)n * L.hout + h0) * L.wout;
-#pragma unroll
-    for (int c0 = 0; c0 < CO / NG; c0 += 16) {
-      uint32_t r[16];
-      const uint32_t taddr = tacc + ((uint32_t)(32 * (warp & 3)) << 16) + (uint32_t)(cbase + c0);
-      asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                   : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                     "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                   : "r"(taddr));
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (m < npos) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const int co = cbase + c0 + j;
-          const float4 s = ld4(sc + co), t = ld4(sf + co);
-          st4(out + (gbase + m) * CO + co,
-              make_float4(fmaxf(fmaf(__uint_as_float(r[j]), s.x, t.x), 0.f), fmaxf(fmaf(__uint_as_float(r[j + 1]), s.y, t.y), 0.f),
-                          fmaxf(fmaf(__uint_as_float(r[j + 2]), s.z, t.z), 0.f), fmaxf(fmaf(__uint_as_float(r[j + 3]), s.w, t.w), 0.f)));
-        }
-      }
-    }
-  };
-  int tile = blockIdx.x, cur = 0, it = 0, prev_tile = -1;
-  uint32_t parity[2] = {0u, 0u};
+  // this warpgroup's quarter of the accumulator
+  const int g = warp >> 2, m0 = 64 * (g & 1), col0 = (g >> 1) * (CO / 2);
+  const uint64_t da_hi = gmma_desc(smem_u32(a_hi + 4 * m0), LBA * 4u, 128u), da_lo = gmma_desc(smem_u32(a_lo + 4 * m0), LBA * 4u, 128u);
+  const uint64_t db_hi = gmma_desc(smem_u32(b_hi + 4 * col0), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo + 4 * col0), LBB * 4u, 128u);
+  int tile = blockIdx.x, cur = 0;
   if (tile < ntiles) fetch_tile(tile, xs0);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = tmem_base_s;
-  constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(CO >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-  const uint64_t da_hi = umma_desc(smem_u32(a_hi), LBA * 4u, 128u), da_lo = umma_desc(smem_u32(a_lo), LBA * 4u, 128u);
-  const uint64_t db_hi = umma_desc(smem_u32(b_hi), LBB * 4u, 128u), db_lo = umma_desc(smem_u32(b_lo), LBB * 4u, 128u);
-  for (; tile < ntiles; tile += gridDim.x, cur ^= 1, ++it) {
+  for (; tile < ntiles; tile += gridDim.x, cur ^= 1) {
     const int n = tile / tpu, h0 = (tile - n * tpu) * RH, rh = imin(RH, L.hout - h0);
-    (void)n;
     const float* xs = xs0 + cur * XT;
     asm volatile("cp.async.wait_all;" ::: "memory");
-    __syncthreads();
+    __syncthreads();                                             // rows landed; the previous tile's MMAs are done with A
     if (tile + (int)gridDim.x < ntiles) fetch_tile(tile + gridDim.x, xs0 + (cur ^ 1) * XT);
-    if (prev_tile >= 0) {
-      mbar_wait(&mma_bar[(it - 1) & 1], parity[(it - 1) & 1]);
-      parity[(it - 1) & 1] ^= 1u;
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
     // im2col gather: task = (position, 4-wide chunk of taps)
     const int npos = rh * L.wout;
 #pragma unroll
@@ -958,35 +840,20 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev
       }
     }
     fence_proxy_async();
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (tid == 0) {
-      const uint32_t tacc = tmem + (uint32_t)((it & 1) * CO);
-      for (int pass = 0; pass < 3; ++pass) {
-        const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
-        for (int ks = 0; ks < KS; ++ks) {
-          const uint64_t da = da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db = db0 + (uint64_t)((2 * ks * LBB * 4) >> 4);
-          const uint32_t accumulate = (pass | ks) ? 1u : 0u;
-          asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-                       "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                       ::"r"(tacc), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-        }
-      }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(&mma_bar[it & 1])) : "memory");
+    float acc[1][CO / 8 * 2];
+#pragma unroll
+    for (int i = 0; i < CO / 4; ++i) acc[0][i] = 0.f;
+    wgmma_fence();
+    for (int pass = 0; pass < 3; ++pass) {
+      const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
+      for (int ks = 0; ks < KS; ++ks)
+        wgmma_m64n32k8_tf32(acc[0], da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db0 + (uint64_t)((2 * ks * LBB * 4) >> 4));
     }
-    if (prev_tile >= 0) epilogue(tmem + (uint32_t)(((it - 1) & 1) * CO), prev_tile);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    prev_tile = tile;
+    wgmma_commit();
+    wgmma_wait_all();
+    gmma_epilogue<1, CO / 16>(acc, m0, col0, CO, npos, sc, sf, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
   }
-  if (prev_tile >= 0) {
-    mbar_wait(&mma_bar[(it - 1) & 1], parity[(it - 1) & 1]);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    epilogue(tmem + (uint32_t)(((it - 1) & 1) * CO), prev_tile);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  }
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TMEM_COLS));
 }
 #endif
 
@@ -1060,9 +927,9 @@ struct tcr_dscnn {
   int64_t n_params = 0, flops = 0;
   float* act[2] = {nullptr, nullptr};
   size_t act_floats = 0;
-  int sms = 148;
-  bool use_tc = true;        // pointwise convs on tcgen05 where they fit (env TCR_DSCNN_TC=0: register-tiled FMA everywhere)
-  bool tc_ws = true;         // warp-specialised tcgen05 block kernel (env TCR_DSCNN_TC=1: the lock-step version)
+  int sms = 1;
+  bool use_tc = true;        // pointwise convs on the tensor cores (wgmma) where they fit (env TCR_DSCNN_TC=0: register-tiled FMA everywhere)
+  bool tc_ws = true;         // warp-specialised wgmma block kernel (env TCR_DSCNN_TC=1: the lock-step version)
 #ifndef TCR_EMU
   struct InMap { CUtensorMap map; const void* ptr = nullptr; int rh = 0; };
   std::vector<InMap> in_maps;   // per layer: TMA descriptor of the block's input activations (re-encoded if the buffer changes)
@@ -1231,7 +1098,7 @@ extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const floa
       RHt = std::max(1, RHt);
       RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);
       const int K4 = L.kh * L.kw / 4, hin_t = (RHt - 1) * L.sh + L.kh, wpt = (L.wout - 1) * L.sw + L.kw;
-      // implicit GEMM on tcgen05 (3xTF32); the limits are the kernel's precomputed per-thread walks (4 cells, 4 gather tasks)
+      // implicit GEMM on wgmma (3xTF32); the limits are the kernel's precomputed per-thread walks (4 cells, 4 gather tasks)
       if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && hin_t * wpt <= 4 * kTcThreads &&
           128 * K4 <= 4 * kTcThreads && hin_t < 512) {
         const size_t smem_cws = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 4 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
@@ -1271,7 +1138,7 @@ extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const floa
                         2 * L.cin + 2 * L.cout) * 4;
       };
 #ifndef TCR_EMU
-      // pointwise conv on the tensor cores (tcgen05, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
+      // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
       if (d->use_tc && L.cin == 64 && L.cout == 64 && L.kh == 3 && L.kw == 3 && L.sh == 1 && L.sw == 1 && L.wout <= 64) {
         int RHt = std::min(L.hout, 128 / L.wout);
         RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);     // balanced: 25 rows -> 5 tiles of 5

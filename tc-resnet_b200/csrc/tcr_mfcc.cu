@@ -1,4 +1,4 @@
-// tcr_mfcc.cu — fused MFCC / log-mel front-end for sm_100a.
+// tcr_mfcc.cu — fused MFCC / log-mel front-end for sm_90a.
 //
 // Replaces the TF graph built by datasets/preprocessors.py:64-96 (_log_mel_spectrogram:
 // stft -> power|magnitude -> mel matmul -> log(x + 1e-6)) and :183-194 (MFCC: DCT-II, first

@@ -1,4 +1,4 @@
-// tcr_net_bwd.cu — TC-ResNet backward kernels for sm_100a (fp32 FMA pipe).
+// tcr_net_bwd.cu — TC-ResNet backward kernels for sm_90a (fp32 FMA pipe).
 //
 // Replaces the gradient graph slim.learning.create_train_op builds (helper/trainer.py:199-211):
 // Conv2DBackpropInput / Conv2DBackpropFilter / FusedBatchNormGrad / ReluGrad per layer.
@@ -478,9 +478,9 @@ static size_t bwd_data_smem(const ConvPlan& cv, const ConvPlan* dn, int U, int K
   return f * 4;
 }
 
-double tile_cost(int n, int U, int occ, bool wsm);     // tcr_net_fwd.cu
+double tile_cost(int sms, int n, int U, int occ, bool wsm);     // tcr_net_fwd.cu
 
-static void pick_bwd_tile(const ConvPlan& cv, const ConvPlan* dn, int n, int* U_out, int* KS_out, int* wsm_out) {
+static void pick_bwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n, int* U_out, int* KS_out, int* wsm_out) {
   const size_t wbytes = ((size_t)cv.wnumel() + (dn ? (size_t)dn->wnumel() : 0)) * 4;
   const int S = cv.stride, NT0 = (cv.k + S - 1) / S;
   double best = 1e30;
@@ -490,7 +490,7 @@ static void pick_bwd_tile(const ConvPlan& cv, const ConvPlan* dn, int n, int* U_
     const int occ = (pass & 1) ? 1 : 2;
     const size_t budget = occ == 2 ? kSmemBudget : kSmemMax;
     if (wsm && wbytes + 16 * 1024 > budget) continue;
-    for (int U = std::min(16, std::max(1, (n + 148 * occ - 1) / (148 * occ))); U >= 1; --U) {
+    for (int U = std::min(16, std::max(1, (n + sms * occ - 1) / (sms * occ))); U >= 1; --U) {
       int best_ks = 0;
       double best_cost = 1e30;
       for (int KS = 1; KS <= NT0; ++KS) {
@@ -505,7 +505,7 @@ static void pick_bwd_tile(const ConvPlan& cv, const ConvPlan* dn, int n, int* U_
         }
       }
       if (!best_ks) continue;
-      const double c = tile_cost(n, U, occ, wsm);
+      const double c = tile_cost(sms, n, U, occ, wsm);
       if (c < best - 1e-9) { best = c; *U_out = U; *KS_out = best_ks; *wsm_out = wsm ? 1 : 0; }
       break;
     }
@@ -526,16 +526,16 @@ static size_t bwd_weight_smem(const ConvPlan& cv, int cot, int RG, int UB) {
 // few waves of CTAs.
 void plan_bwd_weight(tcr_handle* h) {
   // Per layer: the LARGEST output-channel tile that fits 256 threads (tiny tiles re-stage the same x tile many times) and at
-  // most 4 row groups.  Row chunks: ONE wave of CTAs (148 SMs x 2) with equal predicted duration.  tools/timeline.py on
-  // TCResNet8 (N=512) gives the time of a CTA as ~ utterances x (0.9 + MACs per utterance and tile / 70e3) in us: the K=1
-  // shortcut convs are staging-bound, the others FMA-bound at ~40 % of peak.  With chunks of equal MACs the launch took 51 us
-  // (long conv0 chunks, late second wave); balanced it is bounded by sum(tau_l x tiles_l) x N / 296.
+  // most 4 row groups.  Row chunks: ONE wave of CTAs (SMs x 2) with equal predicted duration.  The time of a CTA is modelled
+  // as ~ utterances x (0.9 + MACs per utterance and tile / 70e3): the K=1 shortcut convs are staging-bound, the others
+  // FMA-bound.  Chunks of equal MACs would leave long conv0 chunks and a late second wave; balanced, the launch is bounded by
+  // sum(tau_l x tiles_l) x N / (2 x SMs).
   struct L { ConvPlan* cv; int cot, ncot; double tau; };
   std::vector<L> ls;
   for (auto& cv : h->convs) {
     // output-channel tile: the LARGEST that fits 256 threads (a thread owns 2 ci x 4 co x K taps).  A smaller tile with more row
     // groups keeps more threads busy (75-84 % instead of 56-63 % on 48- and 36-channel layers) but re-stages the x tile per
-    // tile and measured slower: TCResNet8 52 -> 62 us, TCResNet14-1.5 384 -> 421 us.
+    // tile and is slower on TCResNet8 and TCResNet14-1.5.
     int cot = 4;
     for (int c = 4; c <= cv.cout; c += 4)
       if (cv.cout % c == 0 && (cv.cin / 2) * (c / 4) <= kDwThreads) cot = c;
@@ -543,7 +543,7 @@ void plan_bwd_weight(tcr_handle* h) {
     ls.push_back(L{&cv, cot, cv.cout / cot, 0.9 + macs / 70e3});
   }
   const int n = h->cfg.max_batch;
-  int slots = 2 * 148, upc_cap = 256;
+  int slots = 2 * h->sms, upc_cap = 256;
   if (const char* e = getenv("TCR_DW_SLOTS")) slots = atoi(e);              // tuning knobs (tools/sweep_dw.sh)
   if (const char* e = getenv("TCR_DW_UPC")) upc_cap = atoi(e);
   auto ctas_at = [&](double D) {
@@ -635,7 +635,7 @@ static DySrc make_dy(const tcr_handle* h, const ConvPlan& cv, const float* dz, i
 // *gc_out: per-cluster records of BatchNorm-backward sums this launch leaves for the layer(s) below (0 when recording)
 static int bwd_data(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, BwdDataArgs a, const float* params, int n, cudaStream_t s, int* gc_out) {
   int U, KS, wsm;
-  pick_bwd_tile(cv, dn, n, &U, &KS, &wsm);
+  pick_bwd_tile(h->sms, cv, dn, n, &U, &KS, &wsm);
   a.n = n; a.U = U; a.w_smem = wsm;
   (void)params;
   a.w = cv.wT; a.cin = cv.cin; a.cout = cv.cout; a.k = cv.k; a.stride = cv.stride;

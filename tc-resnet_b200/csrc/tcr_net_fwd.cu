@@ -1,4 +1,4 @@
-// tcr_net_fwd.cu — TC-ResNet forward kernels for sm_100a (fp32 CUDA-core FMA; see DESIGN.md for why the
+// tcr_net_fwd.cu — TC-ResNet forward kernels for sm_90a (fp32 CUDA-core FMA; see DESIGN.md for why the
 // 9x1 temporal convolutions stay on the FMA pipe: TF32/BF16 tensor-core products break the 1e-4 logit bound).
 //
 // Replaces tc_resnet() (audio_nets/tc_resnet.py:6-54) under TCResNet_arg_scope (:102-123):
@@ -503,24 +503,23 @@ static size_t fwd_smem_bytes(const ConvPlan& cv, const ConvPlan* dn, int U, int 
 }
 
 // Utterances per CTA, k-slices and whether the filter bank is staged in shared memory.
-// Goals: >= 2 resident CTAs per SM when the batch allows (latency hiding), all 148 SMs busy, balanced thread tasks.
+// Goals: >= 2 resident CTAs per SM when the batch allows (latency hiding), all SMs busy, balanced thread tasks.
 static constexpr size_t kSmemMax = 200 * 1024;      // opt-in limit we are willing to use for one CTA
 
 // Candidate tilings are compared by a small cost model: waves x (U x (co-residency slowdown) + fixed part), where a wave is one
-// round of CTAs over the 148 SMs at the residency the shared-memory footprint allows.  (Measured on TCResNet14-1.5, N=1024: a tile
-// that fits only one CTA per SM must cover the batch in ONE wave of <= 148 CTAs; two waves of 128 cost 2x the fixed part.)
-static constexpr int kSMs = 148;
-double tile_cost(int n, int U, int occ, bool wsm) {
+// round of CTAs over the device's `sms` SMs at the residency the shared-memory footprint allows: a tile that fits only one CTA
+// per SM should cover the batch in ONE wave of <= sms CTAs, since every further wave pays the fixed part again.
+double tile_cost(int sms, int n, int U, int occ, bool wsm) {
   const int groups = (n + U - 1) / U;
-  const int waves = (groups + kSMs * occ - 1) / (kSMs * occ);
-  // unit = FMA time of one utterance on an otherwise idle SM.  Measured on TCResNet14-1.5 (profiles/r01_v11_*): a lone 8-warp CTA
-  // per SM cannot hide its latencies (76-89 us at 152 CTAs vs 47-54 us at 256 CTAs, two per SM), and reading the filter bank
-  // through L1/L2 costs about the same as staging it in shared memory (48 us), so residency decides, not the filter path.
-  // The per-wave fixed part (launch, filter TMA, staging latency, statistics, cluster publish) is ~4 such units.
+  const int waves = (groups + sms * occ - 1) / (sms * occ);
+  // unit = FMA time of one utterance on an otherwise idle SM.  A lone 8-warp CTA per SM cannot hide its latencies as well as
+  // two per SM, and reading the filter bank through L1/L2 costs about the same as staging it in shared memory, so residency
+  // decides, not the filter path.  The per-wave fixed part (launch, filter TMA, staging latency, statistics, cluster publish)
+  // is ~4 such units.
   return waves * (U * (occ == 2 ? 1.7 : 1.8) * (wsm ? 1.0 : 1.1) + 4.0);
 }
 
-static void pick_fwd_tile(const ConvPlan& cv, const ConvPlan* dn, int n, int* U_out, int* KS_out, int* wsm_out) {
+static void pick_fwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n, int* U_out, int* KS_out, int* wsm_out) {
   const size_t wbytes = fwd_weight_floats(cv, dn) * 4;
   double best = 1e30;
   *U_out = 1; *KS_out = 1; *wsm_out = 0;
@@ -530,7 +529,7 @@ static void pick_fwd_tile(const ConvPlan& cv, const ConvPlan* dn, int n, int* U_
     const int occ = (pass & 1) ? 1 : 2;
     const size_t budget = occ == 2 ? kSmemBudget : kSmemMax;
     if (wsm && wbytes + 16 * 1024 > budget) continue;
-    for (int U = std::min(16, std::max(1, (n + kSMs * occ - 1) / (kSMs * occ))); U >= 1; --U) {
+    for (int U = std::min(16, std::max(1, (n + sms * occ - 1) / (sms * occ))); U >= 1; --U) {
       int best_ks = 0;
       double best_cost = 1e30;
       for (int KS = 1; KS <= cv.k; ++KS) {
@@ -544,7 +543,7 @@ static void pick_fwd_tile(const ConvPlan& cv, const ConvPlan* dn, int n, int* U_
         }
       }
       if (!best_ks) continue;
-      const double c = tile_cost(n, U, occ, wsm);
+      const double c = tile_cost(sms, n, U, occ, wsm);
       if (c < best - 1e-9) { best = c; *U_out = U; *KS_out = best_ks; *wsm_out = wsm ? 1 : 0; }
       break;                        // the largest U that fits is the candidate of this pass
     }
@@ -671,7 +670,7 @@ static int launch_conv_fwd(const char* name, const FwdArgs& a, int groups, size_
 static int conv_fwd(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, FwdArgs a, const float* params, int n, bool training,
                     cudaStream_t s) {
   int U, KS, wsm;
-  pick_fwd_tile(cv, dn, n, &U, &KS, &wsm);
+  pick_fwd_tile(h->sms, cv, dn, n, &U, &KS, &wsm);
   a.n = n; a.U = U; a.t_in = cv.t_in; a.cin = cv.cin; a.w_smem = wsm;
   a.w = params + cv.w_off; a.y = cv.y; a.fpart = cv.fpart;
   a.cout = cv.cout; a.stride = cv.stride; a.t_out = cv.t_out; a.pad_left = cv.pad_left; a.KS = KS;

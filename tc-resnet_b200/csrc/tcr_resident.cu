@@ -5,8 +5,7 @@
 // Why: BatchNorm's batch statistics force a grid-wide dependency after every conv layer, forward and backward
 // (audio_nets/tc_resnet.py:21-41 under TCResNet_arg_scope :102-123; FusedBatchNormGrad in the gradient graph of
 // helper/trainer.py:199-211).  As separate launches each layer paid a kernel boundary (~4.5 us), re-staged its tiles from L2 and
-// re-fetched its code: profiles/r02_v0_*: 14 conv launches + head at 16-23 us for 1-2 us of math each, top stalls `no_instruction`
-// and `barrier`, warps_active 22 %.  Here:
+// re-fetched its code: 14 conv launches + head, each far longer than its math, stalled on instruction fetch and barriers.  Here:
 //   * one CTA of 512 threads per SM owns ceil(n / #SMs) whole utterances for the whole pass; a layer's output stays in shared
 //     memory and becomes the next layer's input tile by one smem -> smem pass (BatchNorm + ReLU (+ residual) applied there);
 //   * batch statistics travel as per-CTA records through L2 behind a split grid barrier: a CTA arrives as soon as its record is
@@ -1230,8 +1229,8 @@ static ResidentState* resident_state(tcr_handle* h) {
   if (h->resident) return (ResidentState*)h->resident;
   ResidentState* S = new ResidentState();
   h->resident = S;
-  // default 3.  Measured on B200, TCResNet8-1.0, N=512 (DESIGN.md section 6): mode 1 0.366 ms/step, mode 3 0.356 ms, mode 2 ~0.39 ms:
-  // the weight-gradient FMA loops of mode 2 run 16 warps per SM where the grouped launch runs two CTAs per SM and loses to it.
+  // default 3: the weight-gradient FMA loops of mode 2 run 16 warps per SM where the grouped launch runs two CTAs per SM, and
+  // mode 2 loses to it; mode 3 is ahead of mode 1 by the backward-data launches it saves.
   int want = 3;
   if (const char* e = getenv("TCR_RESIDENT")) want = atoi(e);
   if (h->sync_bn) want = 0;          // SyncBN lives in the per-layer kernels' launch sequence (NCCL between launches)

@@ -215,7 +215,7 @@ class TrainerBase:
         g.set_defaults(relative=True, boundaries_epoch=True)
         g.add_argument("--checkpoint_format", default="tf", choices=["tf", "npz"],
                        help="tf: tensor-bundle files like tf.train.Saver (<Model>-<step>.index/.data-*); npz: one NumPy archive")
-        g = parser.add_argument_group("B200 data-parallel (no reference counterpart)")
+        g = parser.add_argument_group("Multi-GPU data-parallel (no reference counterpart)")
         g.add_argument("--data_parallel", action="store_true",
                        help="one process per GPU under torchrun; gradients are averaged with one NCCL all-reduce per step")
 

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """`python train_audio.py <reference flags> <ModelName> <model flags>` — same command lines as the reference's
 train_audio.py (e.g. scripts/commands/TCResNet8Model-1.0_mfcc_40_3010_0.001_mom_l1.sh line 3), executing on the
-B200 CUDA path.  The model is an argparse sub-command placed last; it is looked up by name in factory.audio_nets."""
+H100 CUDA path.  The model is an argparse sub-command placed last; it is looked up by name in factory.audio_nets."""
 from __future__ import annotations
 
 import argparse

@@ -5,8 +5,10 @@ these are OUR pins (regression anchors for the oracle and the CUDA path), not th
 Re-generate with:  python tests/golden/make_golden.py
 Inputs are re-created from seeds (SURVEY.md 8d), so the files hold outputs only.
 """
+import io
 import os
 import sys
+import zipfile
 
 import numpy as np
 
@@ -20,6 +22,29 @@ CASES = {
     "r8_T49": dict(model="TCResNet8", wm=1.0, window=640, stride=320, n=4),
     "r14_T98": dict(model="TCResNet14", wm=1.0, window=480, stride=160, n=3),
 }
+
+
+def save(path, out):
+    """Writes `out` as an .npz with LZMA-compressed members.  1-D float32 arrays are stored as their four byte planes
+    (uint8 [4, n]): the sign / exponent bytes then compress well, which keeps every fixture under 1 MB."""
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_LZMA) as z:
+        for k, v in out.items():
+            v = np.asarray(v)
+            if v.dtype == np.float32 and v.ndim == 1:
+                v = v.view(np.uint8).reshape(-1, 4).T.copy()
+            buf = io.BytesIO()
+            np.lib.format.write_array(buf, v)
+            z.writestr(k + ".npy", buf.getvalue())
+
+
+def load(path):
+    """Inverse of save() (a plain np.savez file reads the same way): a dict of the stored arrays."""
+    gold = np.load(path)
+    out = {}
+    for k in gold.files:
+        v = gold[k]
+        out[k] = v.T.copy().view(np.float32).ravel() if v.dtype == np.uint8 else v
+    return out
 
 
 def compute(case):
@@ -43,5 +68,5 @@ if __name__ == "__main__":
     here = os.path.dirname(os.path.abspath(__file__))
     for name, case in CASES.items():
         _, out = compute(case)
-        np.savez_compressed(os.path.join(here, name + ".npz"), **out)
+        save(os.path.join(here, name + ".npz"), out)
         print(name, {k: getattr(v, "shape", ()) for k, v in out.items()})

@@ -1,5 +1,5 @@
 """Device input stage (tcr_augment_pcm16) vs the NumPy restatement of datasets/augmentation_factory.py: bit-exact for the same
-random draws.  Kernel logic on the CPU emulator here, the sm_100a build under -m gpu."""
+random draws.  Kernel logic on the CPU emulator here, the sm_90a build under -m gpu."""
 import numpy as np
 import pytest
 

@@ -26,7 +26,7 @@ def test_gradient_exchange_matches_oracle(exchange, env):
     one node) and the ncclAllReduce fallback; 4 steps, averaged gradient vs the oracle's shard-wise mean, identical replicas."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     r = _torchrun("nccl", min(torch.cuda.device_count(), 8), 29612 if exchange == "nccl" else 29613, env)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
     assert "replicas bit-identical" in r.stdout and f"exchange={exchange}" in r.stdout, r.stdout[-500:]
@@ -38,7 +38,7 @@ def test_sync_bn_flag_equals_single_device_global_batch():
     step equals the oracle's single-device step on the concatenated global batch."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     r = _torchrun("syncbn", 2, 29614)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-4000:]
     assert "syncbn world=2" in r.stdout, r.stdout[-500:]
@@ -51,7 +51,7 @@ def test_trainer_data_parallel_two_ranks_checkpoints(tmp_path):
     loop at the same global step, and the checkpoint loads."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs >= 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs >= 2 GPUs")
     root = os.path.dirname(HERE)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1",
            "--master-port", "29615", os.path.join(root, "tc-resnet_b200", "train_audio.py"),

@@ -89,10 +89,10 @@ def test_cuda_dscnn_matches_oracle(size, h, w, n):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", ["0", "1"], ids=["fp32-fma", "tcgen05-lockstep"])
+@pytest.mark.parametrize("mode", ["0", "1"], ids=["fp32-fma", "wgmma-lockstep"])
 def test_cuda_dscnn_other_kernel_paths(mode, monkeypatch):
-    """TCR_DSCNN_TC picks the kernels when the net is created: 0 = register-tiled fp32 FMA, 1 = the lock-step tcgen05 kernels,
-    default = the warp-specialised tcgen05 kernels (TMA input tiles).  Every path meets the same bound."""
+    """TCR_DSCNN_TC picks the kernels when the net is created: 0 = register-tiled fp32 FMA, 1 = the lock-step wgmma kernels,
+    default = the warp-specialised wgmma kernels (TMA input tiles).  Every path meets the same bound."""
     from tcr_harness import TorchBackend
     monkeypatch.setenv("TCR_DSCNN_TC", mode)
     assert _run(TorchBackend(), "S", 49, 40, 150) < 1e-5

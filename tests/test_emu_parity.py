@@ -1,6 +1,6 @@
 """Kernel LOGIC parity on a CPU box: the product kernel sources compiled against the test-only fiber
 emulator (tests/emu) and driven through the same C ABI, compared with the fp64 oracle.  Sizes are tiny; the real
-parity tests are the -m gpu ones (tests/test_gpu_parity.py) that run the sm_100a build."""
+parity tests are the -m gpu ones (tests/test_gpu_parity.py) that run the sm_90a build."""
 import numpy as np
 import pytest
 

@@ -1,4 +1,4 @@
-"""Parity tests proper: the sm_100a CUDA path through the C ABI vs the fp64 oracle, on a real B200."""
+"""Parity tests proper: the sm_90a CUDA path through the C ABI vs the fp64 oracle, on a real H100."""
 import numpy as np
 import pytest
 

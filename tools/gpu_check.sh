@@ -22,7 +22,7 @@ print(run_case(b, model='TCResNet8', wm=1.0, n=9, keep=0.5))
 " > gpurun_out/sanitizer.txt 2>&1 ; echo "sanitizer rc=$?" | tee -a gpurun_out/sanitizer.txt
   tail -5 gpurun_out/sanitizer.txt
   # shared-memory races and divergent barriers: one TC-ResNet step (default kernels), one with the resident backward kernel, and
-  # the DS-CNN forward (mbarrier / TMA / tcgen05 pipeline); racecheck serialises heavily, so the cases are tiny
+  # the DS-CNN forward (mbarrier / TMA / wgmma pipeline); racecheck serialises heavily, so the cases are tiny
   for tool in racecheck synccheck; do
     echo "== compute-sanitizer --tool $tool"
     TCR_RESIDENT=2 timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python -c "

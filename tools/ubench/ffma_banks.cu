@@ -1,5 +1,5 @@
 // Micro-benchmark: throughput of the 4x4 outer-product FFMA block (shared-memory operands) with float4 vs scalar accumulators.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o ffma_banks ffma_banks.cu ; run on the GPU box.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o ffma_banks ffma_banks.cu ; run on the GPU box.
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
@@ -62,18 +62,18 @@ extern "C" __global__ void __launch_bounds__(512,1) varP(int rows, float* out) {
   out[(size_t)blockIdx.x*512+threadIdx.x]=s;
 }
 int main() {
-  float* out; cudaMalloc(&out, 148ull*512*48*4);
+  float* out; cudaMalloc(&out, 132ull*512*48*4);
   cudaFuncSetAttribute(varA, cudaFuncAttributeMaxDynamicSharedMemorySize, 40000);
   cudaFuncSetAttribute(varB, cudaFuncAttributeMaxDynamicSharedMemorySize, 40000);
   cudaEvent_t e0,e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
   const int rows=4096;
   for (int rep=0; rep<3; ++rep) {
     float ms;
-    cudaEventRecord(e0); varA<<<148,512,40000>>>(rows,52,52,out); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms,e0,e1);
+    cudaEventRecord(e0); varA<<<132,512,40000>>>(rows,52,52,out); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms,e0,e1);
     printf("varA float4 acc : %.3f ms  -> %.2f cycles/FFMA/SMSP (at 1.965 GHz)\n", ms, ms*1e-3*1.965e9/(rows*48.0*4));
-    cudaEventRecord(e0); varB<<<148,512,40000>>>(rows,52,52,out); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms,e0,e1);
+    cudaEventRecord(e0); varB<<<132,512,40000>>>(rows,52,52,out); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms,e0,e1);
     printf("varB scalar acc : %.3f ms  -> %.2f cycles/FFMA/SMSP\n", ms, ms*1e-3*1.965e9/(rows*48.0*4));
-    cudaEventRecord(e0); varP<<<148,512>>>(rows,out); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms,e0,e1);
+    cudaEventRecord(e0); varP<<<132,512>>>(rows,out); cudaEventRecord(e1); cudaEventSynchronize(e1); cudaEventElapsedTime(&ms,e0,e1);
     printf("varP reg chains : %.3f ms  -> %.2f cycles/FFMA/SMSP\n", ms, ms*1e-3*1.965e9/(rows*48.0*4));
   }
   printf("err %s\n", cudaGetErrorString(cudaGetLastError()));
