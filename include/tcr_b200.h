@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 5
+#define TCR_ABI_VERSION 6
 
 enum {
   TCR_OK = 0,
@@ -277,6 +277,10 @@ int tcr_dscnn_param_table(const tcr_dscnn* d, const tcr_param_desc** descs, int3
                           int64_t* forward_flops_per_utt);
 int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const float* params, int32_t n, float* logits, float* probs,
                       tcr_stream stream);
+/* Layers [0, num_layers) of the same forward pass, with the same kernels: the NHWC output [n, hout, wout, cout] of layer
+ * num_layers - 1 is written to act_out and nothing else is (for checking one layer at a time against a reference). */
+int tcr_dscnn_forward_partial(tcr_dscnn* d, const float* features, const float* params, int32_t n, int32_t num_layers,
+                              float* act_out, tcr_stream stream);
 
 /* Process-wide launch accounting (no reference counterpart; the reference only logs wall-clock per
  * session.run, helper/trainer.py:312-321).  tcr_launch_count: kernels launched by this library so far.

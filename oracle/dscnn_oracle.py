@@ -122,21 +122,39 @@ def _depthwise(x, w, stride):
     return out
 
 
+def layer(spec: DsSpec, p, l, x):
+    """Layer l of the net (conv + BN + ReLU, or depthwise + BN + ReLU + pointwise + BN + ReLU): x [N, H, W, Cin] NHWC
+    (layer 0 also takes the features [N, H, W]) -> [N, Hout, Wout, Cout]."""
+    typ, _, _, stride, scope = NET_DEFS[spec.size][l]
+    s = f"DSCNN/{scope}"
+    if x.ndim == 3:
+        x = x[..., None]
+    if typ == "conv":
+        x = _conv2d(x, p[s + "/weights"], stride) + p[s + "/biases"]
+        return _bn_relu(x, p, s + "/batch_norm")
+    x = _depthwise(x, p[s + "/depthwise_conv/depthwise_weights"], stride) + p[s + "/depthwise_conv/biases"]
+    x = _bn_relu(x, p, s + "/dw_batch_norm")
+    x = _conv2d(x, p[s + "/pointwise_conv/weights"], (1, 1)) + p[s + "/pointwise_conv/biases"]
+    return _bn_relu(x, p, s + "/pw_batch_norm")
+
+
+def forward_layers(spec: DsSpec, p, feat):
+    """feat [N, H, W] -> [output of layer 0, ..., output of the last layer], each NHWC."""
+    acts, x = [], feat
+    for l in range(len(NET_DEFS[spec.size])):
+        x = layer(spec, p, l, x)
+        acts.append(x)
+    return acts
+
+
+def head(spec: DsSpec, p, x):
+    """Global average pool + fully connected: [N, H, W, C] -> logits [N, classes]."""
+    return x.mean(axis=(1, 2)) @ p["DSCNN/fc1/weights"] + p["DSCNN/fc1/biases"]
+
+
 def forward(spec: DsSpec, p, feat):
     """feat [N, H, W] -> logits [N, classes] (DSCNN(), ds_cnn.py:89-101, is_training=False)."""
-    x = feat[..., None]
-    for typ, depth, k, stride, scope in NET_DEFS[spec.size]:
-        s = f"DSCNN/{scope}"
-        if typ == "conv":
-            x = _conv2d(x, p[s + "/weights"], stride) + p[s + "/biases"]
-            x = _bn_relu(x, p, s + "/batch_norm")
-        else:
-            x = _depthwise(x, p[s + "/depthwise_conv/depthwise_weights"], stride) + p[s + "/depthwise_conv/biases"]
-            x = _bn_relu(x, p, s + "/dw_batch_norm")
-            x = _conv2d(x, p[s + "/pointwise_conv/weights"], (1, 1)) + p[s + "/pointwise_conv/biases"]
-            x = _bn_relu(x, p, s + "/pw_batch_norm")
-    pooled = x.mean(axis=(1, 2))
-    return pooled @ p["DSCNN/fc1/weights"] + p["DSCNN/fc1/biases"]
+    return head(spec, p, forward_layers(spec, p, feat)[-1])
 
 
 def forward_flops(spec: DsSpec) -> int:

@@ -1080,127 +1080,145 @@ extern "C" int tcr_dscnn_param_table(const tcr_dscnn* d, const tcr_param_desc** 
   return TCR_OK;
 }
 
+// Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC).  The kernel is chosen here, once for both entry
+// points: wgmma where the layer's shape fits the tensor-core kernels (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.
+// The warp-specialised block kernel reads its input through a TMA map over max_batch utterances, so only from an activation
+// buffer of the handle.
+static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s) {
+  const DsLayerDev& L = d->net.layer[l];
+  const float eps = 1e-3f;
+  if (L.type == 0) {
+#ifndef TCR_EMU
+    int RHt = std::min(L.hout, 128 / std::max(1, std::min(L.wout, 128)));
+    RHt = std::max(1, RHt);
+    RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);
+    const int K4 = L.kh * L.kw / 4, hin_t = (RHt - 1) * L.sh + L.kh, wpt = (L.wout - 1) * L.sw + L.kw;
+    // implicit GEMM on wgmma (3xTF32); the limits are the kernel's precomputed per-thread walks (4 cells, 4 gather tasks)
+    if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && hin_t * wpt <= 4 * kTcThreads &&
+        128 * K4 <= 4 * kTcThreads && hin_t < 512) {
+      const size_t smem_cws = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 4 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
+      if (d->tc_ws && smem_cws <= 220 * 1024 && hin_t * wpt <= 4 * kWsProducers && 128 * K4 <= 4 * kWsProducers && (K4 & 1) == 0) {
+        auto kws = dscnn_conv_ws_kernel<64>;
+        static SmemOptIn optin_cws;
+        if (optin_cws.ensure(kws, smem_cws) != cudaSuccess) return TCR_ERR_CUDA;
+        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
+        TCR_LAUNCH("dscnn_conv_ws", kws, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_cws, s, L, RHt, n, params, in, out, eps);
+        return TCR_OK;
+      }
+      const size_t smem_tc = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 2 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
+      auto ktc = dscnn_conv_tc_kernel<64>;
+      static SmemOptIn optin_tc;
+      if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
+      const int tiles = ((L.hout + RHt - 1) / RHt) * n;
+      TCR_LAUNCH("dscnn_conv_tc", ktc, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
+      return TCR_OK;
+    }
+#endif
+    const int hp = (L.hout - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
+    const size_t smem = (size_t)(((hp * wp + 3) & ~3) + L.kh * L.kw * L.cout + 2 * L.cout) * 4;
+    auto kfn = dscnn_conv_kernel;
+#ifndef TCR_EMU
+    static SmemOptIn optin;
+    if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
+#endif
+    TCR_LAUNCH("dscnn_conv", kfn, dim3(n), dim3(256), smem, s, L, params, in, out, eps);
+  } else {
+    auto smem_for = [&](int RH, int COT) {
+      const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
+      return (size_t)((size_t)hin_t * wp * L.cin + (size_t)RH * L.wout * L.cin + (size_t)L.cin * COT + L.kh * L.kw * L.cin +
+                      2 * L.cin + 2 * L.cout) * 4;
+    };
+#ifndef TCR_EMU
+    // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
+    if (d->use_tc && L.cin == 64 && L.cout == 64 && L.kh == 3 && L.kw == 3 && L.sh == 1 && L.sw == 1 && L.wout <= 64) {
+      int RHt = std::min(L.hout, 128 / L.wout);
+      RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);     // balanced: 25 rows -> 5 tiles of 5
+      const int C4 = L.cin / 4;
+      const bool walk_ok = (RHt + 2) * (L.wout + 2) <= 8 * (kTcThreads / C4);      // the kernel's precomputed fetch walk: 8 cells
+      const size_t smem_tc = (2 * (size_t)C4 * ((RHt + 2) * (L.wout + 2) * 4 + 4) + 2 * (size_t)C4 * (128 * 4 + 4) + 2 * (size_t)C4 * (L.cout * 4 + 4) +
+                              (size_t)9 * L.cin + 2 * L.cin + 2 * L.cout) * 4;
+      const int lba = ((RHt * L.wout + 7) & ~7) * 4 + 4;
+      const size_t xh = (((size_t)(RHt + 2) * (L.wout + 2) * 128 + 1023) & ~(size_t)1023) / 4;       // floats per half input tile
+      const size_t smem_ws = (4 * xh + 4 * (size_t)C4 * lba + 2 * (size_t)C4 * (L.cout * 4 + 4) + (size_t)9 * L.cin + 2 * L.cin + 2 * L.cout) * 4;
+      if (d->tc_ws && smem_ws <= 226 * 1024 && C4 * L.wout <= kWsProducers && L.wout + 2 <= 256 && RHt + 2 <= 256 && (in == d->act[0] || in == d->act[1])) {
+        auto kws = dscnn_dsblock_ws_kernel<64, 64>;
+        static SmemOptIn optin_ws;
+        if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
+        if ((int)d->in_maps.size() < d->net.nlayers) d->in_maps.resize(d->net.nlayers);
+        tcr_dscnn::InMap& im = d->in_maps[l];
+        if (im.ptr != in || im.rh != RHt) {                    // the activations ping-pong between two buffers: encoded once per layer
+          const int rc = ds_encode_in_map(&im.map, in, L.cin, L.win, L.hin, d->cfg.max_batch, L.wout + 2, RHt + 2);
+          if (rc != TCR_OK) return rc;
+          im.ptr = in;
+          im.rh = RHt;
+        }
+        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
+        TCR_LAUNCH("dscnn_dsblock_ws", kws, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_ws, s, im.map, L, RHt, n, params, out, eps);
+        return TCR_OK;
+      }
+      if (smem_tc <= 200 * 1024 && walk_ok) {
+        auto ktc = dscnn_dsblock_tc_kernel<64, 64>;
+        static SmemOptIn optin_tc;
+        if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
+        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
+        TCR_LAUNCH("dscnn_dsblock_tc", ktc, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
+        return TCR_OK;
+      }
+    }
+#endif
+    // the whole pointwise bank in shared memory when it fits next to a useful tile; else (DS-CNN-L: 276 x 276 fp32 = 305 KB) output-
+    // channel tiles of COT, the depthwise output of the tile being reused for every slice
+    int COT = L.cout;
+    while (COT > 32 && smem_for(1, COT) > 96 * 1024) COT = ((COT / 2) + 3) & ~3;
+    int RH = std::min(L.hout, 8);
+    while (RH > 1 && smem_for(RH, COT) > 100 * 1024) --RH;
+    const size_t smem = smem_for(RH, COT);
+    if (smem > 200 * 1024) { set_error("DS-CNN layer does not fit in shared memory"); return TCR_ERR_UNSUPPORTED; }
+    auto kfn = dscnn_dsblock_kernel;
+#ifndef TCR_EMU
+    static SmemOptIn optin;
+    if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
+#endif
+    TCR_LAUNCH("dscnn_dsblock", kfn, dim3((L.hout + RH - 1) / RH, n), dim3(256), smem, s, L, RH, COT, params, in, out, eps);
+  }
+  return TCR_OK;
+}
+
 extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const float* params, int32_t n, float* logits, float* probs,
                                  tcr_stream stream) {
   pdl_chain_reset();
   if (!d || !features || !params) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   if (n <= 0 || n > d->cfg.max_batch) { set_error("n outside [1, max_batch]"); return TCR_ERR_INVALID; }
   cudaStream_t s = (cudaStream_t)stream;
-  const float eps = 1e-3f;
   const float* in = features;
-  int cur = 0;
   for (int l = 0; l < d->net.nlayers; ++l) {
-    const DsLayerDev& L = d->net.layer[l];
-    float* out = d->act[cur];
-    if (L.type == 0) {
-#ifndef TCR_EMU
-      int RHt = std::min(L.hout, 128 / std::max(1, std::min(L.wout, 128)));
-      RHt = std::max(1, RHt);
-      RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);
-      const int K4 = L.kh * L.kw / 4, hin_t = (RHt - 1) * L.sh + L.kh, wpt = (L.wout - 1) * L.sw + L.kw;
-      // implicit GEMM on wgmma (3xTF32); the limits are the kernel's precomputed per-thread walks (4 cells, 4 gather tasks)
-      if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && hin_t * wpt <= 4 * kTcThreads &&
-          128 * K4 <= 4 * kTcThreads && hin_t < 512) {
-        const size_t smem_cws = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 4 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
-        if (d->tc_ws && smem_cws <= 220 * 1024 && hin_t * wpt <= 4 * kWsProducers && 128 * K4 <= 4 * kWsProducers && (K4 & 1) == 0) {
-          auto kws = dscnn_conv_ws_kernel<64>;
-          static SmemOptIn optin_cws;
-          if (optin_cws.ensure(kws, smem_cws) != cudaSuccess) return TCR_ERR_CUDA;
-          const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-          TCR_LAUNCH("dscnn_conv_ws", kws, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_cws, s, L, RHt, n, params, in, out, eps);
-          in = out;
-          cur ^= 1;
-          continue;
-        }
-        const size_t smem_tc = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 2 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
-        auto ktc = dscnn_conv_tc_kernel<64>;
-        static SmemOptIn optin_tc;
-        if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-        TCR_LAUNCH("dscnn_conv_tc", ktc, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
-        in = out;
-        cur ^= 1;
-        continue;
-      }
-#endif
-      const int hp = (L.hout - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
-      const size_t smem = (size_t)(((hp * wp + 3) & ~3) + L.kh * L.kw * L.cout + 2 * L.cout) * 4;
-      auto kfn = dscnn_conv_kernel;
-#ifndef TCR_EMU
-      static SmemOptIn optin;
-      if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
-#endif
-      TCR_LAUNCH("dscnn_conv", kfn, dim3(n), dim3(256), smem, s, L, params, in, out, eps);
-    } else {
-      auto smem_for = [&](int RH, int COT) {
-        const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
-        return (size_t)((size_t)hin_t * wp * L.cin + (size_t)RH * L.wout * L.cin + (size_t)L.cin * COT + L.kh * L.kw * L.cin +
-                        2 * L.cin + 2 * L.cout) * 4;
-      };
-#ifndef TCR_EMU
-      // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
-      if (d->use_tc && L.cin == 64 && L.cout == 64 && L.kh == 3 && L.kw == 3 && L.sh == 1 && L.sw == 1 && L.wout <= 64) {
-        int RHt = std::min(L.hout, 128 / L.wout);
-        RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);     // balanced: 25 rows -> 5 tiles of 5
-        const int C4 = L.cin / 4;
-        const bool walk_ok = (RHt + 2) * (L.wout + 2) <= 8 * (kTcThreads / C4);      // the kernel's precomputed fetch walk: 8 cells
-        const size_t smem_tc = (2 * (size_t)C4 * ((RHt + 2) * (L.wout + 2) * 4 + 4) + 2 * (size_t)C4 * (128 * 4 + 4) + 2 * (size_t)C4 * (L.cout * 4 + 4) +
-                                (size_t)9 * L.cin + 2 * L.cin + 2 * L.cout) * 4;
-        const int lba = ((RHt * L.wout + 7) & ~7) * 4 + 4;
-        const size_t xh = (((size_t)(RHt + 2) * (L.wout + 2) * 128 + 1023) & ~(size_t)1023) / 4;       // floats per half input tile
-        const size_t smem_ws = (4 * xh + 4 * (size_t)C4 * lba + 2 * (size_t)C4 * (L.cout * 4 + 4) + (size_t)9 * L.cin + 2 * L.cin + 2 * L.cout) * 4;
-        if (d->tc_ws && smem_ws <= 226 * 1024 && C4 * L.wout <= kWsProducers && L.wout + 2 <= 256 && RHt + 2 <= 256 && in != features) {
-          auto kws = dscnn_dsblock_ws_kernel<64, 64>;
-          static SmemOptIn optin_ws;
-          if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
-          if ((int)d->in_maps.size() < d->net.nlayers) d->in_maps.resize(d->net.nlayers);
-          tcr_dscnn::InMap& im = d->in_maps[l];
-          if (im.ptr != in || im.rh != RHt) {                    // the activations ping-pong between two buffers: encoded once per layer
-            const int rc = ds_encode_in_map(&im.map, in, L.cin, L.win, L.hin, d->cfg.max_batch, L.wout + 2, RHt + 2);
-            if (rc != TCR_OK) return rc;
-            im.ptr = in;
-            im.rh = RHt;
-          }
-          const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-          TCR_LAUNCH("dscnn_dsblock_ws", kws, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_ws, s, im.map, L, RHt, n, params, out, eps);
-          in = out;
-          cur ^= 1;
-          continue;
-        }
-        if (smem_tc <= 200 * 1024 && walk_ok) {
-          auto ktc = dscnn_dsblock_tc_kernel<64, 64>;
-          static SmemOptIn optin_tc;
-          if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-          const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-          TCR_LAUNCH("dscnn_dsblock_tc", ktc, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
-          in = out;
-          cur ^= 1;
-          continue;
-        }
-      }
-#endif
-      // the whole pointwise bank in shared memory when it fits next to a useful tile; else (DS-CNN-L: 276 x 276 fp32 = 305 KB) output-
-      // channel tiles of COT, the depthwise output of the tile being reused for every slice
-      int COT = L.cout;
-      while (COT > 32 && smem_for(1, COT) > 96 * 1024) COT = ((COT / 2) + 3) & ~3;
-      int RH = std::min(L.hout, 8);
-      while (RH > 1 && smem_for(RH, COT) > 100 * 1024) --RH;
-      const size_t smem = smem_for(RH, COT);
-      if (smem > 200 * 1024) { set_error("DS-CNN layer does not fit in shared memory"); return TCR_ERR_UNSUPPORTED; }
-      auto kfn = dscnn_dsblock_kernel;
-#ifndef TCR_EMU
-      static SmemOptIn optin;
-      if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
-#endif
-      TCR_LAUNCH("dscnn_dsblock", kfn, dim3((L.hout + RH - 1) / RH, n), dim3(256), smem, s, L, RH, COT, params, in, out, eps);
-    }
+    float* out = d->act[l & 1];
+    const int rc = ds_launch_layer(d, l, params, in, out, n, s);
+    if (rc != TCR_OK) return rc;
     in = out;
-    cur ^= 1;
   }
   const DsLayerDev& last = d->net.layer[d->net.nlayers - 1];
   if (last.cout > 320) { set_error("DS-CNN head supports up to 320 channels"); return TCR_ERR_UNSUPPORTED; }
   TCR_LAUNCH("dscnn_head", dscnn_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes, d->net.fcw,
              d->net.fcb, params, in, logits, probs);
+  if (cudaGetLastError() != cudaSuccess) { set_error("DS-CNN launch failed"); return TCR_ERR_CUDA; }
+  return TCR_OK;
+}
+
+extern "C" int tcr_dscnn_forward_partial(tcr_dscnn* d, const float* features, const float* params, int32_t n, int32_t num_layers,
+                                         float* act_out, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !features || !params || !act_out) { set_error("NULL argument"); return TCR_ERR_INVALID; }
+  if (n <= 0 || n > d->cfg.max_batch) { set_error("n outside [1, max_batch]"); return TCR_ERR_INVALID; }
+  if (num_layers <= 0 || num_layers > d->net.nlayers) { set_error("num_layers outside [1, number of layers]"); return TCR_ERR_INVALID; }
+  cudaStream_t s = (cudaStream_t)stream;
+  const float* in = features;
+  for (int l = 0; l < num_layers; ++l) {
+    float* out = l == num_layers - 1 ? act_out : d->act[l & 1];
+    const int rc = ds_launch_layer(d, l, params, in, out, n, s);
+    if (rc != TCR_OK) return rc;
+    in = out;
+  }
   if (cudaGetLastError() != cudaSuccess) { set_error("DS-CNN launch failed"); return TCR_ERR_CUDA; }
   return TCR_OK;
 }
