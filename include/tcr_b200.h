@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 6
+#define TCR_ABI_VERSION 7
 
 enum {
   TCR_OK = 0,
@@ -91,6 +91,10 @@ typedef struct tcr_info {
   int64_t workspace_bytes;
 } tcr_info;
 
+/* Optimizer of a training step (tcr_step_args::optimizer), the choices of helper/trainer.py:171-197 on the accelerated
+ * path.  "gd" is TCR_OPT_MOMENTUM with momentum 0. */
+enum { TCR_OPT_MOMENTUM = 0, TCR_OPT_ADAM = 1, TCR_OPT_RMSPROP = 2 };
+
 enum { TCR_KIND_WEIGHT = 0, TCR_KIND_BETA = 1, TCR_KIND_GAMMA = 2, TCR_KIND_MOVING_MEAN = 3, TCR_KIND_MOVING_VAR = 4 };
 
 /* One row per TF variable.  `name` is the reference's variable name (e.g.
@@ -115,10 +119,11 @@ typedef struct tcr_step_args {
   const float* onehot;       /* [n, num_classes] fp32 (datasets/audio_data_wrapper.py:113-118) */
   int32_t      n;            /* utterances on THIS rank */
   float*       params;       /* flat trainables, updated in place */
-  float*       slots;        /* flat momentum accumulators (`<var>/Momentum`), updated in place */
+  float*       slots;        /* flat first optimizer slot, updated in place: `<var>/Momentum` (momentum accumulator),
+                              * `<var>/Adam` (m, zero-initialised) or `<var>/RMSProp` (ms, initialised to 1.0) */
   float*       moving;       /* flat BN moving mean/variance, updated in place */
   float        learning_rate;
-  float        momentum;     /* 0.9 */
+  float        momentum;     /* 0.9 (MomentumOptimizer); RMSPropOptimizer's momentum (0 by default); unused by Adam */
   float        weight_decay; /* 0.001 */
   uint64_t     dropout_seed; /* counter-based RNG seed; ignored when dropout_mask != NULL or keep_prob == 1 */
   const float* dropout_mask; /* optional injected {0,1} mask [n, last_channels] (parity runs) */
@@ -126,7 +131,7 @@ typedef struct tcr_step_args {
   float*       logits;       /* optional device [n, num_classes] */
   float*       probs;        /* optional device [n, num_classes] softmax (output/softmax) */
   float*       grads;        /* optional device [num_trainable]: gradient of total_loss actually applied */
-  int32_t      apply_update; /* 1: momentum update + BN moving update; 0: gradients only */
+  int32_t      apply_update; /* 1: optimizer update + BN moving update; 0: gradients only (params, slots, moving untouched) */
   /* Optional device input stage in front of the front-end (TCR_INPUT_WAV_PCM16 only, see tcr_augment_pcm16): when `clips` is not
    * NULL, `input` holds the wav files' int16 samples [n, pcm_stride] and the step first decodes / shifts / mixes / clips them
    * into an internal fp32 buffer.  Zero-initialise these fields when the stage is not used. */
@@ -139,6 +144,26 @@ typedef struct tcr_step_args {
    * the rest of the step waits for it on `stream`.  0: everything is ordered on `stream` (the default; zero-initialise).
    * tcr_train_step_host sets it itself: its inputs arrive on the library's copy stream. */
   int32_t      input_resident;
+  /* Optimizer (ABI 7).  Zero-initialised, these fields select the momentum step above.  The rules, per parameter in fp32 with
+   * g the (rank-averaged) gradient, are TF 1.13's:
+   *   TCR_OPT_MOMENTUM  slots = slots*momentum + g;  params -= learning_rate*slots
+   *   TCR_OPT_ADAM      alpha = learning_rate*sqrt(1 - beta2_power)/(1 - beta1_power);
+   *                     slots += (g - slots)(1 - beta1);  slots2 += (g^2 - slots2)(1 - beta2);
+   *                     params -= (slots*alpha)/(sqrt(slots2) + epsilon)                     (tf.train.AdamOptimizer)
+   *   TCR_OPT_RMSPROP   slots += (g^2 - slots)(1 - rho);  slots2 = slots2*momentum + g*learning_rate/sqrt(slots + epsilon);
+   *                     params -= slots2                                                    (tf.train.RMSPropOptimizer)
+   * beta1_power / beta2_power are Adam's beta^t BEFORE this step (beta1 / beta2 at the first step); the caller advances them
+   * (beta *= beta) after each submitted step, as TF's finish op does.  They are plain values, so tcr_train_step_host captures
+   * them with the call.  Rejected with TCR_ERR_INVALID: an unknown kind, apply_update with Adam / RMSProp and no slots2,
+   * beta1_power == 1. */
+  int32_t      optimizer;    /* TCR_OPT_MOMENTUM | TCR_OPT_ADAM | TCR_OPT_RMSPROP */
+  float*       slots2;       /* flat second slot: `<var>/Adam_1` (v, zero-initialised) or `<var>/RMSProp_1` (mom, zero) */
+  float        beta1;        /* Adam: 0.9 */
+  float        beta2;        /* Adam: 0.999 */
+  float        epsilon;      /* Adam: 1e-8; RMSProp: 1e-10 */
+  float        rho;          /* RMSProp decay: 0.9 */
+  float        beta1_power;  /* Adam: beta1^t before this step */
+  float        beta2_power;  /* Adam: beta2^t before this step */
 } tcr_step_args;
 
 int         tcr_abi_version(void);
@@ -210,14 +235,15 @@ int tcr_forward(tcr_handle* h, const float* input, int32_t input_is_features, co
 int tcr_eval_accumulate(tcr_handle* h, const float* scores, const float* onehot, int32_t n, int32_t topk, int64_t* counts,
                         tcr_stream stream);
 
-/* Forward + backward + SGD-momentum + BN moving-average update (helper/trainer.py:171-222,
- * slim.learning.create_train_op).  With a communicator attached (tcr_comm_init) gradients are
- * averaged over ranks with one ncclAllReduce before the update. */
+/* Forward + backward + optimizer (momentum, Adam or RMSProp: tcr_step_args::optimizer) + BN moving-average update
+ * (helper/trainer.py:171-222, slim.learning.create_train_op).  With a communicator attached (tcr_comm_init) gradients are
+ * averaged over ranks with one ncclAllReduce (or the peer-memory exchange) before the update; every rank then applies the
+ * same update to the same averaged gradient, so the optimizer state stays identical across replicas. */
 int tcr_train_step(tcr_handle* h, const tcr_step_args* args, tcr_stream stream);
 
 /* The same step fed from PINNED HOST memory (the feed_dict / tf.data side of session.run(train_op): helper/trainer.py:312-321,
  * datasets/data_wrapper_base.py:100-108).  `a->input` and `a->onehot` are host pointers (cudaHostAlloc / pin_memory);
- * `a->losses` is ignored.  The batch is copied H2D on a private copy stream into one of 3 staging slots, the step runs on
+ * `a->losses` is ignored; the optimizer fields (and Adam's powers) are taken as they are in this call.  The batch is copied H2D on a private copy stream into one of 3 staging slots, the step runs on
  * `stream` behind it and its two losses are copied back; the call does not wait for the step it submits.  It returns,
  * in losses_out[0..1] and *losses_step, the losses of the step submitted `lag` calls earlier (*losses_step = -1 while
  * fewer than lag+1 steps are outstanding).  lag in [0,2]: 0 = synchronous, 1 = copy/compute overlap, 2 = also keeps

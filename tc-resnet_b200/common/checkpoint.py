@@ -7,7 +7,9 @@ directory (common/tf_utils.py:65-67, 219-247).  Two on-disk formats, same names 
                    format of tf.train.Saver, written / read by common/tf_bundle.py, so reference-trained weights load here
                    and checkpoints written here open with tf.train.load_checkpoint
   "npz"            <train_dir>/<Model>-<step>.npz (one NumPy archive)
-Content: {TF variable name: array, "<var>/Momentum": array, "global_step": int64}.
+Content: {TF variable name: array, the optimizer's state under TF's names, "global_step": int64}.  The optimizer state is
+"<var>/Momentum" (mom, gd), "<var>/Adam" + "<var>/Adam_1" + the scalars "beta1_power" / "beta2_power" (adam), or
+"<var>/RMSProp" + "<var>/RMSProp_1" (rmsprop).
 """
 from __future__ import annotations
 

@@ -648,6 +648,12 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
   pdl_chain_reset();
   if (!h || !a || !a->input || !a->onehot || !a->params) return fail(TCR_ERR_INVALID, "NULL argument");
   if (a->apply_update && (!a->slots || !a->moving)) return fail(TCR_ERR_INVALID, "apply_update needs slots and moving");
+  if (a->optimizer != TCR_OPT_MOMENTUM && a->optimizer != TCR_OPT_ADAM && a->optimizer != TCR_OPT_RMSPROP)
+    return fail(TCR_ERR_INVALID, "unknown optimizer %d", a->optimizer);
+  if (a->optimizer != TCR_OPT_MOMENTUM && a->apply_update && !a->slots2)
+    return fail(TCR_ERR_INVALID, "apply_update with Adam / RMSProp needs slots2");
+  if (a->optimizer == TCR_OPT_ADAM && a->beta1_power == 1.0f)
+    return fail(TCR_ERR_INVALID, "beta1_power == 1: Adam's step size lr*sqrt(1-beta2_power)/(1-beta1_power) is undefined");
   TCR_TRY(check_n(h, a->n));
   cudaStream_t s = (cudaStream_t)stream;
   const float* feat = a->input;

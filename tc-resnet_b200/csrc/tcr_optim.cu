@@ -1,11 +1,16 @@
-// tcr_optim.cu — gradient finalisation, SGD-momentum update, BN moving averages, loss scalars.
+// tcr_optim.cu — gradient finalisation, optimizer update (momentum / Adam / RMSProp), BN moving averages, loss scalars.
 //
 // Replaces, per training step: the 12/18 L2Loss nodes + AddN (factory/audio_nets.py:175-182), the 32/50
-// per-variable ApplyMomentum nodes (tf.train.MomentumOptimizer, helper/trainer.py:188-190: m <- mom*m + g;
-// v <- v - lr*m) and the 20/32 AssignSub moving-average updates of slim.batch_norm (decay 0.997, UNBIASED
-// batch variance, no zero-debias) with two flat multi-tensor kernels over the parameter buffer:
+// per-variable Apply{Momentum,Adam,RMSProp} nodes of the optimizer helper/trainer.py:171-197 builds and the 20/32
+// AssignSub moving-average updates of slim.batch_norm (decay 0.997, UNBIASED batch variance, no zero-debias) with two
+// flat multi-tensor kernels over the parameter buffer:
 //   grad_finalize_kernel : g[p] = sum_r partial[r][p] (+ weight_decay * w[p]); per-block sum of w^2
-//   update_kernel        : m <- mom*m + g/world ; w <- w - lr*m ; moving stats ; loss scalars
+//   update_kernel<opt>   : g/world -> one optimizer step (below) ; moving stats ; loss scalars
+// The three update rules, per parameter in fp32, in TF 1.13's order of operations (training_ops.cc):
+//   momentum  m <- m*mom + g ; w <- w - lr*m                                           (MomentumOptimizer)
+//   adam      alpha = lr*sqrt(1-b2^t)/(1-b1^t) ; m += (g-m)(1-b1) ; v += (g^2-v)(1-b2) ;
+//             w -= (m*alpha)/(sqrt(v)+eps)                                             (AdamOptimizer)
+//   rmsprop   ms += (g^2-ms)(1-rho) ; mom = mom*momentum + g*lr/sqrt(ms+eps) ; w -= mom  (RMSPropOptimizer)
 // The NCCL all-reduce of the flat gradient sits between the two when a communicator is attached.
 #include "tcr_bn.cuh"
 #include "tcr_net.h"
@@ -101,6 +106,10 @@ struct UpdateArgs {
   unsigned p2p_step;
   const float* peer_grads[8];
   unsigned* peer_flags[8];
+  // Adam / RMSProp (after the momentum step's fields, so its kernel reads the same parameter offsets)
+  float* slots2;                                       // Adam v / RMSProp mom (`slots`: Adam m / RMSProp ms)
+  float beta1, beta2, epsilon, rho;
+  float beta1_power, beta2_power;                      // Adam: beta^t before this step
 };
 
 // System-scope flag accesses for the cross-GPU arrival barrier.
@@ -121,6 +130,7 @@ __device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
 #endif
 }
 
+template <int kOpt>
 __global__ void __launch_bounds__(kOptThreads) update_kernel(UpdateArgs a) {
   pdl_wait();
   if (a.p2p_world > 1) {
@@ -151,9 +161,28 @@ __global__ void __launch_bounds__(kOptThreads) update_kernel(UpdateArgs a) {
     const float g = gsum * a.grad_scale;
     if (a.grads_out) a.grads_out[p] = g;
     if (a.apply) {
-      const float m = fmaf(a.slots[p], a.momentum, g);     // accum = accum * momentum + grad
-      a.slots[p] = m;
-      a.params[p] = a.params[p] - a.lr * m;                // var -= lr * accum
+      if constexpr (kOpt == TCR_OPT_MOMENTUM) {
+        const float m = fmaf(a.slots[p], a.momentum, g);     // accum = accum * momentum + grad
+        a.slots[p] = m;
+        a.params[p] = a.params[p] - a.lr * m;                // var -= lr * accum
+      } else if constexpr (kOpt == TCR_OPT_ADAM) {
+        // IEEE sqrtf and division (the library is built without fast-math): alpha is the same bits in every thread
+        const float alpha = a.lr * sqrtf(1.f - a.beta2_power) / (1.f - a.beta1_power);
+        float m = a.slots[p], v = a.slots2[p];
+        m += (g - m) * (1.f - a.beta1);
+        v += (g * g - v) * (1.f - a.beta2);
+        a.slots[p] = m;
+        a.slots2[p] = v;
+        a.params[p] = a.params[p] - (m * alpha) / (sqrtf(v) + a.epsilon);
+      } else {
+        static_assert(kOpt == TCR_OPT_RMSPROP, "unknown optimizer");
+        float ms = a.slots[p];
+        ms += (g * g - ms) * (1.f - a.rho);
+        const float mom = a.slots2[p] * a.momentum + (g * a.lr) / sqrtf(ms + a.epsilon);
+        a.slots[p] = ms;
+        a.slots2[p] = mom;
+        a.params[p] = a.params[p] - mom;
+      }
     }
   }
   // extra CTAs past the parameter range: one per BN layer (moving averages) + one for the loss scalars, so no
@@ -286,7 +315,15 @@ int net_update(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStr
   u.ce_sum = h->d_loss_part; u.ce_count = h->loss_gc; u.inv_n = 1.0f / (float)a->n;
   u.losses = a->losses; u.grads_out = a->grads; u.apply = a->apply_update ? 1 : 0;
   u.param_blocks = blocks;
-  TCR_LAUNCH("update", update_kernel, dim3(blocks + h->n_msegs + 1), dim3(kOptThreads), 0, s, u);
+  u.slots2 = a->slots2;
+  u.beta1 = a->beta1; u.beta2 = a->beta2; u.epsilon = a->epsilon; u.rho = a->rho;
+  u.beta1_power = a->beta1_power; u.beta2_power = a->beta2_power;
+  const dim3 grid(blocks + h->n_msegs + 1);
+  switch (a->optimizer) {            // the kind was validated by train_step_impl
+    case TCR_OPT_ADAM: TCR_LAUNCH("update", update_kernel<TCR_OPT_ADAM>, grid, dim3(kOptThreads), 0, s, u); break;
+    case TCR_OPT_RMSPROP: TCR_LAUNCH("update", update_kernel<TCR_OPT_RMSPROP>, grid, dim3(kOptThreads), 0, s, u); break;
+    default: TCR_LAUNCH("update", update_kernel<TCR_OPT_MOMENTUM>, grid, dim3(kOptThreads), 0, s, u); break;
+  }
   return 0;
 }
 

@@ -18,6 +18,39 @@ from . import _lib as L
 _MODELS = {"TCResNet8": 8, "TCResNet8Model": 8, "TCResNet14": 14, "TCResNet14Model": 14, 8: 8, 14: 14}
 _FEATURES = {"mfcc": L.TCR_FEATURE_MFCC, "log_mel_spectrogram": L.TCR_FEATURE_LOG_MEL}
 
+# Optimizers of the fused step (tcr_step_args::optimizer) with TF 1.13's defaults.  "mom" / "gd" take the step's `momentum`
+# argument; Adam and RMSProp take their hyper-parameters from the `optimizer` dict, Adam also its powers beta^t BEFORE the step.
+OPTIMIZER_DEFAULTS = {
+    "mom": dict(),
+    "gd": dict(),
+    "adam": dict(beta1=0.9, beta2=0.999, epsilon=1e-8),
+    "rmsprop": dict(decay=0.9, momentum=0.0, epsilon=1e-10),
+}
+# TF slot names of the optimizer state: `<var>/<slot>` for each of (slots, slots2)
+OPTIMIZER_SLOT_NAMES = {"mom": ("Momentum", None), "gd": ("Momentum", None), "adam": ("Adam", "Adam_1"),
+                        "rmsprop": ("RMSProp", "RMSProp_1")}
+
+
+def _optimizer_kind(optimizer) -> str:
+    kind = "mom" if optimizer is None else optimizer.get("kind", "mom")
+    if kind not in OPTIMIZER_DEFAULTS:
+        raise NotImplementedError(f"optimizer {kind!r}: expected one of {sorted(OPTIMIZER_DEFAULTS)}")
+    return kind
+
+
+def _set_optimizer(a, optimizer, slots2_ptr):
+    """Fills the optimizer fields of a TcrStepArgs.  None or kind "mom" / "gd" leave them zero: the momentum step."""
+    kind = _optimizer_kind(optimizer)
+    if kind in ("mom", "gd"):
+        return
+    o = dict(OPTIMIZER_DEFAULTS[kind], **{k: v for k, v in optimizer.items() if v is not None})
+    a.slots2, a.epsilon = slots2_ptr, float(o["epsilon"])
+    if kind == "adam":
+        a.optimizer, a.beta1, a.beta2 = L.TCR_OPT_ADAM, float(o["beta1"]), float(o["beta2"])
+        a.beta1_power, a.beta2_power = float(o["beta1_power"]), float(o["beta2_power"])
+    else:
+        a.optimizer, a.rho, a.momentum = L.TCR_OPT_RMSPROP, float(o["decay"]), float(o["momentum"])
+
 
 class Engine:
     def __init__(self, model="TCResNet8", width_multiplier=1.0, num_classes=12, sample_rate=16000,
@@ -115,6 +148,15 @@ class Engine:
                                                       seed, self._stream), "tcr_init_variables")
         return params, slots, moving
 
+    def new_optimizer_state(self, kind: str = "mom"):
+        """(slots, slots2) for an optimizer kind, initialised as TF's slot creators do: the momentum accumulator (slots2 None),
+        Adam's m and v (zeros), RMSProp's ms (ONES, as tf.train.RMSPropOptimizer in TF 1.x) and mom (zeros)."""
+        kind = _optimizer_kind(dict(kind=kind))
+        slots = torch.ones if kind == "rmsprop" else torch.zeros
+        first = slots(self.num_trainable, dtype=torch.float32, device=self.device)
+        second = torch.zeros(self.num_trainable, dtype=torch.float32, device=self.device) if OPTIMIZER_SLOT_NAMES[kind][1] else None
+        return first, second
+
     def variables_to_dict(self, params: torch.Tensor, moving: Optional[torch.Tensor] = None) -> Dict[str, np.ndarray]:
         """{TF variable name: ndarray} — the reference's `var_names_to_values` form (helper/trainer.py:145-154)."""
         p = params.detach().cpu().numpy()
@@ -191,8 +233,13 @@ class Engine:
                    dropout_seed: int = 0, dropout_mask: Optional[torch.Tensor] = None, input_is_features: bool = False,
                    want_outputs: bool = False, want_grads: bool = False, apply_update: bool = True,
                    losses: Optional[torch.Tensor] = None, clips: Optional[torch.Tensor] = None,
-                   background: Optional[torch.Tensor] = None, input_resident: bool = False):
-        """clips (uint8 CUDA tensor of n packed tcr_augment_clip records) + int16 `inputs` [n, stride]: the step starts with
+                   background: Optional[torch.Tensor] = None, input_resident: bool = False, *,
+                   optimizer: Optional[dict] = None, slots2: Optional[torch.Tensor] = None):
+        """optimizer: None or dict(kind="mom" | "gd") for the momentum step (`momentum`), dict(kind="adam", beta1=, beta2=,
+        epsilon=, beta1_power=, beta2_power=) or dict(kind="rmsprop", decay=, momentum=, epsilon=) (missing hyper-parameters
+        take TF's defaults, OPTIMIZER_DEFAULTS).  Adam / RMSProp keep their second slot in `slots2` (new_optimizer_state);
+        Adam's beta1_power / beta2_power are the values before this step, and advancing them is the caller's.
+        clips (uint8 CUDA tensor of n packed tcr_augment_clip records) + int16 `inputs` [n, stride]: the step starts with
         the device input stage (decode, shift, background mix, clip) instead of taking decoded fp32 samples.
         input_resident=True: `inputs` is final when the call is made (nothing queued on the current stream writes it); the
         front-end then runs ahead on the library's own stream and overlaps the previous step's tail (tcr_step_args::input_resident)."""
@@ -219,6 +266,7 @@ class Engine:
             a.grads = self._ptr(out["grads"])
         a.apply_update = int(apply_update)
         a.input_resident = int(bool(input_resident))
+        _set_optimizer(a, optimizer, self._ptr(slots2))
         L.check(self.lib, self.lib.tcr_train_step(self._h, C.byref(a), self._stream), "tcr_train_step")
         return out
 
@@ -320,8 +368,10 @@ class HostFeed:
 
     def submit(self, h_inputs: torch.Tensor, h_onehot: torch.Tensor, params, slots, moving, learning_rate, momentum=0.9,
                weight_decay=1e-4, dropout_seed=0, input_is_features=False, h_clips: Optional[torch.Tensor] = None,
-               background: Optional[torch.Tensor] = None):
-        """h_clips (pinned uint8 tensor of n packed tcr_augment_clip records, datasets/device_input_stage.py) with int16
+               background: Optional[torch.Tensor] = None, *, optimizer: Optional[dict] = None,
+               slots2: Optional[torch.Tensor] = None):
+        """optimizer / slots2: as Engine.train_step; the values (Adam's powers included) are captured with this call.
+        h_clips (pinned uint8 tensor of n packed tcr_augment_clip records, datasets/device_input_stage.py) with int16
         h_inputs [n, stride]: the wav files' samples and the per-clip draws cross the bus; the input stage runs on the device
         (`background`: the CUDA-resident bank)."""
         eng = self.eng
@@ -337,6 +387,7 @@ class HostFeed:
         a.params, a.slots, a.moving = eng._ptr(params), eng._ptr(slots), eng._ptr(moving)
         a.learning_rate, a.momentum, a.weight_decay = float(learning_rate), float(momentum), float(weight_decay)
         a.dropout_seed, a.apply_update = int(dropout_seed), 1
+        _set_optimizer(a, optimizer, eng._ptr(slots2))
         L.check(eng.lib, eng.lib.tcr_train_step_host(eng._h, C.byref(a), self.lag, eng._stream, self._out, C.byref(self._step)),
                 "tcr_train_step_host")
         return self._result()

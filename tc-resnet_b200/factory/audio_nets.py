@@ -16,7 +16,7 @@ import torch
 
 from ..common import utils
 from ..datasets import preprocessor_factory
-from ..engine import Engine
+from ..engine import OPTIMIZER_DEFAULTS, OPTIMIZER_SLOT_NAMES, Engine
 from ..runtime import InvalidArgumentError, Node
 from .base import TFModel
 
@@ -34,7 +34,9 @@ class AudioNetModel(TFModel):
         self.args, self.dataset = args, dataset
         self.engine: Optional[Engine] = None
         self.global_step = 0
-        self.optimizer = dict(kind="mom", momentum=0.9)            # filled in by the trainer (build_optimizer)
+        self.optimizer = dict(kind="mom", momentum=0.9)            # set by the trainer (build_optimizer -> set_optimizer)
+        self.slots2 = None                                          # Adam v / RMSProp mom (`slots`: the first slot)
+        self.beta1_power = self.beta2_power = None                  # Adam's beta^t before the next step (np.float32)
         self.lr_schedule = lambda step: getattr(args, "learning_rate", 1e-4)
         self.var_names_to_values = None                            # in-memory weight injection hook (trainer.py:145-154)
         self.endpoints_loss: Dict[str, Node] = {}
@@ -140,21 +142,72 @@ class AudioNetModel(TFModel):
     def outputs(self):
         return self._outputs
 
+    # ------------------------------------------------------------------ optimizer state
+    def set_optimizer(self, optimizer: Dict[str, object]):
+        """Takes the optimizer the trainer built (TrainerBase.build_optimizer) and allocates its state as TF creates it: the
+        slot buffers of the kind (Engine.new_optimizer_state) and, for Adam, beta1_power / beta2_power = beta1 / beta2."""
+        self.flush_feed()
+        self.optimizer = dict(optimizer)
+        kind = self.optimizer["kind"]
+        if self.engine is not None:
+            self.slots, self.slots2 = self.engine.new_optimizer_state(kind)
+        if kind == "adam":
+            self.beta1_power, self.beta2_power = np.float32(self._opt("beta1")), np.float32(self._opt("beta2"))
+        else:
+            self.beta1_power = self.beta2_power = None
+
+    def _opt(self, key):
+        v = self.optimizer.get(key)
+        return OPTIMIZER_DEFAULTS[self.optimizer["kind"]][key] if v is None else v
+
+    def _step_optimizer(self) -> Dict[str, object]:
+        """The `optimizer` argument of this step (Engine.train_step / HostFeed.submit)."""
+        o = dict(self.optimizer)
+        if o["kind"] == "adam":
+            o.update(beta1_power=self.beta1_power, beta2_power=self.beta2_power)
+        return o
+
+    def _advance_optimizer(self):
+        """After each submitted step: beta^t <- beta^t * beta in fp32, TF's assign(beta1_power * beta1) in the finish op.  Every
+        rank does the same, so data-parallel replicas hold the same powers without exchanging them."""
+        if self.optimizer["kind"] == "adam":
+            self.beta1_power = np.float32(self.beta1_power * np.float32(self._opt("beta1")))
+            self.beta2_power = np.float32(self.beta2_power * np.float32(self._opt("beta2")))
+
     # ------------------------------------------------------------------ variables by TF name
     def get_variables(self, with_slots=True) -> Dict[str, np.ndarray]:
+        """{TF name: array}: the variables, and with_slots the optimizer state under TF's names (`<var>/Momentum`;
+        `<var>/Adam`, `<var>/Adam_1`, beta1_power, beta2_power; `<var>/RMSProp`, `<var>/RMSProp_1`)."""
         self.flush_feed()
         out = self.engine.variables_to_dict(self.params, self.moving)
         if with_slots:
-            for k, v in self.engine.variables_to_dict(self.slots).items():
-                out[k + "/Momentum"] = v
+            names = OPTIMIZER_SLOT_NAMES[self.optimizer["kind"]]
+            for suffix, buf in zip(names, (self.slots, self.slots2)):
+                if suffix is not None:
+                    for k, v in self.engine.variables_to_dict(buf).items():
+                        out[f"{k}/{suffix}"] = v
+            if self.optimizer["kind"] == "adam":
+                out["beta1_power"], out["beta2_power"] = np.float32(self.beta1_power), np.float32(self.beta2_power)
         return out
 
     def set_variables(self, values: Dict[str, np.ndarray], strict=True):
+        """Variables by TF name; the optimizer state of the current kind is optional (slots and powers that are absent keep
+        their values)."""
         self.flush_feed()
         self.engine.variables_from_dict(values, self.params, self.moving, strict=strict)
-        slots = {k[:-len("/Momentum")]: v for k, v in values.items() if k.endswith("/Momentum")}
-        if slots:
-            self.engine.variables_from_dict(slots, self.slots, None, strict=False)
+        names = OPTIMIZER_SLOT_NAMES[self.optimizer["kind"]]
+        for suffix, buf in zip(names, (self.slots, self.slots2)):
+            if suffix is None:
+                continue
+            tail = "/" + suffix
+            slots = {k[:-len(tail)]: v for k, v in values.items() if k.endswith(tail)}
+            if slots:
+                self.engine.variables_from_dict(slots, buf, None, strict=False)
+        if self.optimizer["kind"] == "adam":
+            if "beta1_power" in values:
+                self.beta1_power = np.float32(np.asarray(values["beta1_power"], np.float32).reshape(()))
+            if "beta2_power" in values:
+                self.beta2_power = np.float32(np.asarray(values["beta2_power"], np.float32).reshape(()))
 
     def _dropout_seed(self):
         """Counter-RNG seed of this step: distinct per rank under data parallelism (the kernel indexes utterances locally)."""
@@ -198,7 +251,9 @@ class AudioNetModel(TFModel):
             self._feed = HostFeed(self.engine, lag=lag)
         lr = float(self.lr_schedule(self.global_step))
         r = self._feed.submit(pinned[0], pinned[1], self.params, self.slots, self.moving, lr, self.optimizer.get("momentum") or 0.0,
-                              self.args.weight_decay, dropout_seed=self._dropout_seed())
+                              self.args.weight_decay, dropout_seed=self._dropout_seed(), optimizer=self._step_optimizer(),
+                              slots2=self.slots2)
+        self._advance_optimizer()
         self.global_step += 1
         self._feed_steps.append(self.global_step)
         if r is not None:
@@ -236,7 +291,9 @@ class AudioNetModel(TFModel):
             lr = float(self.lr_schedule(self.global_step))
             out = self.engine.train_step(self._d_wav, self._d_hot, self.params, self.slots, self.moving, lr,
                                          self.optimizer.get("momentum") or 0.0, wd, dropout_seed=self._dropout_seed(),
-                                         want_outputs=bool(names & {"outputs", "logits"}))
+                                         want_outputs=bool(names & {"outputs", "logits"}), optimizer=self._step_optimizer(),
+                                         slots2=self.slots2)
+            self._advance_optimizer()
             self.global_step += 1
             vals["train_op"], vals["learning_rate"] = None, np.float32(lr)
         else:

@@ -2,9 +2,10 @@
 
 What changes underneath: `build_train_op` does not assemble a gradient graph (slim.learning.create_train_op,
 :199-222) — it arms the model so that fetching the train op in `session.run` executes ONE fused CUDA training step
-(front-end, forward, backward, SGD-momentum, BN moving averages).  The learning rate is
+(front-end, forward, backward, optimizer update, BN moving averages).  The learning rate is
 tf.train.piecewise_constant(global_step, boundaries, lr_list) (:135) evaluated on the host per step.
-Optimizers: "mom" (script default) and "gd" (= momentum 0) run on the CUDA path; "adam"/"rmsprop" raise.
+Optimizers: all four choices of --optimizer run on the CUDA path: "adam" (the default), "rmsprop", "mom" and "gd"
+(= momentum 0), with TF 1.13's defaults for whatever --momentum / --optimizer_decay / --optimizer_epsilon leave unset.
 """
 from __future__ import annotations
 
@@ -71,8 +72,17 @@ class TrainerBase:
         if optimizer == "gd":
             self.log.info("Use GradientDescentOptimizer")
             return dict(kind="gd", momentum=0.0)
-        if optimizer in ("adam", "rmsprop"):
-            raise NotImplementedError(f"optimizer '{optimizer}' is not on the CUDA path (TC-ResNet recipes use --optimizer mom)")
+        # Like the reference (:171-197), a flag is passed on only when it is truthy; what is left takes TF's default.
+        if optimizer == "adam":
+            if momentum or decay:       # tf.train.AdamOptimizer has no such arguments: the reference fails with a TypeError
+                raise TypeError("--optimizer adam takes no --momentum or --optimizer_decay "
+                                "(tf.train.AdamOptimizer has neither argument)")
+            self.log.info("Use AdamOptimizer")
+            return dict(kind="adam", beta1=0.9, beta2=0.999, epsilon=epsilon if epsilon else 1e-8)
+        if optimizer == "rmsprop":
+            self.log.info("Use RMSPropOptimizer")
+            return dict(kind="rmsprop", decay=decay if decay else 0.9, momentum=momentum if momentum else 0.0,
+                        epsilon=epsilon if epsilon else 1e-10)
         self.log.error(f"Unknown optimizer: {optimizer}")
         raise NotImplementedError
 
@@ -81,7 +91,7 @@ class TrainerBase:
             raise NotImplementedError("--trainable_scopes (partial training) is not supported by the fused step")
         if self.args.use_ema:
             raise NotImplementedError("--use_ema is not supported by the fused step")
-        self.model.optimizer = optimizer
+        self.model.set_optimizer(optimizer)          # before the restore: the checkpoint may carry the optimizer's state
         return Node("train_op")
 
     def routine_restore_and_initialize(self, checkpoint_path=None):
