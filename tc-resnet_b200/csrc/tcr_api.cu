@@ -703,26 +703,22 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
 #endif
   }
   const int resident = resident_mode(h);
-  if (resident < 1) net_weight_transpose(h, a->params, s);      // the resident forward kernel writes the transposed banks itself
-  int rc = resident >= 1 ? resident_forward(h, feat, a, s)
-                               : net_forward(h, feat, a->params, nullptr, a->n, true, a->dropout_seed, a->dropout_mask, a->onehot,
-                                             a->weight_decay, a->logits, a->probs, nullptr, /*backward=*/true, s);
+  if (resident == kResidentOff) net_weight_transpose(h, a->params, s);   // the resident forward kernel writes the transposed banks itself
+  int rc = resident != kResidentOff ? resident_forward(h, feat, a, s)
+                                    : net_forward(h, feat, a->params, nullptr, a->n, true, a->dropout_seed, a->dropout_mask, a->onehot,
+                                                  a->weight_decay, a->logits, a->probs, nullptr, /*backward=*/true, s);
   if (rc) return fail(rc, "forward launch failed: %s", g_err);
-  if (resident < 2) {               // mode 2: net_update runs the resident backward kernel instead
-    rc = net_backward(h, feat, a->params, a->n, s);
-    if (rc) return fail(rc, "backward launch failed: %s", g_err);
-  } else if (resident == 3) {       // backward-data chain as one resident kernel, then the grouped weight-gradient launch
-    rc = resident_backward_data(h, feat, a, s);
-    if (!rc) rc = net_weight_gradients(h, feat, a->n, s);
-    if (rc) return fail(rc, "backward launch failed: %s", g_err);
-  }
+  rc = resident == kResidentFwdBwdData ? resident_backward_data(h, feat, a, s) : net_backward_data(h, a->params, a->n, s);
+  if (rc) return fail(rc, "backward launch failed: %s", g_err);
+  rc = net_weight_gradients(h, feat, a->n, s);
+  if (rc) return fail(rc, "weight-gradient launch failed: %s", g_err);
 #ifndef TCR_EMU
   if (h->fe_gate) {                   // the gate of the NEXT step's front-end (see above)
     TCR_CUDA(cudaEventRecord((cudaEvent_t)h->fe_gate, s));
     h->fe_gate_valid = 1;
   }
 #endif
-  rc = net_update(h, feat, a, s);
+  rc = net_update(h, a, s);
   if (rc) return fail(rc, "update launch failed: %s", g_err);
   TCR_CUDA(cudaGetLastError());
 #ifndef TCR_EMU

@@ -10,32 +10,35 @@ void set_error(const char* msg);
 int net_alloc_workspace(tcr_handle* h);
 
 // Forward pass on features [n, T, F].  training: batch-statistics BN (+ dropout); otherwise the BN tables are
-// built from `moving`.  backward: the head additionally emits dlogits-derived tensors for net_backward.
+// built from `moving`.  backward: the head additionally emits dlogits-derived tensors for the backward pass.
 int net_forward(tcr_handle* h, const float* feat, const float* params, const float* moving, int n, bool training,
                 uint64_t seed, const float* mask, const float* onehot, float weight_decay, float* logits,
                 float* probs, float* losses, bool backward, cudaStream_t s);
 
-// Backward-data chain + all weight-gradient kernels; leaves per-layer partial sums in the workspace.
 int cluster_size(tcr_handle* h);
 StatSrc stat_src(const tcr_handle* h, const ConvPlan& cv, const float* params, int n);
 int augment_launch(const int16_t* pcm, int64_t pcm_stride, const tcr_augment_clip* clips, const float* background, int64_t background_samples,
                    float* out, int clip, int n, cudaStream_t s);
 int eval_accumulate_launch(const float* scores, const float* onehot, int n, int classes, int topk, int64_t* counts, cudaStream_t s);
 int net_weight_transpose(tcr_handle* h, const float* params, cudaStream_t s);
-// Resident forward (tcr_resident.cu): the training forward + head as one cooperative kernel with SM-resident activations.
 int sync_records(tcr_handle* h, const float* part, int gc, int cols, float* out, cudaStream_t s);   // SyncBN: sum records, all-reduce
 inline bool sync_bn_on(const tcr_handle* h) { return h->sync_bn && h->world > 1 && h->comm; }
 inline float bn_inv(const tcr_handle* h, int n, int t) { return 1.0f / ((float)n * (float)t * (sync_bn_on(h) ? (float)h->world : 1.0f)); }
-int resident_mode(tcr_handle* h);      // 0: per-layer kernels, 1: resident forward, 2: resident forward + backward (dW inside), 3: resident forward + backward-data
+// Resident kernels (tcr_resident.cu): the training forward + head, and the backward-data chain, each as one cooperative kernel with
+// SM-resident activations.  ResidentMode says which of them a handle runs; the values are the TCR_RESIDENT settings that force
+// them.  The weight gradients always come from the grouped launch (net_weight_gradients).
+enum ResidentMode { kResidentOff = 0, kResidentFwd = 1, kResidentFwdBwdData = 3 };
+int resident_mode(tcr_handle* h);
 int resident_forward(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s);
-int resident_backward(tcr_handle* h, const float* feat, const tcr_step_args* a, float* grads, int* l2_records, cudaStream_t s);
-int resident_backward_data(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s);   // mode 3
-int net_weight_gradients(tcr_handle* h, const float* feat, int n, cudaStream_t s);                      // the grouped launch alone
+int resident_backward_data(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s);
 void resident_destroy(tcr_handle* h);
-int net_backward(tcr_handle* h, const float* feat, const float* params, int n, cudaStream_t s);
+// Backward-data chain as per-layer kernels: every layer's masked gradient and BatchNorm-backward sums, as resident_backward_data.
+int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s);
+// Every layer's weight gradient in one grouped launch, from the layer gradients either backward-data chain leaves.
+int net_weight_gradients(tcr_handle* h, const float* feat, int n, cudaStream_t s);
 
-// Gradient finalisation (+ weight decay), optional NCCL all-reduce, momentum update, BN moving averages, losses.
-int net_update(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s);
+// Gradient finalisation (+ weight decay), optional NCCL all-reduce, optimizer update, BN moving averages, losses.
+int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s);
 
 int launch_loss_only(tcr_handle* h, const float* params, float weight_decay, int n, float* losses, cudaStream_t s);
 int head_groups(int n);

@@ -673,7 +673,7 @@ int net_weight_transpose(tcr_handle* h, const float* params, cudaStream_t s) {
   return 0;
 }
 
-int net_backward(tcr_handle* h, const float* feat, const float* params, int n, cudaStream_t s) {
+int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s) {
   for (int i = (int)h->blocks.size() - 1; i >= 0; --i) {
     BlockPlan& b = h->blocks[i];
     ConvPlan& ca = h->convs[b.a];
@@ -736,7 +736,7 @@ int net_backward(tcr_handle* h, const float* feat, const float* params, int n, c
       }
     }
   }
-  return net_weight_gradients(h, feat, n, s);
+  return 0;
 }
 
 // weight gradients: every layer's inputs are final now -> one grouped launch over all layers

@@ -280,7 +280,7 @@ int build_opt_segments(tcr_handle* h) {
 
 static int fc_segment(const tcr_handle* h) { return (int)h->convs.size() * 3; }
 
-int net_update(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s) {
+int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s) {
   const int blocks = (int)((h->n_train + kOptThreads - 1) / kOptThreads);
   if (blocks > 4096) { set_error("parameter count too large for the l2 partial buffer"); return TCR_ERR_UNSUPPORTED; }
   const bool p2p = h->p2p.attached && h->world > 1;
@@ -288,13 +288,7 @@ int net_update(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStr
   float* grads = p2p ? h->p2p.grads + (size_t)(h->p2p.step & 1u) * h->n_train : h->d_grads;
   GradArgs ga{h->d_segs, h->n_segs, h->n_train, fc_segment(h), h->d_dwfc_part, h->fc_records, a->params, a->weight_decay,
               grads, h->d_l2part, sync_bn_on(h) ? 1.0f / (float)h->world : 1.0f};
-  int l2_records = blocks;
-  if (resident_mode(h) == 2) {      // backward chain + weight gradients + this reduction in one cooperative kernel (tcr_resident.cu)
-    int rc = resident_backward(h, feat, a, grads, &l2_records, s);
-    if (rc) return rc;
-  } else {
-    TCR_LAUNCH("grad_finalize", grad_finalize_kernel, dim3(blocks), dim3(kOptThreads), 0, s, ga);
-  }
+  TCR_LAUNCH("grad_finalize", grad_finalize_kernel, dim3(blocks), dim3(kOptThreads), 0, s, ga);
   if (!p2p && h->comm && h->world > 1) {
     int rc = comm_allreduce_sum(h, h->d_grads, h->n_train, s);
     if (rc) return rc;
@@ -311,7 +305,7 @@ int net_update(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStr
   u.one_minus_decay = (float)(1.0 - (double)h->cfg.bn_decay);
   u.grad_scale = 1.0f / (float)h->world;
   u.msegs = h->d_msegs; u.nmsegs = h->n_msegs; u.n = sync_bn_on(h) ? a->n * h->world : a->n;   // rows behind the batch variance
-  u.l2part = h->d_l2part; u.l2blocks = l2_records;
+  u.l2part = h->d_l2part; u.l2blocks = blocks;
   u.ce_sum = h->d_loss_part; u.ce_count = h->loss_gc; u.inv_n = 1.0f / (float)a->n;
   u.losses = a->losses; u.grads_out = a->grads; u.apply = a->apply_update ? 1 : 0;
   u.param_blocks = blocks;

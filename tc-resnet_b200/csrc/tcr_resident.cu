@@ -1,6 +1,6 @@
 // tcr_resident.cu — the training step's network part as TWO cooperative kernels whose activations never leave the SM between
-// layers: resident_fwd_kernel (all conv layers + head) and resident_bwd_kernel (backward-data chain, every layer's weight
-// gradient, gradient reduction + weight decay).
+// layers: resident_fwd_kernel (all conv layers + head) and resident_bwd_kernel (the backward-data chain).  The weight gradients
+// are not computed here: the grouped launch (dw_grouped, two CTAs per SM) reads the layer gradients the backward kernel stores.
 //
 // Why: BatchNorm's batch statistics force a grid-wide dependency after every conv layer, forward and backward
 // (audio_nets/tc_resnet.py:21-41 under TCResNet_arg_scope :102-123; FusedBatchNormGrad in the gradient graph of
@@ -9,16 +9,14 @@
 //   * one CTA of 512 threads per SM owns ceil(n / #SMs) whole utterances for the whole pass; a layer's output stays in shared
 //     memory and becomes the next layer's input tile by one smem -> smem pass (BatchNorm + ReLU (+ residual) applied there);
 //   * batch statistics travel as per-CTA records through L2 behind a split grid barrier: a CTA arrives as soon as its record is
-//     written, then does the work nobody waits for (store the pre-BN output for the backward pass, this layer's weight gradient,
-//     prefetch of the next filter bank by TMA and of the next tensors by cp.async) and only then waits;
+//     written, then does the work nobody waits for (store the pre-BN output or the layer gradient, prefetch of the next filter
+//     bank by TMA and of the next tensors by cp.async) and only then waits;
 //   * every CTA sums the records itself (float4 loads, all in flight at once, fixed order: bit-reproducible), CTA 0 publishes;
-//   * the phase bodies are non-inlined functions shared by all layers, so their code is fetched once and stays in the I-cache;
-//   * weight gradients never go through atomics: one partial per CTA, reduced in a fixed order by the kernel's last phase.
+//   * the phase bodies are non-inlined functions shared by all layers, so their code is fetched once and stays in the I-cache.
 // The forward kernel leaves exactly what the multi-kernel forward leaves (plus the transposed filter banks of the backward pass) and
-// the backward kernel what net_backward + grad_finalize leave, so either can be paired with the per-layer kernels.
-// TCR_RESIDENT = 0: per-layer kernels | 1: resident forward | 2: resident forward + backward with the weight gradients and the
-// gradient reduction inside | 3 (default): resident forward + resident backward-DATA chain; the weight gradients stay in the
-// grouped launch (two CTAs per SM), which reads the layer gradients the kernel stores.
+// the backward kernel what the backward-data launches of net_backward_data leave, so either can be paired with the per-layer kernels.
+// TCR_RESIDENT = 0: per-layer kernels | 1: resident forward, per-layer backward-data | unset or anything else: both resident
+// kernels (resident_state falls back to 1 or 0 where a shape does not fit).
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -37,7 +35,6 @@ struct RConv {
   float* y; float* bnf; float* var; float* bsum;
   float* g;                                        // gradient after this layer's ReLU mask (what the grouped weight-gradient launch reads)
   float* frec; float* brec;                        // [G][2*cout] per-CTA records: (sum y, sum y^2) / (sum dz, sum dz*xhat)
-  float* dwres;                                    // [G][k*cin*cout] per-CTA weight-gradient partials
   const float* wT;                                 // transposed bank [k][cout][cin]
   int tm, ks;                                      // forward tiling: rows per thread task, k-slices
   int bks;                                         // backward-data k-slices
@@ -57,11 +54,8 @@ struct ResProgram {                  // static per handle
   int b_w, b_ys, b_yp, b_dys, b_dyd, b_pl, b_g[3], b_tbl, b_bs, b_red;
   int b_ys_cap;                      // floats of the b_ys region: it doubles as the backward epilogue's reduction scratch
   // head
-  long long fc_off, fc2_off;
+  long long fc_off;
   float* loss_part; float* dwfc_part; float* gout; float* bpartb; float* bpartd;
-  // gradient reduction
-  long long n_train;
-  float* l2part;
 };
 
 struct ResCall {                     // per call
@@ -69,9 +63,6 @@ struct ResCall {                     // per call
   unsigned long long seed; float keep; int use_dropout; float label_smoothing;
   float* logits; float* probs;
   int n; unsigned bar_base; float inv_n;
-  float weight_decay; float* grads;  // backward kernel
-  int dw_inside;                     // backward kernel: 1 = weight gradients + reduction in the kernel, 0 = it stores the layer gradients
-                                     // for the grouped weight-gradient launch instead (mode 3)
   long long* tl;                     // debug timeline (TCR_DEBUG_TIMELINE=1): [cta][32] globaltimer stamps, else null
 };
 
@@ -750,7 +741,8 @@ __device__ __noinline__ void res_convT(float* smem, int dys_off, int dysd_off, i
 }
 
 // Backward epilogue: dx = sum of planes (+ identity gradient); g = dx masked by the consumer-side ReLU; this CTA's
-// (sum g, sum g*xhat) records of the layer(s) below; g stays in shared memory (gdst) for the next phase.
+// (sum g, sum g*xhat) records of the layer(s) below; g stays in shared memory (gdst) for the next phase and goes to global memory
+// (gglob) for the grouped weight-gradient launch.
 //   kind 1: mask bn(yp) > 0, sums for that layer.  kind 2: mask (previous block's output) > 0, sums for its conv_b (yp, tp) and,
 //   when ypd != null, for its shortcut conv (additionally masked by bn_d(ypd) > 0).  The block output is read from outp
 //   (identity shortcut) or recomputed as bn_b(yp) + relu(bn_d(ypd)).
@@ -779,7 +771,7 @@ __device__ __noinline__ void res_bwd_epilogue(const float* dxs, int rcap, int KS
       else if (ypd) g = rmask_pos4(v, add4(chan4_bn(kp, yv), relu4(zd)));      // the block output, recomputed exactly as the forward pass formed it
       else g = rmask_pos4(v, ld4(outp + o));
       st4(gdst + o, g);
-      if (gglob) st4(gglob + o, g);
+      st4(gglob + o, g);
       s1 = add4(s1, g);
       s2 = add4(s2, rmul4(g, chan4_xhat(kp, yv)));
       if (ypd) {
@@ -804,161 +796,6 @@ __device__ __noinline__ void res_bwd_epilogue(const float* dxs, int rcap, int KS
     rec[cc * 2 + (qd & 1)] = s;
   }
   __syncthreads();
-}
-
-// This CTA's weight-gradient partial of one conv: dW[k][ci][co] = sum_rows x[row*S + k][ci] * dy[row][co] over its utterances.
-// Thread (rg, kg, tile) owns 4 ci x 4 co x KT taps (KT = 3 for the 9- and 3-tap convs, 1 for the 1x1 shortcut conv) and walks
-// rows rg, rg + RG, ... of every utterance with the next row's operands already in flight; the row groups then add their tiles one
-// after the other into `scr` [K*cin*cout] (fixed order), which is copied to the global partial.  xs [U][TPx][XS], dy [U][TPd][DS].
-template <int K>
-__device__ __noinline__ void res_dw(float* smem, int xs_off, int TPx, int XS, int dy_off, int TPd, int PLd, int DS, int Ue, int cin,
-                                    int cout, int S, int t_out, float* scr, float* out) {
-  constexpr int KT = K >= 3 ? 3 : 1, NKG = K / KT;
-  const int tid = threadIdx.x;
-  const int NCO = cout >> 2, NT = (cin >> 2) * NCO;          // 4x4 tiles of the [ci][co] plane
-  const int NP = NT * NKG;
-  const int RG = imax(1, imin(imin(kResThreads / NP, 16), t_out));
-  const int rg = tid / NP, pr = tid - rg * NP;
-  const int kg = pr / NT, tile = pr - kg * NT;
-  const int co4 = tile % NCO, ci4 = tile / NCO;
-  const bool worker = rg < RG;
-  float4 acc[KT][4];
-#pragma unroll
-  for (int j = 0; j < KT; ++j)
-#pragma unroll
-    for (int i = 0; i < 4; ++i) acc[j][i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (worker) {
-    const int xstep = S * XS;
-    for (int u = 0; u < Ue; ++u) {
-      int xrow = xs_off + u * TPx * XS + rg * xstep + kg * KT * XS + 4 * ci4;
-      int drow = dy_off + (u * TPd + PLd + rg) * DS + 4 * co4;
-      int t = rg;
-      if (t >= t_out) continue;
-      float4 d = ld4(smem + drow), x[KT];
-#pragma unroll
-      for (int j = 0; j < KT; ++j) x[j] = ld4(smem + xrow + j * XS);
-      for (;;) {
-        t += RG; xrow += RG * xstep; drow += RG * DS;
-        const bool more = t < t_out;
-        float4 dn = d, xn[KT];
-#pragma unroll
-        for (int j = 0; j < KT; ++j) xn[j] = x[j];
-        if (more) {                   // next row's operands are requested before this row's FMAs
-          dn = ld4(smem + drow);
-#pragma unroll
-          for (int j = 0; j < KT; ++j) xn[j] = ld4(smem + xrow + j * XS);
-        }
-#pragma unroll
-        for (int j = 0; j < KT; ++j) {
-          acc[j][0].x = fmaf(x[j].x, d.x, acc[j][0].x); acc[j][0].y = fmaf(x[j].x, d.y, acc[j][0].y);
-          acc[j][0].z = fmaf(x[j].x, d.z, acc[j][0].z); acc[j][0].w = fmaf(x[j].x, d.w, acc[j][0].w);
-          acc[j][1].x = fmaf(x[j].y, d.x, acc[j][1].x); acc[j][1].y = fmaf(x[j].y, d.y, acc[j][1].y);
-          acc[j][1].z = fmaf(x[j].y, d.z, acc[j][1].z); acc[j][1].w = fmaf(x[j].y, d.w, acc[j][1].w);
-          acc[j][2].x = fmaf(x[j].z, d.x, acc[j][2].x); acc[j][2].y = fmaf(x[j].z, d.y, acc[j][2].y);
-          acc[j][2].z = fmaf(x[j].z, d.z, acc[j][2].z); acc[j][2].w = fmaf(x[j].z, d.w, acc[j][2].w);
-          acc[j][3].x = fmaf(x[j].w, d.x, acc[j][3].x); acc[j][3].y = fmaf(x[j].w, d.y, acc[j][3].y);
-          acc[j][3].z = fmaf(x[j].w, d.z, acc[j][3].z); acc[j][3].w = fmaf(x[j].w, d.w, acc[j][3].w);
-        }
-        if (!more) break;
-        d = dn;
-#pragma unroll
-        for (int j = 0; j < KT; ++j) x[j] = xn[j];
-      }
-    }
-  }
-  for (int g = 0; g < RG; ++g) {
-    if (worker && rg == g) {
-#pragma unroll
-      for (int j = 0; j < KT; ++j)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          float* o = scr + ((size_t)(kg * KT + j) * cin + 4 * ci4 + i) * cout + 4 * co4;
-          if (g == 0) st4(o, acc[j][i]);
-          else st4(o, add4(ld4(o), acc[j][i]));
-        }
-    }
-    __syncthreads();
-  }
-  res_store(out, scr, (K * cin * cout) >> 2);
-  __syncthreads();
-}
-
-// Last phase: flat gradient = fixed-order sum of the G per-CTA partials (+ weight_decay * w), BatchNorm gradients from the
-// published sums, per-CTA sum of w^2 for the loss.  A float4 of parameters is owned by 8 consecutive lanes, each adding an
-// eighth of the records (all its loads in flight at once); the eighths meet through three shuffles in a fixed order.
-__device__ __noinline__ void res_grad_reduce(const ResProgram& P, const ResCall& c, int G, int cta, float* red) {
-  const int tid = threadIdx.x, sub = tid & 7;
-  const long long nq = P.n_train >> 2;                       // float4s
-  const long long per = (nq + G - 1) / G;
-  const long long q0 = (long long)cta * per, q1 = q0 + per < nq ? q0 + per : nq;
-  float w2 = 0.f;
-  const int fcseg = 3 * P.nconvs;
-  for (long long qb = q0; qb < q1; qb += kResThreads / 8) {
-    const long long q = qb + (tid >> 3);
-    const bool act = q < q1;
-    const long long pidx = q * 4;
-    // segment lookup: conv l -> (weights, beta, gamma), then fc, fc2 (tf.trainable_variables() order)
-    long long off = 0, numel = 0, stride = 0;
-    const float* part = nullptr;
-    int kind = 2;                                            // 0: partial sums + decay, 1: published BN sums (no decay), 2: decay only
-    if (act) {
-      for (int si = 0; si < fcseg + 2; ++si) {
-        if (si < fcseg) {
-          const RConv& L = P.conv[si / 3];
-          const int w = si % 3;
-          off = w == 0 ? L.w_off : (w == 1 ? L.beta_off : L.gamma_off);
-          numel = w == 0 ? (long long)L.k * L.cin * L.cout : L.cout;
-          part = w == 0 ? L.dwres : (w == 1 ? L.bsum : L.bsum + L.cout);
-          stride = numel;
-          kind = w == 0 ? 0 : 1;
-        } else if (si == fcseg) {
-          off = P.fc_off; numel = P.fc2_off - P.fc_off; part = P.dwfc_part; stride = numel; kind = 0;
-        } else {
-          off = P.fc2_off; numel = P.n_train - P.fc2_off; part = nullptr; stride = 0; kind = 2;
-        }
-        if (pidx >= off && pidx < off + numel) break;
-      }
-    }
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    const long long i = pidx - off;
-    if (act && kind == 0) {
-      const int per_sub = (G + 7) >> 3;                      // 148 records / 8 lanes = 19 loads: one batch, one L2 round trip
-      const int g_lo = sub * per_sub, g_hi = imin(G, g_lo + per_sub);
-      for (int g0 = g_lo; g0 < g_hi; g0 += 20) {
-        float4 v[20];
-#pragma unroll
-        for (int j = 0; j < 20; ++j)
-          v[j] = g0 + j < g_hi ? __ldcg(reinterpret_cast<const float4*>(part + (size_t)(g0 + j) * stride + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int j = 0; j < 20; ++j) s = add4(s, v[j]);
-      }
-    } else if (act && kind == 1 && sub == 0) {
-      s = __ldcg(reinterpret_cast<const float4*>(part + i));
-    }
-    // the eight lanes' sums meet in a fixed (butterfly) order
-#pragma unroll
-    for (int m = 1; m < 8; m <<= 1) {
-      s.x += __shfl_xor_sync(0xffffffffu, s.x, m); s.y += __shfl_xor_sync(0xffffffffu, s.y, m);
-      s.z += __shfl_xor_sync(0xffffffffu, s.z, m); s.w += __shfl_xor_sync(0xffffffffu, s.w, m);
-    }
-    if (act && sub == 0) {
-      if (kind != 1) {
-        const float4 w = ld4(c.params + pidx);
-        s.x = fmaf(c.weight_decay, w.x, s.x); s.y = fmaf(c.weight_decay, w.y, s.y);
-        s.z = fmaf(c.weight_decay, w.z, s.z); s.w = fmaf(c.weight_decay, w.w, s.w);
-        w2 += w.x * w.x + w.y * w.y + w.z * w.z + w.w * w.w;
-      }
-      st4(c.grads + pidx, s);
-    }
-  }
-  w2 = warp_sum(w2);
-  if ((tid & 31) == 0) red[tid >> 5] = w2;
-  __syncthreads();
-  if (tid == 0) {
-    float s = 0.f;
-    for (int i = 0; i < kResThreads / 32; ++i) s += red[i];
-    P.l2part[cta] = s;
-  }
 }
 
 __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __grid_constant__ ResProgram P, const __grid_constant__ ResCall c) {
@@ -1032,23 +869,15 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
       __syncthreads();
       res_stamp(c, slot + 1);
       res_bwd_epilogue(smem + P.b_pl, rcap, Lb.bks, R, C, nullptr, 1, ypr, tblr + La.tbl, nullptr, nullptr, nullptr, smem + P.b_g[gi_a],
-                       c.dw_inside ? nullptr : La.g + (size_t)u0 * B.t * C, ysr, P.b_ys_cap, La.brec + (size_t)cta * 2 * C, nullptr);
+                       La.g + (size_t)u0 * B.t * C, ysr, P.b_ys_cap, La.brec + (size_t)cta * 2 * C, nullptr);
       res_stamp(c, slot + 2);
       gbar_arrive(P.bar);
       target += (unsigned)G;
-      // ---- nobody waits for the rest of this phase ----
-      // x_a = relu(bn_a(y_a)) as the padded input tile of conv_b (aliases the dx planes, which are dead)
-      const int TPx = Lb.pad_left + B.t + Lb.pad_right;
-      if (c.dw_inside) {
-        res_stage(ypr, tblr + La.tbl, smem + P.b_pl, Ue, B.t, C, TPx, C, Lb.pad_left, Lb.pad_right);
-        __syncthreads();
-      }
-      // next phase (conv_a): its tensors travel during this layer's weight gradient; the bank region doubles as the
-      // weight-gradient scratch, so the TMA of the next bank(s) goes out after it
+      // ---- nobody waits for the rest of this phase: the next phase's (conv_a) tensors and bank(s) travel during the barrier ----
       const int Ca = La.cin, Rin = Ue * La.t_in;
       res_fetch(ysr, La.y + (size_t)u0 * B.t * C, R * (C >> 2));
       if (Dd) res_fetch(ysr + P.umax * B.t * C, Dd->y + (size_t)u0 * B.t * C, R * (C >> 2));
-      {                                 // y / out of the layer(s) below into ypr (y_a there has been consumed into x_a)
+      {                                 // y / out of the layer(s) below into ypr (the epilogue has consumed y_a)
         const int n4 = Rin * (Ca >> 2), cap = P.umax * La.t_in * Ca;
         if (bi > 0) {
           const RBlock& Bp = P.blk[bi - 1];
@@ -1058,7 +887,6 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
           res_fetch(ypr, P.conv[0].y + (size_t)u0 * La.t_in * Ca, n4);
         }
       }
-      if (c.dw_inside) res_dw<9>(smem, P.b_pl, TPx, C, P.b_dys, TPd, PLd, COS, Ue, C, C, 1, B.t, smem + P.b_w, Lb.dwres + (size_t)cta * 9 * C * C);
       res_load_bank(smem + P.b_w, La.wT, (unsigned)(La.k * La.cin * La.cout), Dd ? Dd->wT : nullptr, Dd ? (unsigned)(Dd->cin * Dd->cout) : 0u, wbar);
       res_stamp(c, slot + 3);
       gbar_wait(P.bar, target);
@@ -1090,46 +918,23 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
         const RConv& Lpb = P.conv[Bp.b];
         const RConv* Lpd = Bp.down >= 0 ? &P.conv[Bp.down] : nullptr;
         res_bwd_epilogue(smem + P.b_pl, rcap, La.bks, Rin, Ca, gid, 2, ypr, tblr + Lpb.tbl, Lpd ? nullptr : ypr + cap, Lpd ? ypr + cap : nullptr,
-                         Lpd ? tblr + Lpd->tbl : nullptr, smem + P.b_g[gi_n], c.dw_inside ? nullptr : Bp.gblk + (size_t)u0 * La.t_in * Ca, ysr,
+                         Lpd ? tblr + Lpd->tbl : nullptr, smem + P.b_g[gi_n], Bp.gblk + (size_t)u0 * La.t_in * Ca, ysr,
                          P.b_ys_cap, Lpb.brec + (size_t)cta * 2 * Ca,
                          Lpd ? Lpd->brec + (size_t)cta * 2 * Ca : nullptr);
       } else {
         res_bwd_epilogue(smem + P.b_pl, rcap, La.bks, Rin, Ca, gid, 1, ypr, tblr + P.conv[0].tbl, nullptr, nullptr, nullptr, smem + P.b_g[gi_n],
-                         c.dw_inside ? nullptr : P.conv[0].g + (size_t)u0 * La.t_in * Ca, ysr, P.b_ys_cap, P.conv[0].brec + (size_t)cta * 2 * Ca,
+                         P.conv[0].g + (size_t)u0 * La.t_in * Ca, ysr, P.b_ys_cap, P.conv[0].brec + (size_t)cta * 2 * Ca,
                          nullptr);
       }
       res_stamp(c, slot + 2);
       gbar_arrive(P.bar);
       target += (unsigned)G;
-      // ---- weight gradients of conv_a and the shortcut conv: X = block input as conv_a's padded tile (aliases the planes) ----
-      const int TPx = La.pad_left + La.t_in + La.pad_right;
-      if (!c.dw_inside) {
-        // mode 3: the grouped launch computes the weight gradients from the stored layer gradients
-      } else if (bi > 0 && P.blk[bi - 1].down >= 0) {
-        const RBlock& Bp = P.blk[bi - 1];
-        res_block_out(ypr, tblr + P.conv[Bp.b].tbl, ypr + cap, tblr + P.conv[Bp.down].tbl, nullptr, 0, 0, 0, smem + P.b_pl, Ue, La.t_in, Ca, TPx, Ca,
-                      La.pad_left, La.pad_right, nullptr);
-      } else if (bi > 0) {
-        res_stage(ypr + cap, nullptr, smem + P.b_pl, Ue, La.t_in, Ca, TPx, Ca, La.pad_left, La.pad_right);
-      } else {
-        res_stage(ypr, tblr + P.conv[0].tbl, smem + P.b_pl, Ue, La.t_in, Ca, TPx, Ca, La.pad_left, La.pad_right);
-      }
-      __syncthreads();
-      // the next phase's tensors travel during the weight gradients (ysr and ypr are dead)
+      // ---- nobody waits for the rest of this phase: the next phase's tensors (ysr and ypr are dead) and bank travel ----
       if (bi > 0) {
         const RBlock& Bp = P.blk[bi - 1];
-        res_fetch(ysr, P.conv[Bp.b].y + (size_t)u0 * Bp.t * Bp.c, Ue * Bp.t * (Bp.c >> 2));
+        const RConv& Lpb = P.conv[Bp.b];
+        res_fetch(ysr, Lpb.y + (size_t)u0 * Bp.t * Bp.c, Ue * Bp.t * (Bp.c >> 2));
         res_fetch(ypr, P.conv[Bp.a].y + (size_t)u0 * Bp.t * Bp.c, Ue * Bp.t * (Bp.c >> 2));
-      } else if (c.dw_inside) {         // last phase: conv0's y and its input, the features
-        const RConv& L0 = P.conv[0];
-        res_fetch(ysr, L0.y + (size_t)u0 * La.t_in * Ca, Rin * (Ca >> 2));
-        res_fetch(ypr, c.feat + (size_t)u0 * L0.t_in * L0.cin, Ue * L0.t_in * (L0.cin >> 2));
-      }
-      if (c.dw_inside) res_dw<9>(smem, P.b_pl, TPx, Ca, P.b_dys, TPd, PLd, COS, Ue, Ca, C, S, B.t, smem + P.b_w, La.dwres + (size_t)cta * 9 * Ca * C);
-      if (Dd && c.dw_inside)            // 1x1 / stride 2, no padding: x row = pad_left + 2 t
-        res_dw<1>(smem, P.b_pl + La.pad_left * Ca, TPx, Ca, P.b_dyd, B.t, 0, COS, Ue, Ca, C, 2, B.t, smem + P.b_w, Dd->dwres + (size_t)cta * Ca * C);
-      if (bi > 0) {
-        const RConv& Lpb = P.conv[P.blk[bi - 1].b];
         res_load_bank(smem + P.b_w, Lpb.wT, (unsigned)(Lpb.k * Lpb.cin * Lpb.cout), nullptr, 0u, wbar);
       }
       res_stamp(c, slot + 3);
@@ -1151,25 +956,6 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
       const int t = gi_b; gi_b = gi_n; gi_n = t;               // the produced gradient is the next block's gblk
     }
   }
-  // =============== conv0's weight gradient (no input gradient), then the gradient reduction ===============
-  if (c.dw_inside) {
-    const RConv& L0 = P.conv[0];
-    const int C = L0.cout, COS = chan_stride(C), TPx = L0.pad_left + L0.t_in + L0.pad_right;
-    cp_async_wait_all();
-    __syncthreads();
-    res_dy_stage(smem + P.b_g[gi_b], ysr, tblr + L0.tbl, bsr + L0.bs, 1.0f / ((float)c.n * (float)L0.t_out), 0, smem + P.b_dys, Ue, L0.t_out, C,
-                 L0.t_out, 0, COS);
-    const int xt = P.b_w + ((3 * L0.cin * C + 3) & ~3);      // no bank is needed any more: scratch first, the tile behind it
-    res_stage(ypr, nullptr, smem + xt, Ue, L0.t_in, L0.cin, TPx, L0.cin, L0.pad_left, L0.pad_right);
-    __syncthreads();
-    res_dw<3>(smem, xt, TPx, L0.cin, P.b_dys, L0.t_out, 0, COS, Ue, L0.cin, C, 1, L0.t_out, smem + P.b_w, L0.dwres + (size_t)cta * 3 * L0.cin * C);
-    res_stamp(c, 29);
-    gbar_arrive(P.bar);
-    target += (unsigned)G;
-    gbar_wait(P.bar, target);
-    res_stamp(c, 30);
-    res_grad_reduce(P, c, G, cta, red);
-  }
   res_stamp(c, 31);
 }
 
@@ -1181,7 +967,7 @@ struct ResidentState {
   size_t smem_f = 0, smem_b = 0;
   int grid_max = 0;                  // CTAs that can be co-resident (one per SM)
   int umax = 0;
-  int mode = 0;                      // 0 off, 1 forward only, 2 forward + backward
+  int mode = kResidentOff;           // which kernels of the step run resident (ResidentMode)
   unsigned bar_next = 0;             // value the arrival counter will have when the next launch starts
 };
 
@@ -1229,12 +1015,14 @@ static ResidentState* resident_state(tcr_handle* h) {
   if (h->resident) return (ResidentState*)h->resident;
   ResidentState* S = new ResidentState();
   h->resident = S;
-  // default 3: the weight-gradient FMA loops of mode 2 run 16 warps per SM where the grouped launch runs two CTAs per SM, and
-  // mode 2 loses to it; mode 3 is ahead of mode 1 by the backward-data launches it saves.
-  int want = 3;
-  if (const char* e = getenv("TCR_RESIDENT")) want = atoi(e);
-  if (h->sync_bn) want = 0;          // SyncBN lives in the per-layer kernels' launch sequence (NCCL between launches)
-  if (want <= 0) return S;
+  // default: both resident kernels, ahead of the resident forward alone by the backward-data launches they save
+  int want = kResidentFwdBwdData;
+  if (const char* e = getenv("TCR_RESIDENT")) {
+    const int v = atoi(e);
+    if (v == kResidentOff || v == kResidentFwd) want = v;
+  }
+  if (h->sync_bn) want = kResidentOff;   // SyncBN lives in the per-layer kernels' launch sequence (NCCL between launches)
+  if (want == kResidentOff) return S;
   int sms = 3;                       // emulator: a few CTAs exercise ragged ownership
 #ifndef TCR_EMU
   int dev = 0, coop = 0;
@@ -1266,7 +1054,6 @@ static ResidentState* resident_state(tcr_handle* h) {
     bs += 2 * cv.cout;
     if (cv.cout > kResThreads / 2) return S;                       // single-pass statistics need 2C <= blockDim
     if (cv.k != 9 && cv.k != 3 && cv.k != 1) return S;
-    if ((cv.cin / 4) * (cv.cout / 4) * (cv.k >= 3 ? cv.k / 3 : 1) > kResThreads && want == 2) want = 3;   // weight-gradient tiles of one CTA: grouped launch instead
   }
   if (h->convs[0].k != 3) return S;
   for (int b = 0; b < P.nblocks; ++b) {
@@ -1328,38 +1115,33 @@ static ResidentState* resident_state(tcr_handle* h) {
   }
   // ---------------- backward layout ----------------
   {
-    int gmax = 0, ysmax = 0, ypmax = 0, dysmax = 0, dydmax = 0, plmax = 0;
+    int ysmax = 0, ypmax = 0, dysmax = 0, dydmax = 0, plmax = 0;
     for (size_t b = 0; b < h->blocks.size(); ++b) {
       const BlockPlan& bp = h->blocks[b];
       const ConvPlan& ca = h->convs[bp.a];
       const ConvPlan& cb = h->convs[bp.b];
       const int C = bp.c, COS = chan_stride(C), rows = umax * bp.t;
-      gmax = std::max(gmax, std::max(rows * C, umax * ca.t_in * ca.cin));
       ysmax = std::max(ysmax, rows * C * (bp.down >= 0 ? 2 : 1));
       ypmax = std::max(ypmax, std::max(rows * C, umax * ca.t_in * ca.cin * (b > 0 ? 2 : 1)));
       // phase Bb
       dysmax = std::max(dysmax, umax * (8 + bp.t + cb.pad_left) * COS);
-      const int prb = std::max((cb.t_out - 1) + cb.k - cb.pad_left - cb.t_in, 0);
-      plmax = std::max(plmax, std::max(P.conv[bp.b].bks * rows * C, umax * (cb.pad_left + bp.t + prb) * C));
+      plmax = std::max(plmax, P.conv[bp.b].bks * rows * C);
       // phase Ba
       const int S_ = ca.stride, PLd = 8 / S_, PRd = std::max(0, (ca.t_in - 1 + ca.pad_left) / S_ - (ca.t_out - 1));
       dysmax = std::max(dysmax, umax * (PLd + bp.t + PRd) * COS);
       if (bp.down >= 0) dydmax = std::max(dydmax, rows * COS);
-      const int pra = std::max((ca.t_out - 1) * ca.stride + ca.k - ca.pad_left - ca.t_in, 0);
-      plmax = std::max(plmax, std::max(P.conv[bp.a].bks * umax * ca.t_in * ca.cin, umax * (ca.pad_left + ca.t_in + pra) * ca.cin));
+      plmax = std::max(plmax, P.conv[bp.a].bks * umax * ca.t_in * ca.cin);
     }
+    // conv0's rows and the input features are never staged here, but these sizes decide which shapes fit the kernel: without
+    // them TCResNet14-1.0 at N=512 (T=49) would move from the per-layer backward-data kernels to this one.
     const ConvPlan& c0 = h->convs[0];
-    gmax = std::max(gmax, umax * c0.t_out * c0.cout);
     ysmax = std::max(ysmax, umax * c0.t_out * c0.cout);
     ypmax = std::max(ypmax, umax * c0.t_in * c0.cin);
     dysmax = std::max(dysmax, umax * c0.t_out * chan_stride(c0.cout));
-    // conv0's input tile (last phase) goes into the bank region, which holds no bank then
-    const int c0tile = umax * (c0.pad_left + c0.t_in + std::max((c0.t_out - 1) + c0.k - c0.pad_left - c0.t_in, 0)) * c0.cin;
-    wmax = std::max(wmax, (int)c0.wnumel() + 4 + c0tile);
     int o = 4;
     P.b_w = o; o += al(wmax);
     ysmax = std::max(ysmax, 1024);                                 // epilogue scratch [4][nseg][C] lives here
-    plmax = std::max(plmax, red_floats);                           // record sums / gradient reduction scratch alias the (then dead) planes
+    plmax = std::max(plmax, red_floats);                           // the record sums' scratch aliases the (then dead) planes
     P.b_ys = o; o += al(ysmax);
     P.b_ys_cap = al(ysmax);
     P.b_yp = o; o += al(ypmax);
@@ -1376,7 +1158,6 @@ static ResidentState* resident_state(tcr_handle* h) {
         gsz[gn] = std::max(gsz[gn], umax * ca.t_in * ca.cin);
         std::swap(gb, gn);
       }
-      (void)gmax;
       for (int i = 0; i < 3; ++i) { P.b_g[i] = o; o += al(gsz[i]); }
     }
     P.b_tbl = o; o += al(tbl);
@@ -1386,13 +1167,12 @@ static ResidentState* resident_state(tcr_handle* h) {
   }
   S->umax = umax;
   P.bar = h->d_gridbar;
-  P.fc_off = h->fc_off; P.fc2_off = h->fc2_off; P.n_train = h->n_train;
-  P.loss_part = h->d_loss_part; P.dwfc_part = h->d_dwfc_part; P.l2part = h->d_l2part;
+  P.fc_off = h->fc_off;
+  P.loss_part = h->d_loss_part; P.dwfc_part = h->d_dwfc_part;
   const BlockPlan& lb = h->blocks.back();
   P.gout = lb.gblk;
   P.bpartb = h->convs[lb.b].bpart;
   P.bpartd = lb.down >= 0 ? h->convs[lb.down].bpart : nullptr;
-  if ((h->n_train & 3) || (h->fc_off & 3) || (h->fc2_off & 3)) want = std::min(want, 1);
 #ifndef TCR_EMU
   if (S->smem_f > 227 * 1024) return S;
   // the opt-in limit is a property of the FUNCTION, shared by every handle of the process: it is only ever raised
@@ -1400,25 +1180,15 @@ static ResidentState* resident_state(tcr_handle* h) {
   if (optin_f.ensure(resident_fwd_kernel, S->smem_f) != cudaSuccess) return S;
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resident_fwd_kernel, kResThreads, S->smem_f) != cudaSuccess || per_sm < 1) return S;
-  if (want >= 2) {
+  if (want == kResidentFwdBwdData) {
     if (S->smem_b > 227 * 1024 ||
         optin_b.ensure(resident_bwd_kernel, S->smem_b) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resident_bwd_kernel, kResThreads, S->smem_b) != cudaSuccess || per_sm < 1)
-      want = 1;
+      want = kResidentFwd;
   }
 #endif
-  if (want == 2) {                   // per-CTA weight-gradient partials
-    for (int l = 0; l < P.nconvs; ++l) {
-      void* q = nullptr;
-      const size_t bytes = (size_t)sms * h->convs[l].wnumel() * sizeof(float);
-      if (cudaMalloc(&q, bytes) != cudaSuccess) { want = 1; break; }
-      h->allocs.push_back(q);
-      h->workspace_bytes += (int64_t)bytes;
-      P.conv[l].dwres = (float*)q;
-    }
-  }
   S->grid_max = sms;
-  S->mode = want >= 3 ? 3 : (want == 2 ? 2 : 1);
+  S->mode = want;
   if (getenv("TCR_RESIDENT_VERBOSE")) {
     fprintf(stderr, "[tcr] resident mode %d, umax %d, smem fwd %zu B, bwd %zu B\n", S->mode, umax, S->smem_f, S->smem_b);
     for (int l = 0; l < P.nconvs; ++l)
@@ -1433,8 +1203,8 @@ void resident_destroy(tcr_handle* h) {
   h->resident = nullptr;
 }
 
-// 0: per-layer kernels; 1: the training forward runs as the resident kernel; 2: forward and backward do (the activations of
-// ceil(max_batch / #SMs) utterances and the largest filter bank fit in one SM's shared memory).
+// The resident kernels run where the activations of ceil(max_batch / #SMs) utterances and the largest filter bank fit in one
+// SM's shared memory; see resident_state for what TCR_RESIDENT and SyncBN select.
 int resident_mode(tcr_handle* h) { return resident_state(h)->mode; }
 
 static int res_launch(tcr_handle* h, const char* name, void (*kernel)(const ResProgram, const ResCall), int G, size_t smem, const ResCall& c,
@@ -1469,7 +1239,6 @@ static ResCall res_call(tcr_handle* h, const float* feat, const tcr_step_args* a
   c.logits = a->logits ? a->logits : h->d_logits;
   c.probs = a->probs ? a->probs : h->d_probs;
   c.n = a->n; c.inv_n = 1.0f / (float)a->n;
-  c.weight_decay = a->weight_decay;
   c.tl = h->d_timeline;
   return c;
 }
@@ -1491,29 +1260,12 @@ int resident_forward(tcr_handle* h, const float* feat, const tcr_step_args* a, c
   return res_launch(h, "resident_fwd", resident_fwd_kernel, G, S->smem_f, c, s);
 }
 
-// Backward-data chain, all weight gradients and the gradient reduction (+ weight decay, sum of w^2): leaves the flat gradient in
-// `grads` and the published BatchNorm-backward sums, i.e. what net_backward + grad_finalize leave.  *l2_records: entries of l2part.
-int resident_backward(tcr_handle* h, const float* feat, const tcr_step_args* a, float* grads, int* l2_records, cudaStream_t s) {
-  ResidentState* S = resident_state(h);
-  const int G = std::min(S->grid_max, a->n);
-  ResCall c = res_call(h, feat, a);
-  c.grads = grads;
-  c.tl = h->d_timeline ? h->d_timeline + 148 * 32 : nullptr;
-  c.dw_inside = 1;
-  c.bar_base = S->bar_next;
-  S->bar_next += (unsigned)G * (unsigned)(2 * h->blocks.size() + 1);
-  *l2_records = G;
-  return res_launch(h, "resident_bwd", resident_bwd_kernel, G, S->smem_b, c, s);
-}
-
-// Mode 3: the backward-data chain alone as the resident kernel.  It leaves every layer's masked gradient (ConvPlan::g,
-// BlockPlan::gblk) and the published BatchNorm-backward sums, i.e. what the conv_bwd_data launches of net_backward leave.
+// The backward-data chain as the resident kernel.  It leaves every layer's masked gradient (ConvPlan::g, BlockPlan::gblk) and
+// the published BatchNorm-backward sums, i.e. what the conv_bwd_data launches of net_backward_data leave.
 int resident_backward_data(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s) {
   ResidentState* S = resident_state(h);
   const int G = std::min(S->grid_max, a->n);
   ResCall c = res_call(h, feat, a);
-  c.grads = nullptr;
-  c.dw_inside = 0;
   c.tl = h->d_timeline ? h->d_timeline + 148 * 32 : nullptr;
   c.bar_base = S->bar_next;
   S->bar_next += (unsigned)G * (unsigned)(2 * h->blocks.size());

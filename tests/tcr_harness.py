@@ -7,6 +7,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 import subprocess
+from collections import Counter
 
 import numpy as np
 
@@ -221,6 +222,18 @@ class Engine:
         L.check(self.lib, self.lib.tcr_workspace_tensor(self.h, name.encode(), C.byref(p), C.byref(numel)),
                 f"tcr_workspace_tensor({name})")
         return self.b.view(p.value, numel.value)
+
+
+def launched(lib, fn):
+    """Kernel launches of one call, {name: count}, from the library's launch profiler (CUDA build only)."""
+    L.check(lib, lib.tcr_profile_enable(1), "tcr_profile_enable")
+    try:
+        fn()
+        stats, count = C.POINTER(L.TcrKernelStat)(), C.c_int32()
+        L.check(lib, lib.tcr_profile_read(C.byref(stats), C.byref(count)), "tcr_profile_read")
+        return Counter({stats[i].name.decode(): int(stats[i].launches) for i in range(count.value)})
+    finally:
+        lib.tcr_profile_enable(0)
 
 
 def rel_err(a, ref):

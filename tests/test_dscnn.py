@@ -7,7 +7,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import dscnn_oracle as D
-from tcr_harness import rel_err
+from tcr_harness import launched, rel_err
 from tcresnet_b200 import _lib as L
 
 
@@ -134,19 +134,6 @@ def expected_kernels(size, h, w, mode):
     else:
         conv, block = S_KERNELS[h, w][mode == "1"]
     return ["dscnn_" + conv] + ["dscnn_" + block] * (NLAYERS[size] - 1)
-
-
-def launched(lib, fn):
-    """Kernel launches of one call, {name: count}, from the library's launch profiler (CUDA build only)."""
-    from collections import Counter
-    L.check(lib, lib.tcr_profile_enable(1), "tcr_profile_enable")
-    try:
-        fn()
-        stats, count = C.POINTER(L.TcrKernelStat)(), C.c_int32()
-        L.check(lib, lib.tcr_profile_read(C.byref(stats), C.byref(count)), "tcr_profile_read")
-        return Counter({stats[i].name.decode(): int(stats[i].launches) for i in range(count.value)})
-    finally:
-        lib.tcr_profile_enable(0)
 
 
 def features(kind, n, h, w, seed=3):

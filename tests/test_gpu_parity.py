@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from parity_cases import run_case, perturbed_variables
-from tcr_harness import Engine, rel_err
+from tcr_harness import Engine, launched, rel_err
 from oracle import tcr_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -28,14 +28,40 @@ def test_cuda_path_matches_oracle(backend, kw):
     run_case(backend, **kw)
 
 
-@pytest.mark.parametrize("mode", ["0", "1", "2", "3"])
+def step_launches(backend, model, n):
+    """Kernel names of one training step on a handle sized for n utterances (each handle picks its resident mode)."""
+    spec = O.build_spec(model, 1.0, 49)
+    pv, mv = O.init_variables(spec, 0)
+    pf, mf = O.flatten_vars(spec, pv).astype(np.float32), O.flatten_moving(spec, mv).astype(np.float32)
+    wav, onehot = O.synthetic_batch(n)
+    eng = Engine(backend, model=int(model[len("TCResNet"):]), max_batch=n, dropout_keep_prob=0.5)
+    try:
+        return set(launched(backend.lib, lambda: eng.train_step(wav, onehot, pf, np.zeros_like(pf), mf)))
+    finally:
+        eng.close()
+
+
+@pytest.mark.parametrize("mode", ["0", "1", "3"])
 def test_resident_kernels_match_oracle(backend, monkeypatch, mode):
-    """TCR_RESIDENT = 0 / 1 / 2: per-layer kernels, resident forward kernel, resident forward + backward kernels
-    (csrc/tcr_resident.cu): every combination meets the same bounds, including the headline shape (4 utterances per SM)."""
+    """TCR_RESIDENT = 0: per-layer kernels; 1: resident forward kernel, per-layer backward-data kernels; 3 (the default): resident
+    forward and backward-data kernels (csrc/tcr_resident.cu).  Every mode meets the same bounds, including the headline shape
+    (4 utterances per SM), and the launch profiler shows that each shape ran the kernels of the mode asked for."""
     monkeypatch.setenv("TCR_RESIDENT", mode)
     run_case(backend, model="TCResNet8", wm=1.0, window=640, stride=320, n=64, keep=0.5, steps=2)
     run_case(backend, model="TCResNet8", wm=1.0, window=640, stride=320, n=512, keep=0.5, force_masks=True)
     run_case(backend, model="TCResNet14", wm=1.0, window=640, stride=320, n=33, keep=1.0)
+    for model, n in (("TCResNet8", 64), ("TCResNet8", 512), ("TCResNet14", 33)):
+        names = step_launches(backend, model, n)
+        fwd, dx = any(k.startswith("fwd:") for k in names), any(k.startswith("dx:") for k in names)
+        if mode == "0":
+            assert {"weight_transpose", "dw_grouped", "grad_finalize", "update"} <= names and fwd and dx, (model, n, names)
+            assert not {"resident_fwd", "resident_bwd_data"} & names, (model, n, names)
+        elif mode == "1":
+            assert {"resident_fwd", "dw_grouped", "grad_finalize", "update"} <= names and dx and not fwd, (model, n, names)
+            assert "resident_bwd_data" not in names, (model, n, names)
+        else:
+            assert {"resident_fwd", "resident_bwd_data", "dw_grouped", "grad_finalize", "update"} <= names, (model, n, names)
+            assert not fwd and not dx, (model, n, names)
 
 
 def test_log_mel_front_end_on_sm100a(backend):

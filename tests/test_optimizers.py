@@ -172,9 +172,9 @@ def test_emulated_update_matches_oracle_on_the_applied_gradient(emu, opt):
     print(opt["kind"], worst)
 
 
-@pytest.mark.parametrize("mode", ["0", "1", "2", "3"])
+@pytest.mark.parametrize("mode", ["0", "1", "3"])
 def test_emulated_resident_modes_and_gradient_only_steps(emu, monkeypatch, mode):
-    """TCR_RESIDENT = 0..3 all end in the same update launch: one Adam and one RMSProp step meet the bounds, and apply_update = 0
+    """TCR_RESIDENT = 0, 1 and 3 (the default) all end in the same update launch: one Adam and one RMSProp step meet the bounds, and apply_update = 0
     computes the gradient but leaves the parameters, both slots and the moving statistics untouched, bit for bit."""
     monkeypatch.setenv("TCR_RESIDENT", mode)
     for opt in (ADAM, RMSPROP):
@@ -364,7 +364,7 @@ def test_cuda_update_matches_oracle_tcresnet14x15_n1024(cuda, opt):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("mode", ["0", "1", "2", "3"])
+@pytest.mark.parametrize("mode", ["0", "1", "3"])
 def test_cuda_resident_modes(cuda, monkeypatch, mode):
     monkeypatch.setenv("TCR_RESIDENT", mode)
     run_optimizer_case(cuda, ADAM, n=64, steps=2)

@@ -21,11 +21,11 @@ print(run_case(b, model='TCResNet14', wm=1.5, window=480, stride=160, n=5, keep=
 print(run_case(b, model='TCResNet8', wm=1.0, n=9, keep=0.5))
 " > gpurun_out/sanitizer.txt 2>&1 ; echo "sanitizer rc=$?" | tee -a gpurun_out/sanitizer.txt
   tail -5 gpurun_out/sanitizer.txt
-  # shared-memory races and divergent barriers: one TC-ResNet step (default kernels), one with the resident backward kernel, and
-  # the DS-CNN forward (mbarrier / TMA / wgmma pipeline); racecheck serialises heavily, so the cases are tiny
+  # shared-memory races and divergent barriers: one TC-ResNet step on the default kernels (resident forward and backward-data,
+  # grouped weight gradients) and the DS-CNN forward (mbarrier / TMA / wgmma pipeline); racecheck serialises heavily, so the cases are tiny
   for tool in racecheck synccheck; do
     echo "== compute-sanitizer --tool $tool"
-    TCR_RESIDENT=2 timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python -c "
+    timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python -c "
 import sys; sys.path.insert(0,'tests'); sys.path.insert(0,'.')
 from tcr_harness import TorchBackend
 from parity_cases import run_case

@@ -14,7 +14,7 @@ timeout 900 ncu --set full --clock-control none --import-source on --kernel-name
 timeout 600 ncu --set full --clock-control none --import-source on --kernel-name-base demangled -k regex:dscnn -s 12 -c 6 -o $O/dscnn python bench.py --workload dscnn --steps 3 --warmup 3 > $O/ncu_dscnn.log 2>&1; echo "ncu dscnn rc=$?"
 TCR_DSCNN_TC=0 timeout 600 ncu --metrics gpu__time_duration.sum,sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active,sm__inst_executed_pipe_fma.avg.pct_of_peak_sustained_active --clock-control none --kernel-name-base demangled -k regex:dscnn -s 12 -c 6 --csv --log-file $O/dscnn_fma.csv python bench.py --workload dscnn --steps 3 --warmup 3 > $O/ncu_dscnn_fma.log 2>&1; echo "ncu dscnn fma rc=$?"
 for tool in memcheck racecheck synccheck; do
-  TCR_RESIDENT=2 timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python -c "
+  timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python -c "
 import sys; sys.path.insert(0,'tests'); sys.path.insert(0,'.')
 from tcr_harness import TorchBackend
 from parity_cases import run_case

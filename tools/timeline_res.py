@@ -2,7 +2,7 @@
 relative to the earliest CTA start of that kernel, and min / max over CTAs.
 forward slots: 0 start; per phase ph<3 at 1+8ph: +0 bank ready, +1 fma done, +2 stats done (arrive), +3 y stored, +4 barrier passed,
 +5 tables built, +6 next tile staged; 31 end.   backward slots: 0 start; per phase (Bb2,Ba2,Bb1,Ba1,Bb0,Ba0) at 1+5i: +0 inputs landed,
-+1 convT done, +2 epilogue done (arrive), +3 dW + prefetch issued, +4 barrier passed; 29 dW0 done, 30 final barrier, 31 end."""
++1 convT done, +2 epilogue done (arrive), +3 prefetch issued, +4 barrier passed; 31 end."""
 import os, sys, ctypes as C
 import numpy as np, torch
 os.environ["TCR_DEBUG_TIMELINE"] = "1"
