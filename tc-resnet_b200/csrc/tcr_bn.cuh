@@ -164,26 +164,70 @@ __device__ __forceinline__ void cluster_publish(const PubSeg (&seg)[NSEG], int v
   cluster_sync_all();               // nobody exits (and releases its shared memory) while a peer may still read it
 }
 
+// ---- record sums and their per-channel finalisation, shared by the per-layer and the resident kernels ----------------------
+__device__ __forceinline__ float rec_ld(const float* p, float) { return __ldcg(p); }
+__device__ __forceinline__ float4 rec_ld(const float* p, float4) { return __ldcg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float rec_add(float a, float b) { return a + b; }
+__device__ __forceinline__ float4 rec_add(float4 a, float4 b) { return add4(a, b); }
+
+// Sum of records ch, ch + nch, ch + 2 nch, ... < G of column `col` (V = float) or of the four columns from `col` (V = float4) of
+// records `stride` floats apart, in a fixed order; DEPTH loads of a thread are in flight at once.
+template <class V, int DEPTH>
+__device__ __forceinline__ V rec_column_sum(const float* p, int col, int stride, int ch, int nch, int G) {
+  V s = V{};
+  for (int g0 = ch; g0 < G; g0 += DEPTH * nch) {
+    V v[DEPTH];
+#pragma unroll
+    for (int j = 0; j < DEPTH; ++j) {
+      const int g = g0 + j * nch;
+      v[j] = g < G ? rec_ld(p + (size_t)g * stride + col, V{}) : V{};
+    }
+#pragma unroll
+    for (int j = 0; j < DEPTH; ++j) s = rec_add(s, v[j]);
+  }
+  return s;
+}
+
+// One BatchNorm channel from the nch chunk sums of its (sum y, sum y^2) at scratch[ch * cols + col + {0,1}]: mean, variance and
+// rstd in fp64, the table entry tbl[4][C] (mean, rstd, gamma * rstd, beta) and, with `publish`, the global table and variance.
+__device__ __forceinline__ void bn_channel_finalize(const float* scratch, int cols, int col, int nch, float inv_m, float eps, float gamma,
+                                                    float beta, int C, int c, float* tbl, float* bnf, float* var, bool publish) {
+  double s1 = 0.0, s2 = 0.0;
+  for (int ch = 0; ch < nch; ++ch) {
+    s1 += (double)scratch[ch * cols + col];
+    s2 += (double)scratch[ch * cols + col + 1];
+  }
+  const double mean = s1 * (double)inv_m;
+  double v = s2 * (double)inv_m - mean * mean;
+  if (v < 0.0) v = 0.0;
+  const double rstd = 1.0 / sqrt(v + (double)eps);
+  const float fm = (float)mean, fr = (float)rstd, fs = (float)((double)gamma * rstd);
+  tbl[c] = fm; tbl[C + c] = fr; tbl[2 * C + c] = fs; tbl[3 * C + c] = beta;
+  if (publish) {
+    bnf[c] = fm; bnf[C + c] = fr; bnf[2 * C + c] = fs; bnf[3 * C + c] = beta;
+    var[c] = (float)v;
+  }
+}
+
+// One BatchNorm-backward sum (record column j = c*2 + q) from its nch chunk sums at scratch[ch * cols + i] -> sb[q][C] and, with
+// `publish`, the global bsum[q][C].
+__device__ __forceinline__ void bsum_finalize(const float* scratch, int cols, int i, int nch, int j, int C, float* sb, float* bsum, bool publish) {
+  double s = 0.0;
+  for (int ch = 0; ch < nch; ++ch) s += (double)scratch[ch * cols + i];
+  const float f = (float)s;
+  sb[(j & 1) * C + (j >> 1)] = f;
+  if (publish) bsum[(j & 1) * C + (j >> 1)] = f;
+}
+
 // Sum `gc` records of `cols` floats each: thread i < cols * nch takes column i % cols and records i / cols, + nch, ...
-// (loads batched 8 deep); the nch chunk sums land in scratch[chunk * cols + col].  Needs cols <= blockDim.x.
+// (loads batched kRecB deep); the nch chunk sums land in scratch[chunk * cols + col].  Needs cols <= blockDim.x.
 constexpr int kRecB = 32;          // records in flight per thread: one batch covers 32 records x column chunks
 __device__ __forceinline__ int records_sum(const float* part, int gc, int cols, float* scratch) {
   const int nch = imax(1, (int)blockDim.x / cols);
   const int i = threadIdx.x;
   if (i < cols * nch) {
     const int col = i % cols, ch = i / cols;
-    float s = 0.f;
-    for (int g0 = ch; g0 < gc; g0 += nch * kRecB) {
-      float v[kRecB];
-#pragma unroll
-      for (int j = 0; j < kRecB; ++j) {
-        const int g = g0 + j * nch;
-        v[j] = g < gc ? __ldcg(part + (size_t)g * cols + col) : 0.f;
-      }
-#pragma unroll
-      for (int j = 0; j < kRecB; ++j) s += v[j];
-    }
-    scratch[ch * cols + col] = s;
+    scratch[ch * cols + col] = rec_column_sum<float, kRecB>(part, col, cols, ch, nch, gc);
   }
   return nch;
 }
@@ -198,24 +242,8 @@ __device__ __forceinline__ void bn_table_build(const StatSrc& st, const float* b
   }
   const int nch = records_sum(st.cpart, st.gc, 2 * C, scratch);
   __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    double s1 = 0.0, s2 = 0.0;
-    for (int ch = 0; ch < nch; ++ch) {
-      s1 += (double)scratch[ch * 2 * C + 2 * c];
-      s2 += (double)scratch[ch * 2 * C + 2 * c + 1];
-    }
-    const double mean = s1 * (double)st.inv_m;
-    double var = s2 * (double)st.inv_m - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const double rstd = 1.0 / sqrt(var + (double)st.eps);
-    const float g = st.gamma[c], b = st.beta[c];
-    const float fm = (float)mean, fr = (float)rstd, fs = (float)((double)g * rstd);
-    tbl[c] = fm; tbl[C + c] = fr; tbl[2 * C + c] = fs; tbl[3 * C + c] = b;
-    if (publish) {
-      st.bnf[c] = fm; st.bnf[C + c] = fr; st.bnf[2 * C + c] = fs; st.bnf[3 * C + c] = b;
-      st.var[c] = (float)var;
-    }
-  }
+  for (int c = threadIdx.x; c < C; c += blockDim.x)
+    bn_channel_finalize(scratch, 2 * C, 2 * c, nch, st.inv_m, st.eps, st.gamma[c], st.beta[c], C, c, tbl, st.bnf, st.var, publish);
   __syncthreads();
 }
 
@@ -234,43 +262,16 @@ __device__ __forceinline__ void bn_table_build2(const StatSrc& sa, const float* 
   if (i < cols * nch) {
     const int col = i % cols, ch = i / cols;
     const bool second = col >= 2 * C;
-    const float* part = second ? sb.cpart : sa.cpart;
-    const int gc = second ? sb.gc : sa.gc, cc = second ? col - 2 * C : col;
-    float s = 0.f;
-    for (int g0 = ch; g0 < gc; g0 += nch * kRecB) {
-      float v[kRecB];
-#pragma unroll
-      for (int j = 0; j < kRecB; ++j) {
-        const int g = g0 + j * nch;
-        v[j] = g < gc ? __ldcg(part + (size_t)g * 2 * C + cc) : 0.f;
-      }
-#pragma unroll
-      for (int j = 0; j < kRecB; ++j) s += v[j];
-    }
-    scratch[ch * cols + col] = s;
+    const StatSrc& st = second ? sb : sa;
+    scratch[ch * cols + col] = rec_column_sum<float, kRecB>(st.cpart, second ? col - 2 * C : col, 2 * C, ch, nch, st.gc);
   }
   __syncthreads();
   for (int j = threadIdx.x; j < 2 * C; j += blockDim.x) {
     const bool second = j >= C;
     const int c = second ? j - C : j;
     const StatSrc& st = second ? sb : sa;
-    float* tbl = second ? tbl_b : tbl_a;
-    double s1 = 0.0, s2 = 0.0;
-    for (int ch = 0; ch < nch; ++ch) {
-      s1 += (double)scratch[ch * cols + (second ? 2 * C : 0) + 2 * c];
-      s2 += (double)scratch[ch * cols + (second ? 2 * C : 0) + 2 * c + 1];
-    }
-    const double mean = s1 * (double)st.inv_m;
-    double var = s2 * (double)st.inv_m - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const double rstd = 1.0 / sqrt(var + (double)st.eps);
-    const float g = st.gamma[c], b = st.beta[c];
-    const float fm = (float)mean, fr = (float)rstd, fs = (float)((double)g * rstd);
-    tbl[c] = fm; tbl[C + c] = fr; tbl[2 * C + c] = fs; tbl[3 * C + c] = b;
-    if (publish) {
-      st.bnf[c] = fm; st.bnf[C + c] = fr; st.bnf[2 * C + c] = fs; st.bnf[3 * C + c] = b;
-      st.var[c] = (float)var;
-    }
+    bn_channel_finalize(scratch, cols, (second ? 2 * C : 0) + 2 * c, nch, st.inv_m, st.eps, st.gamma[c], st.beta[c], C, c,
+                        second ? tbl_b : tbl_a, st.bnf, st.var, publish);
   }
   __syncthreads();
 }
@@ -284,20 +285,14 @@ __device__ __forceinline__ void bsum_build(const BsumSrc& bs, const float* bsum_
   }
   const int nch = records_sum(bs.cpart, bs.gc, 2 * C, scratch);
   __syncthreads();
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
-    double s = 0.0;
-    for (int ch = 0; ch < nch; ++ch) s += (double)scratch[ch * 2 * C + i];
-    const float f = (float)s;
-    sb[(i & 1) * C + (i >> 1)] = f;
-    if (publish) bs.bsum[(i & 1) * C + (i >> 1)] = f;
-  }
+  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) bsum_finalize(scratch, 2 * C, i, nch, i, C, sb, bs.bsum, publish);
   __syncthreads();
 }
 
 // Per-channel (sum y, sum y^2) of a [rows][C] shared-memory tile -> part_out[c*2 + {0,1}] (shared memory), ONE pass.
 // Requires C <= blockDim.x.  red: 2 * blockDim.x floats of scratch.  The cross-CTA combination is then a plain
 // fixed-order sum; var = E[y^2] - mean^2 is formed once per channel in fp64 (relative error ~1e-7 (1 + mean^2/var)).
-__device__ __forceinline__ void tile_stats(const float* tile, int rows, int C, float* red, float* /*unused*/, float* part_out) {
+__device__ __forceinline__ void tile_stats(const float* tile, int rows, int C, float* red, float* part_out) {
   const int tid = threadIdx.x;
   const int ns = imax(1, (int)blockDim.x / C);
   const int seg = tid / C, c = tid - seg * C;

@@ -53,7 +53,6 @@ struct FwdArgs {
   ActSrc shortcut;          // kind 2 only: raw prev activation / relu(bn(y_down))
   float* out_write;         // kind 2 only: materialised block output [N, t_in, cin]
   int n, U, t_in, cin;
-  int nvb;                  // CTAs with work; the launch grid is nvb rounded up to whole clusters
   // main conv
   const float* w; float* y; float* fpart;
   int cout, stride, t_out, pad_left, KS;
@@ -72,7 +71,6 @@ struct HeadArgs {
   ActSrc shortcut;          // raw / relu(bn(y_down))
   float* out_write;         // [N, T', C]
   int n, t, c, classes;
-  int nvb;                  // CTAs with work (grid = nvb rounded up to whole clusters)
   const float* wfc;         // [C, classes]
   const float* onehot;      // may be null (no loss, no backward)
   const float* mask;        // injected dropout mask or null
@@ -101,7 +99,6 @@ struct DySrc {              // dy = scale * (dz - s1/M - xhat * s2/M), dz option
 
 struct BwdDataArgs {
   int n, U;
-  int nvb;                  // CTAs with work (grid = nvb rounded up to whole clusters)
   int w_smem;               // 1: filter bank(s) staged in shared memory by one TMA bulk copy
   // conv whose input gradient we compute
   DySrc dy; const float* w; int cin, cout, k, stride, t_in, t_out, pad_left, KS;

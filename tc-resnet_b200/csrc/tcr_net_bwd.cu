@@ -14,31 +14,23 @@
 //   conv_bwd_weight_kernel<K> : dW[k,ci,co] = sum_rows x[row+k, ci] * dy[row, co]; each thread owns 2 ci x 4 co
 //                               x K taps in registers, CTAs split (co tile, row chunk); row-chunk partials are
 //                               reduced in a fixed order by the optimizer kernel (deterministic, no atomics).
-#include "tcr_bn.cuh"
+#include "tcr_layer.cuh"
 #include "tcr_net.h"
 
 namespace tcr {
 
 constexpr int TMB = 4;   // input rows per thread task (backward-data)
 
-__device__ __forceinline__ float dot4(float4 a, float4 b) { return fmaf(a.x, b.x, fmaf(a.y, b.y, fmaf(a.z, b.z, a.w * b.w))); }
-__device__ __forceinline__ float4 mask_pos4(float4 v, float4 z) {
-  return make_float4(z.x > 0.f ? v.x : 0.f, z.y > 0.f ? v.y : 0.f, z.z > 0.f ? v.z : 0.f, z.w > 0.f ? v.w : 0.f);
-}
-__device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
-
 // ------------------------------------------------------------------------------------------------
 // backward data
 // ------------------------------------------------------------------------------------------------
 template <int K, bool WSMEM>
-__device__ __forceinline__ void conv_bwd_data_body(const BwdDataArgs& a, const int vb, const int nvb, unsigned char* smem_raw,
-                                                   MbarCtx& mb) {
+__device__ __forceinline__ void conv_bwd_data_body(const BwdDataArgs& a, const int vb, unsigned char* smem_raw, MbarCtx& mb) {
   float* smem = reinterpret_cast<float*>(smem_raw);
   const int tid = threadIdx.x;
   const int S = a.stride;
   const int u0 = vb * a.U;
   const int Ue = imax(0, imin(a.U, a.n - u0));        // 0: a CTA that only pads the grid to whole clusters
-  (void)nvb;
   const int COS = chan_stride(a.cout);
   const int PLd = (K - 1) / S;
   const int PRd = imax(0, (a.t_in - 1 + a.pad_left) / S - (a.t_out - 1));
@@ -135,157 +127,15 @@ __device__ __forceinline__ void conv_bwd_data_body(const BwdDataArgs& a, const i
   if (WSMEM) { mbar_wait(bar, mb.parity); mb.parity ^= 1u; }
   __syncthreads();
 
-  // ---- transposed conv, one parity class of input rows at a time ----
-  // input row t belongs to class p = (t + pad_left) % S; it receives taps k = p + S m from dy row (t+pad_left-p)/S - m.
-  const int NCIG = a.cin >> 2;
-  int t0[2], np[2], nrt[2];
-  for (int p = 0; p < 2; ++p) {
-    t0[p] = ((p - a.pad_left) % S + S) % S;
-    np[p] = (p < S && t0[p] < a.t_in) ? (a.t_in - t0[p] + S - 1) / S : 0;
-    nrt[p] = (np[p] + TMB - 1) / TMB;
-  }
-  const int NRTU = nrt[0] + nrt[1];
-  const int NT0 = (K + S - 1) / S;
-  const int MPS = (NT0 + a.KS - 1) / a.KS;
-  const int ntasks = a.KS * Ue * NRTU * NCIG;
-  for (int task = tid; task < ntasks; task += kThreads) {
-    const int cig = task % NCIG;
-    int q = task / NCIG;
-    const int rtu = q % NRTU;
-    q /= NRTU;
-    const int u = q % Ue, ks = q / Ue;
-    const int p = rtu >= nrt[0] ? 1 : 0;
-    const int rt = rtu - p * nrt[0];
-    // 32-bit float offsets from the shared-memory base (LDS.128 + FFMA + integer adds in the inner loop)
-    int dyo[TMB], tt[TMB];
-#pragma unroll
-    for (int i = 0; i < TMB; ++i) {
-      const int j = imin(rt + i * nrt[p], np[p] - 1);   // rows of a task are nrt apart: adjacent lanes -> adjacent rows
-      tt[i] = t0[p] + S * j;
-      const int b = (tt[i] + a.pad_left - p) / S;
-      dyo[i] = dys_off + (u * TPd + PLd + b) * COS;
-    }
-    float4 acc[TMB];
-#pragma unroll
-    for (int i = 0; i < TMB; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int NT = (K - p + S - 1) / S;
-    const int m_lo = ks * MPS, m_hi = imin(NT, m_lo + MPS);
-    for (int m = m_lo; m < m_hi; ++m) {
-      // transposed filter bank wT[k][co][ci]: lanes (adjacent cig) read adjacent float4s -> no bank conflicts
-      const int dm = m * COS;
-      if (WSMEM) {
-        int wk = ws_off + (p + S * m) * a.cout * a.cin + 4 * cig;
-#pragma unroll 2
-        for (int co = 0; co < a.cout; co += 4, wk += 4 * a.cin) {
-          const float4 w0 = ld4(smem + wk), w1 = ld4(smem + wk + a.cin), w2 = ld4(smem + wk + 2 * a.cin), w3 = ld4(smem + wk + 3 * a.cin);
-#pragma unroll
-          for (int i = 0; i < TMB; ++i) {
-            const float4 d = ld4(smem + dyo[i] - dm + co);
-            acc[i].x = fmaf(d.x, w0.x, fmaf(d.y, w1.x, fmaf(d.z, w2.x, fmaf(d.w, w3.x, acc[i].x))));
-            acc[i].y = fmaf(d.x, w0.y, fmaf(d.y, w1.y, fmaf(d.z, w2.y, fmaf(d.w, w3.y, acc[i].y))));
-            acc[i].z = fmaf(d.x, w0.z, fmaf(d.y, w1.z, fmaf(d.z, w2.z, fmaf(d.w, w3.z, acc[i].z))));
-            acc[i].w = fmaf(d.x, w0.w, fmaf(d.y, w1.w, fmaf(d.z, w2.w, fmaf(d.w, w3.w, acc[i].w))));
-          }
-        }
-      } else {
-        const float* wk = a.w + (size_t)(p + S * m) * a.cout * a.cin + 4 * cig;
-#pragma unroll 2
-        for (int co = 0; co < a.cout; co += 4, wk += 4 * a.cin) {
-          const float4 w0 = ldg4(wk), w1 = ldg4(wk + a.cin), w2 = ldg4(wk + 2 * a.cin), w3 = ldg4(wk + 3 * a.cin);
-#pragma unroll
-          for (int i = 0; i < TMB; ++i) {
-            const float4 d = ld4(smem + dyo[i] - dm + co);
-            acc[i].x = fmaf(d.x, w0.x, fmaf(d.y, w1.x, fmaf(d.z, w2.x, fmaf(d.w, w3.x, acc[i].x))));
-            acc[i].y = fmaf(d.x, w0.y, fmaf(d.y, w1.y, fmaf(d.z, w2.y, fmaf(d.w, w3.y, acc[i].y))));
-            acc[i].z = fmaf(d.x, w0.z, fmaf(d.y, w1.z, fmaf(d.z, w2.z, fmaf(d.w, w3.z, acc[i].z))));
-            acc[i].w = fmaf(d.x, w0.w, fmaf(d.y, w1.w, fmaf(d.z, w2.w, fmaf(d.w, w3.w, acc[i].w))));
-          }
-        }
-      }
-    }
-    if (a.has_down && ks == 0 && (t0[p] & 1) == 0) {     // 1x1 stride-2 shortcut conv touches even input rows only
-      int ddo[TMB];
-#pragma unroll
-      for (int i = 0; i < TMB; ++i) ddo[i] = dysd_off + (u * a.t_out + (tt[i] >> 1)) * COSD;
-      if (WSMEM) {
-        int wk = wsd_off + 4 * cig;                        // wdT[co][ci]
-        for (int co = 0; co < a.coutd; co += 4, wk += 4 * a.cin) {
-          const float4 w0 = ld4(smem + wk), w1 = ld4(smem + wk + a.cin), w2 = ld4(smem + wk + 2 * a.cin), w3 = ld4(smem + wk + 3 * a.cin);
-#pragma unroll
-          for (int i = 0; i < TMB; ++i) {
-            const float4 d = ld4(smem + ddo[i] + co);
-            acc[i].x = fmaf(d.x, w0.x, fmaf(d.y, w1.x, fmaf(d.z, w2.x, fmaf(d.w, w3.x, acc[i].x))));
-            acc[i].y = fmaf(d.x, w0.y, fmaf(d.y, w1.y, fmaf(d.z, w2.y, fmaf(d.w, w3.y, acc[i].y))));
-            acc[i].z = fmaf(d.x, w0.z, fmaf(d.y, w1.z, fmaf(d.z, w2.z, fmaf(d.w, w3.z, acc[i].z))));
-            acc[i].w = fmaf(d.x, w0.w, fmaf(d.y, w1.w, fmaf(d.z, w2.w, fmaf(d.w, w3.w, acc[i].w))));
-          }
-        }
-      } else {
-        const float* wk = a.wd + 4 * cig;
-        for (int co = 0; co < a.coutd; co += 4, wk += 4 * a.cin) {
-          const float4 w0 = ldg4(wk), w1 = ldg4(wk + a.cin), w2 = ldg4(wk + 2 * a.cin), w3 = ldg4(wk + 3 * a.cin);
-#pragma unroll
-          for (int i = 0; i < TMB; ++i) {
-            const float4 d = ld4(smem + ddo[i] + co);
-            acc[i].x = fmaf(d.x, w0.x, fmaf(d.y, w1.x, fmaf(d.z, w2.x, fmaf(d.w, w3.x, acc[i].x))));
-            acc[i].y = fmaf(d.x, w0.y, fmaf(d.y, w1.y, fmaf(d.z, w2.y, fmaf(d.w, w3.y, acc[i].y))));
-            acc[i].z = fmaf(d.x, w0.z, fmaf(d.y, w1.z, fmaf(d.z, w2.z, fmaf(d.w, w3.z, acc[i].z))));
-            acc[i].w = fmaf(d.x, w0.w, fmaf(d.y, w1.w, fmaf(d.z, w2.w, fmaf(d.w, w3.w, acc[i].w))));
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < TMB; ++i)
-      if (rt + i * nrt[p] < np[p]) st4(dxs + ((size_t)ks * Rin_max + (size_t)u * a.t_in + tt[i]) * a.cin + 4 * cig, acc[i]);
-  }
+  // ---- transposed conv (+ shortcut conv^T) into the dx planes ----
+  if (WSMEM) convT_tasks<K, TMB, kThreads>(smem, WShared{smem, ws_off, wsd_off}, a, dys_off, dysd_off, dxs, Rin_max, Ue, TPd, PLd, COS, COSD);
+  else convT_tasks<K, TMB, kThreads>(smem, WGlobal{a.w, a.wd}, a, dys_off, dysd_off, dxs, Rin_max, Ue, TPd, PLd, COS, COSD);
   __syncthreads();
 
-  // ---- epilogue: dz of the layer(s) below + partial BatchNorm-backward sums ----
-  const int Rin = Ue * a.t_in;
-  const int nseg = imax(1, kThreads / NCIG);
-  const int seg = tid / NCIG, cig = tid - seg * NCIG;
-  const size_t grow0 = (size_t)u0 * a.t_in;
-  float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1, sd1 = s1, sd2 = s1;
-  if (seg < nseg) {
-    const Chan4 kp = chan4_load(a.bnfp, a.cin, 4 * cig);
-    const bool has_pd = a.epi_kind == 2 && a.ypd;
-    Chan4 kpd = kp;
-    if (has_pd) kpd = chan4_load(a.bnfpd, a.cin, 4 * cig);
-    for (int r = seg; r < Rin; r += nseg) {
-      const size_t gofs = (grow0 + r) * a.cin + 4 * cig;
-      float4 v = ld4(dxs + (size_t)r * a.cin + 4 * cig);
-      for (int ks = 1; ks < a.KS; ++ks) v = add4(v, ld4(dxs + ((size_t)ks * Rin_max + r) * a.cin + 4 * cig));
-      if (a.gid) v = add4(v, ld4(a.gid + gofs));
-      const float4 yv = ld4(a.yp + gofs);
-      float4 g;
-      if (a.epi_kind == 1) g = mask_pos4(v, chan4_bn(kp, yv));
-      else g = mask_pos4(v, ld4(a.out_prev + gofs));
-      st4(a.gprev + gofs, g);
-      s1 = add4(s1, g);
-      s2 = add4(s2, mul4(g, chan4_xhat(kp, yv)));
-      if (has_pd) {
-        const float4 yd = ld4(a.ypd + gofs);
-        const float4 gs = mask_pos4(g, chan4_bn(kpd, yd));
-        sd1 = add4(sd1, gs);
-        sd2 = add4(sd2, mul4(gs, chan4_xhat(kpd, yd)));
-      }
-    }
-    float* r0 = red + ((size_t)(0 * nseg + seg) * a.cin + 4 * cig);
-    st4(r0, s1);
-    st4(r0 + (size_t)nseg * a.cin, s2);
-    st4(r0 + (size_t)2 * nseg * a.cin, sd1);
-    st4(r0 + (size_t)3 * nseg * a.cin, sd2);
-  }
-  __syncthreads();
-  const int nq = (a.epi_kind == 2 && a.ypd) ? 4 : 2;
-  for (int i = tid; i < nq * a.cin; i += kThreads) {
-    const int qd = i / a.cin, c = i - qd * a.cin;
-    float s = 0.f;
-    for (int sg = 0; sg < nseg; ++sg) s += red[((size_t)qd * nseg + sg) * a.cin + c];
-    stat[(qd >> 1) * 2 * a.cin + c * 2 + (qd & 1)] = s;          // producer layer: [c*2+q], then its down conv: [c*2+q]
-  }
-  const PubSeg segs[2] = {{stat, 2 * a.cin, a.bpartp}, {stat + 2 * a.cin, nq == 4 ? 2 * a.cin : 0, a.bpartpd}};
+  // ---- epilogue: dz of the layer(s) below + partial BatchNorm-backward sums, one record per cluster ----
+  bwd_epilogue<kThreads, false>(a, dxs, Rin_max, Ue * a.t_in, imax(1, kThreads / (a.cin >> 2)), (size_t)u0 * a.t_in, nullptr, red, stat,
+                                stat + 2 * a.cin);
+  const PubSeg segs[2] = {{stat, 2 * a.cin, a.bpartp}, {stat + 2 * a.cin, (a.epi_kind == 2 && a.ypd) ? 2 * a.cin : 0, a.bpartpd}};
   cluster_publish(segs, vb);
 }
 
@@ -294,7 +144,7 @@ __global__ void __launch_bounds__(kThreads) conv_bwd_data_kernel(BwdDataArgs a) 
   TCR_DYNAMIC_SMEM(smem_raw);
   MbarCtx mb{reinterpret_cast<uint64_t*>(smem_raw), 0u, false};
   pdl_trigger();
-  conv_bwd_data_body<K, WSMEM>(a, blockIdx.x, a.nvb, smem_raw, mb);
+  conv_bwd_data_body<K, WSMEM>(a, blockIdx.x, smem_raw, mb);
 }
 
 // Transposed filter banks wT[k][co][ci] for the backward-data kernels (all conv layers, one launch).  `params`
@@ -305,11 +155,8 @@ __device__ __forceinline__ void weight_transpose_body(const WtArgs& a, const int
   int l = 0;
   while (l + 1 < a.nlayers && p >= a.layer[l + 1].begin) ++l;
   const WtLayer L = a.layer[l];
-  const int64_t i = p - L.begin;                       // index into wT: ((k*cout + co)*cin + ci)
-  const int ci = (int)(i % L.cin);
-  const int co = (int)((i / L.cin) % L.cout);
-  const int k = (int)(i / ((int64_t)L.cin * L.cout));
-  L.wT[i] = a.params[L.w_off + ((int64_t)k * L.cin + ci) * L.cout + co];
+  const int64_t i = p - L.begin;
+  L.wT[i] = a.params[L.w_off + wT_source(i, L.cin, L.cout)];
 }
 __global__ void __launch_bounds__(256) weight_transpose_kernel(WtArgs a) {
   pdl_wait();
@@ -347,11 +194,7 @@ __device__ __forceinline__ void dw_body(const BwdWeightArgs& a, int bx, int by, 
   const int c4n = a.cin >> 2, d4n = a.cot >> 2, npad = a.pad_left + pad_right;
   for (int ub0 = ubeg; ub0 < uend; ub0 += a.UB) {
     const int Ue = imin(a.UB, uend - ub0);
-    for (int idx = tid; idx < Ue * npad * c4n; idx += blockDim.x) {
-      const int c4 = idx % c4n, prow = (idx / c4n) % npad, u = idx / (c4n * npad);
-      const int row = prow < a.pad_left ? prow : a.t_in + prow;
-      st4(xs + ((size_t)(u * TP + row) * a.cin + 4 * c4), make_float4(0.f, 0.f, 0.f, 0.f));
-    }
+    zero_pad_rows(xs, Ue, a.t_in, c4n, TP, a.cin, a.pad_left, npad, (int)blockDim.x);
     {
       const RowWalk w = row_walk(tid, (int)blockDim.x, c4n);
       const int rows = Ue * a.t_in;
@@ -633,18 +476,16 @@ static DySrc make_dy(const tcr_handle* h, const ConvPlan& cv, const float* dz, i
 }
 
 // *gc_out: per-cluster records of BatchNorm-backward sums this launch leaves for the layer(s) below (0 when recording)
-static int bwd_data(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, BwdDataArgs a, const float* params, int n, cudaStream_t s, int* gc_out) {
+static int bwd_data(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, BwdDataArgs a, int n, cudaStream_t s, int* gc_out) {
   int U, KS, wsm;
   pick_bwd_tile(h->sms, cv, dn, n, &U, &KS, &wsm);
   a.n = n; a.U = U; a.w_smem = wsm;
-  (void)params;
   a.w = cv.wT; a.cin = cv.cin; a.cout = cv.cout; a.k = cv.k; a.stride = cv.stride;
   a.t_in = cv.t_in; a.t_out = cv.t_out; a.pad_left = cv.pad_left; a.KS = KS;
   a.has_down = dn ? 1 : 0;
   a.wd = dn ? dn->wT : nullptr;
   a.coutd = dn ? dn->cout : 0;
   const int groups = (n + U - 1) / U;
-  a.nvb = groups;
   const size_t smem = bwd_data_smem(cv, dn, U, KS, wsm != 0);
   *gc_out = 0;
   const int CL = cluster_size(h);
@@ -687,7 +528,7 @@ int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s)
       a.epi_kind = 1;
       a.yp = ca.y; a.bnfp = ca.bnf; a.bpartp = ca.bpart; a.gprev = ca.g;
       int gc = 0;
-      int rc = bwd_data(h, cb, nullptr, a, params, n, s, &gc);
+      int rc = bwd_data(h, cb, nullptr, a, n, s, &gc);
       if (rc) return rc;
       ca.b_gc = gc;
       if (sync_bn_on(h) && (rc = sync_records(h, ca.bpart, gc, 2 * ca.cout, ca.bsync, s))) return rc;
@@ -716,7 +557,7 @@ int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s)
         a.yp = c0.y; a.bnfp = c0.bnf; a.bpartp = c0.bpart; a.gprev = c0.g;
       }
       int gc = 0;
-      int rc = bwd_data(h, ca, dn, a, params, n, s, &gc);
+      int rc = bwd_data(h, ca, dn, a, n, s, &gc);
       if (rc) return rc;
       if (i > 0) {
         BlockPlan& pb = h->blocks[i - 1];

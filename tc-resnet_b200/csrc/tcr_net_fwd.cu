@@ -11,7 +11,7 @@
 // A CTA owns U whole utterances, so SAME padding is a few zero rows of the shared-memory tile.
 #include <stdlib.h>
 
-#include "tcr_bn.cuh"
+#include "tcr_layer.cuh"
 #include "tcr_net.h"
 
 namespace tcr {
@@ -22,12 +22,11 @@ constexpr int TM = 4;   // output rows per thread task
 // conv forward
 // ------------------------------------------------------------------------------------------------
 template <int K, bool WSMEM>
-__device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, const int nvb, unsigned char* smem_raw, MbarCtx& mb) {
+__device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, unsigned char* smem_raw, MbarCtx& mb) {
   float* smem = reinterpret_cast<float*>(smem_raw);
   const int tid = threadIdx.x;
   const int u0 = vb * a.U;
   const int Ue = imax(0, imin(a.U, a.n - u0));        // 0: a CTA that only pads the grid to whole clusters
-  (void)nvb;
   const int CS = chan_stride(a.cin);
   const int pad_right = imax((a.t_out - 1) * a.stride + K - a.pad_left - a.t_in, 0);
   const int TP = a.pad_left + a.t_in + pad_right;
@@ -65,12 +64,7 @@ __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, co
 
   // ---- stage the input tile (producer's BN/ReLU/residual applied here) ----
   const int c4n = a.cin >> 2;
-  const int npad = a.pad_left + pad_right;
-  for (int idx = tid; idx < Ue * npad * c4n; idx += kThreads) {
-    const int c4 = idx % c4n, pr = (idx / c4n) % npad, u = idx / (c4n * npad);
-    const int row = pr < a.pad_left ? pr : a.t_in + pr;
-    st4(xs + ((size_t)(u * TP + row) * CS + 4 * c4), make_float4(0.f, 0.f, 0.f, 0.f));
-  }
+  zero_pad_rows(xs, Ue, a.t_in, c4n, TP, CS, a.pad_left, a.pad_left + pad_right, kThreads);
   pdl_wait();                       // everything above is independent of the producer kernel (filters: caller-owned params)
   tl_stamp(a.tl, vb, 7);
   {
@@ -131,91 +125,18 @@ __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, co
   __syncthreads();
   tl_stamp(a.tl, vb, 2);
 
-  // ---- register-tiled conv: task = (k-slice, row tile of TM, 4 output channels) ----
+  // ---- register-tiled conv (+ shortcut conv) into the k-slice planes ----
   const int R = Ue * a.t_out;
-  const int NRT = (R + TM - 1) / TM;
-  const int NCG = a.cout >> 2;
-  const int KPS = K / a.KS;
-  const int ntasks = NRT * NCG * a.KS;
-  const int NCGD = a.wd ? (a.coutd >> 2) : 0;
-  const int ntasks_all = ntasks + NRT * NCGD;
-  for (int task = tid; task < ntasks_all; task += kThreads) {
-    const bool is_down = task >= ntasks;
-    const int tk = is_down ? task - ntasks : task;
-    const int ncg = is_down ? NCGD : NCG;
-    const int cg = tk % ncg;
-    const int rt = (tk / ncg) % NRT;
-    const int ks = is_down ? 0 : tk / (ncg * NRT);
-    // 32-bit float offsets from the shared-memory base: the inner loop is LDS.128 + FFMA with integer adds only
-    int xo[TM];
-#pragma unroll
-    for (int i = 0; i < TM; ++i) {
-      const int r = imin(rt + i * NRT, R - 1);      // rows of a task are NRT apart: adjacent lanes -> adjacent rows
-      const int u = r / a.t_out, t = r - u * a.t_out;
-      xo[i] = xs_off + (is_down ? (u * TP + a.pad_left + 2 * t) : (u * TP + t * a.stride)) * CS;
-    }
-    float4 acc[TM];
-#pragma unroll
-    for (int i = 0; i < TM; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int k_lo = is_down ? 0 : ks * KPS, k_hi = is_down ? 1 : k_lo + KPS;
-    const int co_n = is_down ? a.coutd : a.cout;
-    if (WSMEM) {
-      const int wb = (is_down ? wsd_off : ws_off) + 4 * cg;
-      for (int k = k_lo; k < k_hi; ++k) {
-        int wk = wb + k * a.cin * co_n;
-        const int xk = k * CS;
-#pragma unroll 2
-        for (int ci = 0; ci < a.cin; ci += 4, wk += 4 * co_n) {
-          const float4 w0 = ld4(smem + wk), w1 = ld4(smem + wk + co_n), w2 = ld4(smem + wk + 2 * co_n), w3 = ld4(smem + wk + 3 * co_n);
-#pragma unroll
-          for (int i = 0; i < TM; ++i) {
-            const float4 x = ld4(smem + xo[i] + xk + ci);
-            acc[i].x = fmaf(x.x, w0.x, acc[i].x); acc[i].y = fmaf(x.x, w0.y, acc[i].y);
-            acc[i].z = fmaf(x.x, w0.z, acc[i].z); acc[i].w = fmaf(x.x, w0.w, acc[i].w);
-            acc[i].x = fmaf(x.y, w1.x, acc[i].x); acc[i].y = fmaf(x.y, w1.y, acc[i].y);
-            acc[i].z = fmaf(x.y, w1.z, acc[i].z); acc[i].w = fmaf(x.y, w1.w, acc[i].w);
-            acc[i].x = fmaf(x.z, w2.x, acc[i].x); acc[i].y = fmaf(x.z, w2.y, acc[i].y);
-            acc[i].z = fmaf(x.z, w2.z, acc[i].z); acc[i].w = fmaf(x.z, w2.w, acc[i].w);
-            acc[i].x = fmaf(x.w, w3.x, acc[i].x); acc[i].y = fmaf(x.w, w3.y, acc[i].y);
-            acc[i].z = fmaf(x.w, w3.z, acc[i].z); acc[i].w = fmaf(x.w, w3.w, acc[i].w);
-          }
-        }
-      }
-    } else {
-      const float* wbase = (is_down ? a.wd : a.w) + 4 * cg;
-      for (int k = k_lo; k < k_hi; ++k) {
-        const float* wk = wbase + (size_t)k * a.cin * co_n;
-        const int xk = k * CS;
-#pragma unroll 2
-        for (int ci = 0; ci < a.cin; ci += 4, wk += 4 * co_n) {
-          const float4 w0 = ldg4(wk), w1 = ldg4(wk + co_n), w2 = ldg4(wk + 2 * co_n), w3 = ldg4(wk + 3 * co_n);
-#pragma unroll
-          for (int i = 0; i < TM; ++i) {
-            const float4 x = ld4(smem + xo[i] + xk + ci);
-            acc[i].x = fmaf(x.x, w0.x, acc[i].x); acc[i].y = fmaf(x.x, w0.y, acc[i].y);
-            acc[i].z = fmaf(x.x, w0.z, acc[i].z); acc[i].w = fmaf(x.x, w0.w, acc[i].w);
-            acc[i].x = fmaf(x.y, w1.x, acc[i].x); acc[i].y = fmaf(x.y, w1.y, acc[i].y);
-            acc[i].z = fmaf(x.y, w1.z, acc[i].z); acc[i].w = fmaf(x.y, w1.w, acc[i].w);
-            acc[i].x = fmaf(x.z, w2.x, acc[i].x); acc[i].y = fmaf(x.z, w2.y, acc[i].y);
-            acc[i].z = fmaf(x.z, w2.z, acc[i].z); acc[i].w = fmaf(x.z, w2.w, acc[i].w);
-            acc[i].x = fmaf(x.w, w3.x, acc[i].x); acc[i].y = fmaf(x.w, w3.y, acc[i].y);
-            acc[i].z = fmaf(x.w, w3.z, acc[i].z); acc[i].w = fmaf(x.w, w3.w, acc[i].w);
-          }
-        }
-      }
-    }
-    float* dst = is_down ? ysd : ys + (size_t)ks * Rmax * a.cout;
-#pragma unroll
-    for (int i = 0; i < TM; ++i) {
-      const int r = rt + i * NRT;
-      if (r < R) st4(dst + (size_t)r * co_n + 4 * cg, acc[i]);
-    }
-  }
+  if (WSMEM) conv_fwd_tasks<K, TM, kThreads>(smem, WShared{smem, ws_off, wsd_off}, xs_off, ys, ysd, Rmax, R, a.cin, a.cout, a.coutd, a.stride,
+                                             a.t_out, TP, CS, a.pad_left, a.KS);
+  else conv_fwd_tasks<K, TM, kThreads>(smem, WGlobal{a.w, a.wd}, xs_off, ys, ysd, Rmax, R, a.cin, a.cout, a.coutd, a.stride, a.t_out, TP, CS,
+                                       a.pad_left, a.KS);
   __syncthreads();
   tl_stamp(a.tl, vb, 3);
 
   // ---- epilogue: sum k-slices in fixed order, coalesced store of the pre-BN output ----
   const size_t grow0 = (size_t)u0 * a.t_out;
+  const int NCG = a.cout >> 2, NCGD = a.coutd >> 2;
   for (int idx = tid; idx < R * NCG; idx += kThreads) {
     float4 v = ld4(ys + (size_t)idx * 4);
     for (int ks = 1; ks < a.KS; ++ks) v = add4(v, ld4(ys + (size_t)ks * Rmax * a.cout + (size_t)idx * 4));
@@ -227,8 +148,8 @@ __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, co
   if (!a.train) return;
   __syncthreads();
   tl_stamp(a.tl, vb, 4);
-  tile_stats(ys, R, a.cout, red, nullptr, spart);
-  if (a.wd) tile_stats(ysd, R, a.coutd, red, nullptr, spart + 2 * a.cout);
+  tile_stats(ys, R, a.cout, red, spart);
+  if (a.wd) tile_stats(ysd, R, a.coutd, red, spart + 2 * a.cout);
   tl_stamp(a.tl, vb, 5);
   const PubSeg segs[2] = {{spart, 2 * a.cout, a.fpart}, {spart + 2 * a.cout, a.wd ? 2 * a.coutd : 0, a.fpartd}};
   cluster_publish(segs, vb);
@@ -240,7 +161,7 @@ __global__ void __launch_bounds__(kThreads) conv_fwd_kernel(FwdArgs a) {
   TCR_DYNAMIC_SMEM(smem_raw);
   MbarCtx mb{reinterpret_cast<uint64_t*>(smem_raw), 0u, false};
   pdl_trigger();                    // grid <= resident CTA slots: the next kernel's CTAs may take slots as ours retire
-  conv_fwd_body<K, WSMEM>(a, blockIdx.x, a.nvb, smem_raw, mb);
+  conv_fwd_body<K, WSMEM>(a, blockIdx.x, smem_raw, mb);
 }
 
 // Eval mode: BN tables from the moving statistics (bn_forward with is_training=False).
@@ -282,11 +203,10 @@ __host__ __device__ inline size_t head_smem_floats(int T, int C, int NC) {
          kHeadU + 8 + 4 * kHeadThreads + 4 * C + 4;
 }
 
-__device__ __forceinline__ void head_body(const HeadArgs& a, const int vb, const int nvb, unsigned char* smem_raw) {
-  (void)nvb;
+__device__ __forceinline__ void head_body(const HeadArgs& a, const int vb, unsigned char* smem_raw) {
   float* smem = reinterpret_cast<float*>(smem_raw) + 4;          // first 16 bytes: the persistent kernel's mbarrier
   const int C = a.c, T = a.t, NC = a.classes, TC = T * C;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int u0 = vb * kHeadU, nu = imax(0, imin(kHeadU, a.n - u0)), rows = nu * T;   // nu == 0: cluster padding CTA
   float* tb = smem;
   float* td = tb + 4 * C;
@@ -346,60 +266,10 @@ __device__ __forceinline__ void head_body(const HeadArgs& a, const int vb, const
     }
   }
   __syncthreads();
-  // average pool + dropout
-#pragma unroll 1
-  for (int i = tid; i < nu * C; i += kHeadThreads) {
-    const int u = i / C, cc = i - u * C;
-    float acc = 0.f;
-    for (int t = 0; t < T; ++t) acc += so[(u * T + t) * C + cc];
-    const float pooled = acc / (float)T;
-    float mk = 1.f, dropped = pooled;
-    if (a.use_dropout) {
-      const size_t gi = (size_t)(u0 + u) * C + cc;
-      mk = a.mask ? a.mask[gi] : floorf(a.keep + uniform01(a.seed, (uint64_t)gi));
-      dropped = pooled / a.keep * mk;                       // tf.nn.dropout: x / keep_prob * floor(keep_prob + U)
-    }
-    s_drop[i] = dropped;
-    s_mk[i] = mk;
-  }
-  __syncthreads();
-  // fc (no bias): one warp per (utterance, class)
-#pragma unroll 1
-  for (int o = warp; o < nu * NC; o += kHeadThreads / 32) {
-    const int u = o / NC, k = o - u * NC;
-    float p = 0.f;
-    for (int cc = lane; cc < C; cc += 32) p = fmaf(s_drop[u * C + cc], s_wfc[cc * NC + k], p);
-    p = warp_sum(p);
-    if (lane == 0) s_logit[o] = p;
-  }
-  __syncthreads();
-  // softmax cross-entropy: one warp per utterance, lane k keeps class k (NC <= 32)
-#pragma unroll 1
-  for (int u = warp; u < nu; u += kHeadThreads / 32) {
-    const bool act = lane < NC;
-    const float logit = act ? s_logit[u * NC + lane] : 0.f;
-    const float mx = warp_max(act ? logit : -3.0e38f);
-    const float e = act ? expf(logit - mx) : 0.f;
-    const float se = warp_sum(e);
-    const float prob = e / se;
-    const float logp = (logit - mx) - logf(se);
-    const size_t gi = (size_t)(u0 + u) * NC + lane;
-    if (act) {
-      if (a.logits) a.logits[gi] = logit;
-      if (a.probs) a.probs[gi] = prob;
-    }
-    float loss_n = 0.f, dl = 0.f;
-    if (a.onehot) {
-      float lab = act ? a.onehot[gi] : 0.f;
-      if (a.label_smoothing > 0.f && act) lab = lab * (1.f - a.label_smoothing) + a.label_smoothing / (float)NC;
-      const float labsum = warp_sum(lab);
-      loss_n = -warp_sum(act ? lab * logp : 0.f);
-      dl = act ? (prob * labsum - lab) * a.inv_n : 0.f;
-    }
-    if (act) s_dl[u * NC + lane] = dl;
-    if (lane == 0) s_loss[u] = loss_n;
-  }
-  __syncthreads();
+  HeadSmem hs{s_wfc, s_drop, s_mk, s_dnet, s_logit, s_dl, s_loss, red};
+  float* sp = red + 4 * SEG * C;                          // [4C + 1] this CTA's sums: conv_b (c*2+q), down (c*2+q), CE
+  head_tail<kHeadThreads>(a, hs, C, T, NC, u0, nu, so, syb, a.ydn ? ssh : nullptr, tb, td, a.backward != 0,
+                          a.backward ? a.gout + base : nullptr, sp, a.backward ? a.dwfc_part + (size_t)vb * C * NC : nullptr);
   if (!a.backward) {
     if (a.onehot) {
       if (tid == 0) {
@@ -412,64 +282,6 @@ __device__ __forceinline__ void head_body(const HeadArgs& a, const int vb, const
     }
     return;
   }
-
-  // ---- head backward: d logits -> d pooled (fc^T, dropout, AvgPoolGrad) ----
-#pragma unroll 1
-  for (int i = tid; i < nu * C; i += kHeadThreads) {
-    const int u = i / C, cc = i - u * C;
-    float d = 0.f;
-    for (int k = 0; k < NC; ++k) d = fmaf(s_dl[u * NC + k], s_wfc[cc * NC + k], d);
-    if (a.use_dropout) d = d / a.keep * s_mk[i];
-    s_dnet[i] = d / (float)T;
-  }
-  __syncthreads();
-  // gradient at the block output and the BN-backward partial sums of conv_b (and of the down conv)
-  {
-    float sb1 = 0.f, sb2 = 0.f, sd1 = 0.f, sd2 = 0.f;
-    if (seg < SEG) {
-      const float mb_ = tb[c], rb_ = tb[C + c];
-      const float md_ = td[c], rd_ = td[C + c], sd_ = td[2 * C + c], bd_ = td[3 * C + c];
-#pragma unroll 1
-      for (int r = seg; r < rows; r += SEG) {
-        const int u = r / T;
-        const float g = so[r * C + c] > 0.f ? s_dnet[u * C + c] : 0.f;
-        a.gout[base + r * C + c] = g;
-        sb1 += g;
-        sb2 = fmaf(g, (syb[r * C + c] - mb_) * rb_, sb2);
-        if (a.ydn) {
-          const float yd = ssh[r * C + c];
-          const float gs = fmaf(yd - md_, sd_, bd_) > 0.f ? g : 0.f;
-          sd1 += gs;
-          sd2 = fmaf(gs, (yd - md_) * rd_, sd2);
-        }
-      }
-      red[(0 * SEG + seg) * C + c] = sb1;
-      red[(1 * SEG + seg) * C + c] = sb2;
-      red[(2 * SEG + seg) * C + c] = sd1;
-      red[(3 * SEG + seg) * C + c] = sd2;
-    }
-  }
-  __syncthreads();
-  float* sp = red + 4 * SEG * C;                          // [4C + 1] this CTA's sums: conv_b (c*2+q), down (c*2+q), CE
-#pragma unroll 1
-  for (int i = tid; i < 4 * C; i += kHeadThreads) {
-    const int q = i / C, cc = i - q * C;
-    float s = 0.f;
-    for (int k = 0; k < SEG; ++k) s += red[(q * SEG + k) * C + cc];
-    sp[(q >> 1) * 2 * C + cc * 2 + (q & 1)] = s;
-  }
-  if (tid == 0) {
-    float s = 0.f;
-    for (int u = 0; u < nu; ++u) s += s_loss[u];
-    sp[4 * C] = s;
-  }
-#pragma unroll 1
-  for (int i = tid; i < C * NC; i += kHeadThreads) {
-    const int cc = i / NC, k = i - cc * NC;
-    float s = 0.f;
-    for (int u = 0; u < nu; ++u) s = fmaf(s_drop[u * C + cc], s_dl[u * NC + k], s);
-    if (nu > 0) a.dwfc_part[(size_t)vb * C * NC + i] = s;     // cluster-padding CTAs own no record
-  }
   const PubSeg segs[3] = {{sp, 2 * C, a.bpartb}, {sp + 2 * C, a.ydn ? 2 * C : 0, a.bpartd}, {sp + 4 * C, 1, a.loss_part}};
   cluster_publish(segs, vb);
 }
@@ -478,7 +290,7 @@ __global__ void __launch_bounds__(kHeadThreads) head_kernel(HeadArgs a) {
   TCR_DYNAMIC_SMEM(smem_raw);
   pdl_trigger();
   pdl_wait();
-  head_body(a, blockIdx.x, a.nvb, smem_raw);
+  head_body(a, blockIdx.x, smem_raw);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -683,7 +495,6 @@ static int conv_fwd(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, FwdArgs a, const 
     a.wd = params + dn->w_off; a.yd = dn->y; a.fpartd = dn->fpart; a.coutd = dn->cout;
   }
   const int groups = (n + U - 1) / U;
-  a.nvb = groups;
   const size_t smem = fwd_smem_bytes(cv, dn, U, KS, wsm != 0);
   cv.f_gc = 0;
   if (dn) dn->f_gc = 0;
@@ -786,7 +597,6 @@ int net_forward(tcr_handle* h, const float* feat, const float* params, const flo
       ha.ydn = dn ? dn->y : nullptr; ha.bnfd = dn ? dn->bnf : nullptr; ha.bpartd = dn ? dn->bpart : nullptr;
       ha.dwfc_part = h->d_dwfc_part;
       const int groups = head_groups(n);
-      ha.nvb = groups;
       const int CL = cluster_size(h);
       const int grid = (groups + CL - 1) / CL * CL;
       h->loss_gc = grid / CL;

@@ -20,13 +20,14 @@
 #include <stdio.h>
 #include <stdlib.h>
 
-#include "tcr_bn.cuh"
+#include "tcr_layer.cuh"
 #include "tcr_net.h"
 
 namespace tcr {
 
 constexpr int kResThreads = 512;
 constexpr int kResMaxU = 8;          // utterances per CTA the head's scratch is sized for
+static_assert(kResMaxU * 1 >= 5, "res_head keeps its [4C + 1] sums in the [kResMaxU][C] dnet region");
 constexpr int TMR = 4;               // input rows per thread task of the transposed conv
 
 struct RConv {
@@ -142,19 +143,8 @@ __device__ __noinline__ int res_rec_sum(const float* recA, int colsA, const floa
   if (t < Q * nch) {
     const int q = t % Q, ch = t / Q;
     const float* base = q < QA ? recA + 4 * q : recB + 4 * (q - QA);
-    const int stride = q < QA ? colsA : colsB;
-    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int g0 = ch; g0 < G; g0 += 20 * nch) {      // 148 records / 8 chunks = 19 loads: one batch, one L2 round trip
-      float4 v[20];
-#pragma unroll
-      for (int j = 0; j < 20; ++j) {
-        const int g = g0 + j * nch;
-        v[j] = g < G ? __ldcg(reinterpret_cast<const float4*>(base + (size_t)g * stride)) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int j = 0; j < 20; ++j) s = add4(s, v[j]);
-    }
-    st4(scratch + (size_t)ch * 4 * Q + 4 * q, s);
+    // 148 records / 8 chunks = 19 loads: one batch, one L2 round trip
+    st4(scratch + (size_t)ch * 4 * Q + 4 * q, rec_column_sum<float4, 20>(base, 0, q < QA ? colsA : colsB, ch, nch, G));
   }
   __syncthreads();
   return nch;
@@ -171,23 +161,8 @@ __device__ __noinline__ void res_tables(const float* recA, const TblDst& A, cons
     const bool second = j >= A.C;
     const TblDst& D = second ? B : A;
     const int c = second ? j - A.C : j, C = D.C;
-    const int col = (second ? colsA : 0) + 2 * c;
-    double s1 = 0.0, s2 = 0.0;
-    for (int ch = 0; ch < nch; ++ch) {
-      s1 += (double)scratch[ch * cols + col];
-      s2 += (double)scratch[ch * cols + col + 1];
-    }
-    const double mean = s1 * (double)D.inv_m;
-    double var = s2 * (double)D.inv_m - mean * mean;
-    if (var < 0.0) var = 0.0;
-    const double rstd = 1.0 / sqrt(var + (double)eps);
-    const float g = D.gamma[c], b = D.beta[c];
-    const float fm = (float)mean, fr = (float)rstd, fs = (float)((double)g * rstd);
-    D.tbl[c] = fm; D.tbl[C + c] = fr; D.tbl[2 * C + c] = fs; D.tbl[3 * C + c] = b;
-    if (publish) {
-      D.bnf[c] = fm; D.bnf[C + c] = fr; D.bnf[2 * C + c] = fs; D.bnf[3 * C + c] = b;
-      D.var[c] = (float)var;
-    }
+    bn_channel_finalize(scratch, cols, (second ? colsA : 0) + 2 * c, nch, D.inv_m, eps, D.gamma[c], D.beta[c], C, c, D.tbl, D.bnf, D.var,
+                        publish);
   }
   __syncthreads();
 }
@@ -202,12 +177,7 @@ __device__ __noinline__ void res_bsums(const float* recA, const BsDst& A, const 
   for (int i = threadIdx.x; i < cols; i += kResThreads) {
     const bool second = i >= colsA;
     const BsDst& D = second ? B : A;
-    const int j = second ? i - colsA : i;
-    double s = 0.0;
-    for (int ch = 0; ch < nch; ++ch) s += (double)scratch[ch * cols + i];
-    const float f = (float)s;
-    D.sb[(j & 1) * D.C + (j >> 1)] = f;
-    if (publish) D.bsum[(j & 1) * D.C + (j >> 1)] = f;
+    bsum_finalize(scratch, cols, i, nch, second ? i - colsA : i, D.C, D.sb, D.bsum, publish);
   }
   __syncthreads();
 }
@@ -219,61 +189,8 @@ __device__ __noinline__ void res_bsums(const float* recA, const BsDst& A, const 
 template <int K, int TM>
 __device__ __noinline__ void res_conv(float* smem, int xs_off, int ws_off, int ys_off, int ysd_off, int rcap, int Ue,
                                       int cin, int cout, int coutd, int stride, int t_out, int TP, int CS, int pad_left, int KS) {
-  const int R = Ue * t_out;
-  const int NRT = (R + TM - 1) / TM;
-  const int NCG = cout >> 2;
-  const int KPS = K / KS;
-  const int ntasks = NRT * NCG * KS;
-  const int NCGD = coutd >> 2;
-  const int ntasks_all = ntasks + NRT * NCGD;
-  const int wsd_off = ws_off + K * cin * cout;
-  for (int task = threadIdx.x; task < ntasks_all; task += kResThreads) {
-    const bool is_down = task >= ntasks;
-    const int tk = is_down ? task - ntasks : task;
-    const int ncg = is_down ? NCGD : NCG;
-    const int cg = tk % ncg;
-    const int rt = (tk / ncg) % NRT;
-    const int ks = is_down ? 0 : tk / (ncg * NRT);
-    int xo[TM];
-#pragma unroll
-    for (int i = 0; i < TM; ++i) {
-      const int r = imin(rt + i * NRT, R - 1);
-      const int u = r / t_out, t = r - u * t_out;
-      xo[i] = xs_off + (is_down ? (u * TP + pad_left + 2 * t) : (u * TP + t * stride)) * CS;
-    }
-    float4 acc[TM];
-#pragma unroll
-    for (int i = 0; i < TM; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int k_lo = is_down ? 0 : ks * KPS, k_hi = is_down ? 1 : k_lo + KPS;
-    const int co_n = is_down ? coutd : cout;
-    const int wb = (is_down ? wsd_off : ws_off) + 4 * cg;
-    for (int k = k_lo; k < k_hi; ++k) {
-      int wk = wb + k * cin * co_n;
-      const int xk = k * CS;
-#pragma unroll 2
-      for (int ci = 0; ci < cin; ci += 4, wk += 4 * co_n) {
-        const float4 w0 = ld4(smem + wk), w1 = ld4(smem + wk + co_n), w2 = ld4(smem + wk + 2 * co_n), w3 = ld4(smem + wk + 3 * co_n);
-#pragma unroll
-        for (int i = 0; i < TM; ++i) {
-          const float4 x = ld4(smem + xo[i] + xk + ci);
-          acc[i].x = fmaf(x.x, w0.x, acc[i].x); acc[i].y = fmaf(x.x, w0.y, acc[i].y);
-          acc[i].z = fmaf(x.x, w0.z, acc[i].z); acc[i].w = fmaf(x.x, w0.w, acc[i].w);
-          acc[i].x = fmaf(x.y, w1.x, acc[i].x); acc[i].y = fmaf(x.y, w1.y, acc[i].y);
-          acc[i].z = fmaf(x.y, w1.z, acc[i].z); acc[i].w = fmaf(x.y, w1.w, acc[i].w);
-          acc[i].x = fmaf(x.z, w2.x, acc[i].x); acc[i].y = fmaf(x.z, w2.y, acc[i].y);
-          acc[i].z = fmaf(x.z, w2.z, acc[i].z); acc[i].w = fmaf(x.z, w2.w, acc[i].w);
-          acc[i].x = fmaf(x.w, w3.x, acc[i].x); acc[i].y = fmaf(x.w, w3.y, acc[i].y);
-          acc[i].z = fmaf(x.w, w3.z, acc[i].z); acc[i].w = fmaf(x.w, w3.w, acc[i].w);
-        }
-      }
-    }
-    const int dst = is_down ? ysd_off : ys_off + ks * rcap * cout;
-#pragma unroll
-    for (int i = 0; i < TM; ++i) {
-      const int r = rt + i * NRT;
-      if (r < R) st4(smem + dst + r * co_n + 4 * cg, acc[i]);
-    }
-  }
+  conv_fwd_tasks<K, TM, kResThreads>(smem, WShared{smem, ws_off, ws_off + K * cin * cout}, xs_off, smem + ys_off, smem + ysd_off, rcap,
+                                     Ue * t_out, cin, cout, coutd, stride, t_out, TP, CS, pad_left, KS);
 }
 
 // One pass: sum the k-slice planes into plane 0 (fixed order) and form this CTA's per-channel (sum y, sum y^2) record.
@@ -307,12 +224,8 @@ __device__ __noinline__ void res_reduce_stats(float* ys, int rcap, int KS, int R
 // dst padded tile [U][TP][CS] <- relu(bn(src [rows][C])) (tbl != null) or the raw rows (global features); pad rows zeroed.
 __device__ __noinline__ void res_stage(const float* src, const float* tbl, float* dst, int Ue, int t, int C, int TP, int CS,
                                        int pad_left, int pad_right) {
-  const int c4n = C >> 2, npad = pad_left + pad_right;
-  for (int idx = threadIdx.x; idx < Ue * npad * c4n; idx += kResThreads) {
-    const int c4 = idx % c4n, pr = (idx / c4n) % npad, u = idx / (c4n * npad);
-    const int row = pr < pad_left ? pr : t + pr;
-    st4(dst + ((size_t)(u * TP + row) * CS + 4 * c4), make_float4(0.f, 0.f, 0.f, 0.f));
-  }
+  const int c4n = C >> 2;
+  zero_pad_rows(dst, Ue, t, c4n, TP, CS, pad_left, pad_left + pad_right, kResThreads);
   // c4 fixed per thread (table entries in registers), rows advance by rstep: no division per element
   const RowWalk w = row_walk(threadIdx.x, kResThreads, c4n);
   const int rows = Ue * t;
@@ -336,12 +249,8 @@ __device__ __noinline__ void res_stage(const float* src, const float* tbl, float
 __device__ __noinline__ void res_block_out(const float* yb, const float* tb, const float* sh, const float* td, const float* xin,
                                            int TPx, int CSx, int plx, float* dst, int Ue, int t, int C, int TP, int CS,
                                            int pad_left, int pad_right, float* ogl) {
-  const int c4n = C >> 2, npad = pad_left + pad_right;
-  for (int idx = threadIdx.x; idx < Ue * npad * c4n; idx += kResThreads) {
-    const int c4 = idx % c4n, pr = (idx / c4n) % npad, u = idx / (c4n * npad);
-    const int row = pr < pad_left ? pr : t + pr;
-    st4(dst + ((size_t)(u * TP + row) * CS + 4 * c4), make_float4(0.f, 0.f, 0.f, 0.f));
-  }
+  const int c4n = C >> 2;
+  zero_pad_rows(dst, Ue, t, c4n, TP, CS, pad_left, pad_left + pad_right, kResThreads);
   const RowWalk w = row_walk(threadIdx.x, kResThreads, c4n);
   const int rows = Ue * t;
   if (w.row < rows) {
@@ -363,122 +272,33 @@ __device__ __noinline__ void res_block_out(const float* yb, const float* tb, con
 }
 
 // ------------------------------------------------------------------------------------------------
-// head on the CTA's utterances (same arithmetic as head_body in tcr_net_fwd.cu; inputs are already in shared memory):
+// head on the CTA's utterances (head_tail, tcr_layer.cuh; its inputs are already in shared memory):
 //   so [rows][C] block output, syb raw conv_b output, ssh raw shortcut-conv output (or null), tables tb / td.
+// The CTA's records: BatchNorm-backward sums of conv_b and of the shortcut conv, cross-entropy, fc weight gradient.
 // ------------------------------------------------------------------------------------------------
 __device__ __noinline__ void res_head(const ResProgram& P, const ResCall& a, float* smem, const float* so, const float* syb, const float* ssh,
                                       const float* tb, const float* td, int u0, int nu, int cta) {
   const int C = P.blk[P.nblocks - 1].c, T = P.blk[P.nblocks - 1].t, NC = P.classes;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int rows = nu * T;
-  float* s_wfc = smem + P.o_head;
-  float* s_drop = s_wfc + ((C * NC + 3) & ~3);
-  float* s_mk = s_drop + kResMaxU * C;
-  float* s_dnet = s_mk + kResMaxU * C;
-  float* s_logit = s_dnet + kResMaxU * C;
-  float* s_dl = s_logit + kResMaxU * NC;
-  float* s_loss = s_dl + kResMaxU * NC;
-  float* red = s_loss + kResMaxU;                            // [4 * blockDim]
-  const size_t base = (size_t)u0 * T * C;
-  for (int i = tid; i < C * NC; i += kResThreads) s_wfc[i] = __ldg(a.params + P.fc_off + i);
-  // average pool + dropout
-  for (int i = tid; i < nu * C; i += kResThreads) {
-    const int u = i / C, cc = i - u * C;
-    float acc = 0.f;
-    for (int t = 0; t < T; ++t) acc += so[(u * T + t) * C + cc];
-    const float pooled = acc / (float)T;
-    float mk = 1.f, dropped = pooled;
-    if (a.use_dropout) {
-      const size_t gi = (size_t)(u0 + u) * C + cc;
-      mk = a.mask ? a.mask[gi] : floorf(a.keep + uniform01(a.seed, (uint64_t)gi));
-      dropped = pooled / a.keep * mk;
-    }
-    s_drop[i] = dropped;
-    s_mk[i] = mk;
-  }
+  const int tid = threadIdx.x;
+  HeadSmem hs;
+  hs.wfc = smem + P.o_head;
+  hs.drop = hs.wfc + ((C * NC + 3) & ~3);
+  hs.mk = hs.drop + kResMaxU * C;
+  hs.dnet = hs.mk + kResMaxU * C;
+  hs.logit = hs.dnet + kResMaxU * C;
+  hs.dl = hs.logit + kResMaxU * NC;
+  hs.loss = hs.dl + kResMaxU * NC;
+  hs.red = hs.loss + kResMaxU;                               // [4 * blockDim]
+  for (int i = tid; i < C * NC; i += kResThreads) hs.wfc[i] = __ldg(a.params + P.fc_off + i);
+  float* sp = hs.dnet;                                       // [4C + 1] sums (8C floats, dead once the sums are formed)
+  head_tail<kResThreads>(a, hs, C, T, NC, u0, nu, so, syb, ssh, tb, td, true, P.gout + (size_t)u0 * T * C, sp,
+                         P.dwfc_part + (size_t)cta * C * NC);
   __syncthreads();
-  for (int o = warp; o < nu * NC; o += kResThreads / 32) {
-    const int u = o / NC, k = o - u * NC;
-    float p = 0.f;
-    for (int cc = lane; cc < C; cc += 32) p = fmaf(s_drop[u * C + cc], s_wfc[cc * NC + k], p);
-    p = warp_sum(p);
-    if (lane == 0) s_logit[o] = p;
+  for (int i = tid; i < 2 * C; i += kResThreads) {
+    P.bpartb[(size_t)cta * 2 * C + i] = sp[i];
+    if (P.bpartd) P.bpartd[(size_t)cta * 2 * C + i] = sp[2 * C + i];
   }
-  __syncthreads();
-  for (int u = warp; u < nu; u += kResThreads / 32) {
-    const bool act = lane < NC;
-    const float logit = act ? s_logit[u * NC + lane] : 0.f;
-    const float mx = warp_max(act ? logit : -3.0e38f);
-    const float e = act ? expf(logit - mx) : 0.f;
-    const float se = warp_sum(e);
-    const float prob = e / se;
-    const float logp = (logit - mx) - logf(se);
-    const size_t gi = (size_t)(u0 + u) * NC + lane;
-    if (act) {
-      if (a.logits) a.logits[gi] = logit;
-      if (a.probs) a.probs[gi] = prob;
-    }
-    float lab = act ? a.onehot[gi] : 0.f;
-    if (a.label_smoothing > 0.f && act) lab = lab * (1.f - a.label_smoothing) + a.label_smoothing / (float)NC;
-    const float labsum = warp_sum(lab);
-    const float loss_n = -warp_sum(act ? lab * logp : 0.f);
-    if (act) s_dl[u * NC + lane] = (prob * labsum - lab) * a.inv_n;
-    if (lane == 0) s_loss[u] = loss_n;
-  }
-  __syncthreads();
-  // head backward: d logits -> d pooled (fc^T, dropout, AvgPoolGrad)
-  for (int i = tid; i < nu * C; i += kResThreads) {
-    const int u = i / C, cc = i - u * C;
-    float d = 0.f;
-    for (int k = 0; k < NC; ++k) d = fmaf(s_dl[u * NC + k], s_wfc[cc * NC + k], d);
-    if (a.use_dropout) d = d / a.keep * s_mk[i];
-    s_dnet[i] = d / (float)T;
-  }
-  __syncthreads();
-  const int SEG = kResThreads / C;
-  const int seg = tid / C, c = tid - seg * C;
-  if (seg < SEG) {
-    float sb1 = 0.f, sb2 = 0.f, sd1 = 0.f, sd2 = 0.f;
-    const float mb_ = tb[c], rb_ = tb[C + c];
-    const float md_ = ssh ? td[c] : 0.f, rd_ = ssh ? td[C + c] : 0.f, sd_ = ssh ? td[2 * C + c] : 0.f, bd_ = ssh ? td[3 * C + c] : 0.f;
-    for (int r = seg; r < rows; r += SEG) {
-      const int u = r / T;
-      const float g = so[r * C + c] > 0.f ? s_dnet[u * C + c] : 0.f;
-      P.gout[base + r * C + c] = g;
-      sb1 += g;
-      sb2 = fmaf(g, (syb[r * C + c] - mb_) * rb_, sb2);
-      if (ssh) {
-        const float yd = ssh[r * C + c];
-        const float gs = fmaf(yd - md_, sd_, bd_) > 0.f ? g : 0.f;
-        sd1 += gs;
-        sd2 = fmaf(gs, (yd - md_) * rd_, sd2);
-      }
-    }
-    red[(0 * SEG + seg) * C + c] = sb1;
-    red[(1 * SEG + seg) * C + c] = sb2;
-    red[(2 * SEG + seg) * C + c] = sd1;
-    red[(3 * SEG + seg) * C + c] = sd2;
-  }
-  __syncthreads();
-  // this CTA's records: BatchNorm-backward sums of conv_b (c*2+q) and of the shortcut conv, cross-entropy, fc weight gradient
-  for (int i = tid; i < 4 * C; i += kResThreads) {
-    const int q = i / C, cc = i - q * C;
-    float s = 0.f;
-    for (int k = 0; k < SEG; ++k) s += red[(q * SEG + k) * C + cc];
-    float* dstp = (q >> 1) ? P.bpartd : P.bpartb;
-    if (dstp) dstp[(size_t)cta * 2 * C + cc * 2 + (q & 1)] = s;
-  }
-  if (tid == 0) {
-    float s = 0.f;
-    for (int u = 0; u < nu; ++u) s += s_loss[u];
-    P.loss_part[cta] = s;
-  }
-  for (int i = tid; i < C * NC; i += kResThreads) {
-    const int cc = i / NC, k = i - cc * NC;
-    float s = 0.f;
-    for (int u = 0; u < nu; ++u) s = fmaf(s_drop[u * C + cc], s_dl[u * NC + k], s);
-    P.dwfc_part[(size_t)cta * C * NC + i] = s;
-  }
+  if (tid == 0) P.loss_part[cta] = sp[4 * C];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -499,7 +319,7 @@ __device__ __forceinline__ void res_run_conv(float* smem, const ResProgram& P, c
   }
 }
 
-// Transposed filter banks wT[k][co][ci] for the backward-data pass (what weight_transpose_kernel writes), spread over the CTAs and
+// Transposed filter banks wT[k][co][ci] for the backward-data pass (wT_source, as in weight_transpose_kernel), spread over the CTAs and
 // run in the shadow of the first grid barrier: nobody waits for it before the kernel ends.
 __device__ __noinline__ void res_weight_transpose(const ResProgram& P, const float* __restrict__ params, int cta, int G) {
   // one flat index space over all banks, an equal slice per CTA (a per-layer split left the low CTAs with nine dependent
@@ -518,8 +338,7 @@ __device__ __noinline__ void res_weight_transpose(const ResProgram& P, const flo
     }
     const RConv& L = P.conv[l];
     const int i = p - base;
-    const int ci = i % L.cin, r = i / L.cin, co = r % L.cout, k = r / L.cout;
-    const_cast<float*>(L.wT)[i] = __ldg(params + L.w_off + ((long long)k * L.cin + ci) * L.cout + co);
+    const_cast<float*>(L.wT)[i] = __ldg(params + L.w_off + wT_source(i, L.cin, L.cout));
   }
 }
 
@@ -628,21 +447,12 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_fwd_kernel(const __gr
 // ================================================================================================
 // backward
 // ================================================================================================
-__device__ __forceinline__ float4 rmask_pos4(float4 v, float4 z) {
-  return make_float4(z.x > 0.f ? v.x : 0.f, z.y > 0.f ? v.y : 0.f, z.z > 0.f ? v.z : 0.f, z.w > 0.f ? v.w : 0.f);
-}
-__device__ __forceinline__ float4 rmul4(float4 a, float4 b) { return make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
-
 // dy = FusedBatchNormGrad(dz) of one layer for the CTA's rows: dz [rows][C] and y [rows][C] in shared memory ->
 // dst [U][TPd][COS] (rows at PLd.., pad rows zeroed).  mask: dz *= (bn(y) > 0) first (the shortcut conv's own ReLU).
 __device__ __noinline__ void res_dy_stage(const float* dz, const float* y, const float* tbl, const float* sb, float inv_m, int mask,
                                           float* dst, int Ue, int t, int C, int TPd, int PLd, int COS) {
-  const int c4n = C >> 2, npad = TPd - t;
-  for (int idx = threadIdx.x; idx < Ue * npad * c4n; idx += kResThreads) {
-    const int c4 = idx % c4n, pr = (idx / c4n) % npad, u = idx / (c4n * npad);
-    const int row = pr < PLd ? pr : t + pr;
-    st4(dst + ((size_t)(u * TPd + row) * COS + 4 * c4), make_float4(0.f, 0.f, 0.f, 0.f));
-  }
+  const int c4n = C >> 2;
+  zero_pad_rows(dst, Ue, t, c4n, TPd, COS, PLd, TPd - t, kResThreads);
   const RowWalk w = row_walk(threadIdx.x, kResThreads, c4n);
   const int rows = Ue * t;
   if (w.row < rows) {
@@ -663,138 +473,28 @@ __device__ __noinline__ void res_dy_stage(const float* dz, const float* y, const
   }
 }
 
-// Transposed conv (K = 9) split by input-row parity for stride 2 (+ the 1x1/stride-2 shortcut conv^T on even rows); same loop as
-// conv_bwd_data_body.  dys [U][TPd][COS], dysd [U*t_out][COSD], banks wT [k][cout][cin] | wdT [coutd][cin] -> dx planes [KS][rcap][cin].
+// Transposed conv (K = 9, convT_tasks in tcr_layer.cuh): dys [U][TPd][COS], dysd [U*t_out][COSD], banks wT [k][cout][cin] |
+// wdT [coutd][cin] -> dx planes [KS][rcap][cin].
+struct ConvTShape { int cin, cout, coutd, stride, t_in, t_out, pad_left, KS; };
 __device__ __noinline__ void res_convT(float* smem, int dys_off, int dysd_off, int ws_off, int wsd_off, int dxs_off, int rcap, int Ue,
                                        int cin, int cout, int coutd, int S, int t_in, int t_out, int pad_left, int TPd, int PLd, int COS,
                                        int COSD, int KS) {
-  constexpr int K = 9;
-  const int NCIG = cin >> 2;
-  int t0[2], np[2], nrt[2];
-  for (int p = 0; p < 2; ++p) {
-    t0[p] = ((p - pad_left) % S + S) % S;
-    np[p] = (p < S && t0[p] < t_in) ? (t_in - t0[p] + S - 1) / S : 0;
-    nrt[p] = (np[p] + TMR - 1) / TMR;
-  }
-  const int NRTU = nrt[0] + nrt[1];
-  const int NT0 = (K + S - 1) / S;
-  const int MPS = (NT0 + KS - 1) / KS;
-  const int ntasks = KS * Ue * NRTU * NCIG;
-  for (int task = threadIdx.x; task < ntasks; task += kResThreads) {
-    const int cig = task % NCIG;
-    int q = task / NCIG;
-    const int rtu = q % NRTU;
-    q /= NRTU;
-    const int u = q % Ue, ks = q / Ue;
-    const int p = rtu >= nrt[0] ? 1 : 0;
-    const int rt = rtu - p * nrt[0];
-    int dyo[TMR], tt[TMR];
-#pragma unroll
-    for (int i = 0; i < TMR; ++i) {
-      const int j = imin(rt + i * nrt[p], np[p] - 1);
-      tt[i] = t0[p] + S * j;
-      const int b = (tt[i] + pad_left - p) / S;
-      dyo[i] = dys_off + (u * TPd + PLd + b) * COS;
-    }
-    float4 acc[TMR];
-#pragma unroll
-    for (int i = 0; i < TMR; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int NT = (K - p + S - 1) / S;
-    const int m_lo = ks * MPS, m_hi = imin(NT, m_lo + MPS);
-    for (int m = m_lo; m < m_hi; ++m) {
-      const int dm = m * COS;
-      int wk = ws_off + (p + S * m) * cout * cin + 4 * cig;
-#pragma unroll 2
-      for (int co = 0; co < cout; co += 4, wk += 4 * cin) {
-        const float4 w0 = ld4(smem + wk), w1 = ld4(smem + wk + cin), w2 = ld4(smem + wk + 2 * cin), w3 = ld4(smem + wk + 3 * cin);
-#pragma unroll
-        for (int i = 0; i < TMR; ++i) {
-          const float4 d = ld4(smem + dyo[i] - dm + co);
-          acc[i].x = fmaf(d.x, w0.x, fmaf(d.y, w1.x, fmaf(d.z, w2.x, fmaf(d.w, w3.x, acc[i].x))));
-          acc[i].y = fmaf(d.x, w0.y, fmaf(d.y, w1.y, fmaf(d.z, w2.y, fmaf(d.w, w3.y, acc[i].y))));
-          acc[i].z = fmaf(d.x, w0.z, fmaf(d.y, w1.z, fmaf(d.z, w2.z, fmaf(d.w, w3.z, acc[i].z))));
-          acc[i].w = fmaf(d.x, w0.w, fmaf(d.y, w1.w, fmaf(d.z, w2.w, fmaf(d.w, w3.w, acc[i].w))));
-        }
-      }
-    }
-    if (coutd && ks == 0 && (t0[p] & 1) == 0) {          // 1x1 stride-2 shortcut conv touches even input rows only
-      int ddo[TMR];
-#pragma unroll
-      for (int i = 0; i < TMR; ++i) ddo[i] = dysd_off + (u * t_out + (tt[i] >> 1)) * COSD;
-      int wk = wsd_off + 4 * cig;
-      for (int co = 0; co < coutd; co += 4, wk += 4 * cin) {
-        const float4 w0 = ld4(smem + wk), w1 = ld4(smem + wk + cin), w2 = ld4(smem + wk + 2 * cin), w3 = ld4(smem + wk + 3 * cin);
-#pragma unroll
-        for (int i = 0; i < TMR; ++i) {
-          const float4 d = ld4(smem + ddo[i] + co);
-          acc[i].x = fmaf(d.x, w0.x, fmaf(d.y, w1.x, fmaf(d.z, w2.x, fmaf(d.w, w3.x, acc[i].x))));
-          acc[i].y = fmaf(d.x, w0.y, fmaf(d.y, w1.y, fmaf(d.z, w2.y, fmaf(d.w, w3.y, acc[i].y))));
-          acc[i].z = fmaf(d.x, w0.z, fmaf(d.y, w1.z, fmaf(d.z, w2.z, fmaf(d.w, w3.z, acc[i].z))));
-          acc[i].w = fmaf(d.x, w0.w, fmaf(d.y, w1.w, fmaf(d.z, w2.w, fmaf(d.w, w3.w, acc[i].w))));
-        }
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < TMR; ++i)
-      if (rt + i * nrt[p] < np[p]) st4(smem + dxs_off + ((size_t)ks * rcap + (size_t)u * t_in + tt[i]) * cin + 4 * cig, acc[i]);
-  }
+  const ConvTShape g{cin, cout, coutd, S, t_in, t_out, pad_left, KS};
+  convT_tasks<9, TMR, kResThreads>(smem, WShared{smem, ws_off, wsd_off}, g, dys_off, dysd_off, smem + dxs_off, rcap, Ue, TPd, PLd, COS, COSD);
 }
 
-// Backward epilogue: dx = sum of planes (+ identity gradient); g = dx masked by the consumer-side ReLU; this CTA's
-// (sum g, sum g*xhat) records of the layer(s) below; g stays in shared memory (gdst) for the next phase and goes to global memory
-// (gglob) for the grouped weight-gradient launch.
+// Backward epilogue (bwd_epilogue in tcr_layer.cuh) on shared-memory tensors: g stays in shared memory (gdst) for the next phase
+// and goes to global memory (gglob) for the grouped weight-gradient launch; the CTA's records go to recp / recpd.
 //   kind 1: mask bn(yp) > 0, sums for that layer.  kind 2: mask (previous block's output) > 0, sums for its conv_b (yp, tp) and,
-//   when ypd != null, for its shortcut conv (additionally masked by bn_d(ypd) > 0).  The block output is read from outp
-//   (identity shortcut) or recomputed as bn_b(yp) + relu(bn_d(ypd)).
+//   when ypd != null, for its shortcut conv.  The block output is read from outp (identity shortcut) or recomputed.
+struct ResEpi { const float* gid; int epi_kind; const float* yp; const float* bnfp; const float* out_prev; const float* ypd;
+                const float* bnfpd; float* gprev; int cin, KS; };
 __device__ __noinline__ void res_bwd_epilogue(const float* dxs, int rcap, int KS, int Rin, int C, const float* gid, int kind,
                                               const float* yp, const float* tp, const float* outp, const float* ypd, const float* tpd,
                                               float* gdst, float* gglob, float* red, int red_cap, float* recp, float* recpd) {
-  const int tid = threadIdx.x;
-  const int NCIG = C >> 2;
-  const int nseg = imax(1, imin(kResThreads / NCIG, red_cap / (4 * C)));   // red: [4][nseg][C]
-  const int seg = tid / NCIG, cig = tid - seg * NCIG;
-  float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1, sd1 = s1, sd2 = s1;
-  if (seg < nseg) {
-    const Chan4 kp = chan4_load_s(tp, C, 4 * cig);
-    Chan4 kpd = kp;
-    if (ypd) kpd = chan4_load_s(tpd, C, 4 * cig);
-    for (int r = seg; r < Rin; r += nseg) {
-      const int o = r * C + 4 * cig;
-      float4 v = ld4(dxs + o);
-      for (int ks = 1; ks < KS; ++ks) v = add4(v, ld4(dxs + (size_t)ks * rcap * C + o));
-      if (gid) v = add4(v, ld4(gid + o));
-      const float4 yv = ld4(yp + o);
-      float4 yd = make_float4(0.f, 0.f, 0.f, 0.f), zd = yd;
-      if (ypd) { yd = ld4(ypd + o); zd = chan4_bn(kpd, yd); }
-      float4 g;
-      if (kind == 1) g = rmask_pos4(v, chan4_bn(kp, yv));
-      else if (ypd) g = rmask_pos4(v, add4(chan4_bn(kp, yv), relu4(zd)));      // the block output, recomputed exactly as the forward pass formed it
-      else g = rmask_pos4(v, ld4(outp + o));
-      st4(gdst + o, g);
-      st4(gglob + o, g);
-      s1 = add4(s1, g);
-      s2 = add4(s2, rmul4(g, chan4_xhat(kp, yv)));
-      if (ypd) {
-        const float4 gs = rmask_pos4(g, zd);
-        sd1 = add4(sd1, gs);
-        sd2 = add4(sd2, rmul4(gs, chan4_xhat(kpd, yd)));
-      }
-    }
-    float* r0 = red + ((size_t)seg * C + 4 * cig);
-    st4(r0, s1);
-    st4(r0 + (size_t)nseg * C, s2);
-    st4(r0 + (size_t)2 * nseg * C, sd1);
-    st4(r0 + (size_t)3 * nseg * C, sd2);
-  }
-  __syncthreads();
-  const int nq = ypd ? 4 : 2;
-  for (int i = tid; i < nq * C; i += kResThreads) {
-    const int qd = i / C, cc = i - qd * C;
-    float s = 0.f;
-    for (int sg = 0; sg < nseg; ++sg) s += red[((size_t)qd * nseg + sg) * C + cc];
-    float* rec = (qd >> 1) ? recpd : recp;
-    rec[cc * 2 + (qd & 1)] = s;
-  }
+  const ResEpi e{gid, kind, yp, tp, outp, ypd, tpd, gglob, C, KS};
+  const int nseg = imax(1, imin(kResThreads / (C >> 2), red_cap / (4 * C)));   // red: [4][nseg][C]
+  bwd_epilogue<kResThreads, true>(e, dxs, rcap, Rin, nseg, 0, gdst, red, recp, recpd);
   __syncthreads();
 }
 
