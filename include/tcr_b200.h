@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 7
+#define TCR_ABI_VERSION 8
 
 enum {
   TCR_OK = 0,
@@ -164,6 +164,13 @@ typedef struct tcr_step_args {
   float        rho;          /* RMSProp decay: 0.9 */
   float        beta1_power;  /* Adam: beta1^t before this step */
   float        beta2_power;  /* Adam: beta2^t before this step */
+  /* Exponential moving average of the trained weights (ABI 8), tf.train.ExponentialMovingAverage(decay).apply(variables_to_train)
+   * run behind the train op (helper/trainer.py:213-217): after the optimizer step, per TRAINED parameter in fp32 and on the
+   * updated weight, ema -= (ema - params) * (1 - ema_decay) (no num_updates, no zero-debias).  Entries of frozen variables
+   * (tcr_set_trainable) are not touched.  NULL = off (zero-initialise); with apply_update == 0 nothing is averaged.
+   * Rejected with TCR_ERR_INVALID: ema_decay outside [0, 1] when ema is set. */
+  float*       ema;          /* flat shadow `<var>/ExponentialMovingAverage` [num_trainable], updated in place */
+  float        ema_decay;    /* 0.999 (--ema_decay) */
 } tcr_step_args;
 
 int         tcr_abi_version(void);
@@ -241,9 +248,21 @@ int tcr_eval_accumulate(tcr_handle* h, const float* scores, const float* onehot,
  * same update to the same averaged gradient, so the optimizer state stays identical across replicas. */
 int tcr_train_step(tcr_handle* h, const tcr_step_args* args, tcr_stream stream);
 
+/* Which variables the training steps of this handle train (--trainable_scopes: slim.learning.create_train_op's
+ * variables_to_train, helper/trainer.py:199-222, resolved by common/tf_utils.py:19-37).  `flags`: one int per TRAINABLE row of
+ * tcr_param_table, in table order, nonzero = trained; NULL = every variable (the default).  A frozen variable gets no gradient
+ * (0 in tcr_step_args::grads), its parameters and optimizer slots are left bit for bit as they are, and the step skips the
+ * backward work only it needed: its weight gradient, and the backward-data chain below the lowest conv with a trained variable
+ * (none at all when only fc / fc2 are trained).  Unchanged: the forward pass, total_loss (weight decay over ALL weights), the
+ * BatchNorm moving averages of every layer, and the gradients of the trained variables, which are bit-identical to the full
+ * step's.  Host-side planning, not per step: the plans are rewritten in place, so no step of this handle may still be queued on
+ * the caller's stream (synchronise it first); the streams the handle owns itself are drained by the call.
+ * TCR_ERR_INVALID: count != the number of trainable rows, or no flag set. */
+int tcr_set_trainable(tcr_handle* h, const int32_t* flags, int32_t count);
+
 /* The same step fed from PINNED HOST memory (the feed_dict / tf.data side of session.run(train_op): helper/trainer.py:312-321,
  * datasets/data_wrapper_base.py:100-108).  `a->input` and `a->onehot` are host pointers (cudaHostAlloc / pin_memory);
- * `a->losses` is ignored; the optimizer fields (and Adam's powers) are taken as they are in this call.  The batch is copied H2D on a private copy stream into one of 3 staging slots, the step runs on
+ * `a->losses` is ignored; the optimizer fields (and Adam's powers) and ema / ema_decay are taken as they are in this call.  The batch is copied H2D on a private copy stream into one of 3 staging slots, the step runs on
  * `stream` behind it and its two losses are copied back; the call does not wait for the step it submits.  It returns,
  * in losses_out[0..1] and *losses_step, the losses of the step submitted `lag` calls earlier (*losses_step = -1 while
  * fewer than lag+1 steps are outstanding).  lag in [0,2]: 0 = synchronous, 1 = copy/compute overlap, 2 = also keeps

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtcr_b200.so")
 
 TCR_MODEL_TCRESNET8 = 8
 TCR_MODEL_TCRESNET14 = 14
-ABI_VERSION = 7          # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
+ABI_VERSION = 8         # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
 TCR_INPUT_WAV_F32, TCR_INPUT_FEATURES, TCR_INPUT_WAV_PCM16 = 0, 1, 2
 TCR_OPT_MOMENTUM, TCR_OPT_ADAM, TCR_OPT_RMSPROP = 0, 1, 2
 TCR_FEATURE_MFCC = 0
@@ -72,6 +72,7 @@ class TcrStepArgs(C.Structure):
         ("clips", C.c_void_p), ("background", C.c_void_p), ("pcm_stride", C.c_int64), ("input_resident", C.c_int32),
         ("optimizer", C.c_int32), ("slots2", C.c_void_p), ("beta1", C.c_float), ("beta2", C.c_float),
         ("epsilon", C.c_float), ("rho", C.c_float), ("beta1_power", C.c_float), ("beta2_power", C.c_float),
+        ("ema", C.c_void_p), ("ema_decay", C.c_float),
     ]
 
 
@@ -95,6 +96,7 @@ SYMBOLS = {
     "tcr_eval_accumulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "tcr_comm_set_sync_bn": (C.c_int, [C.c_void_p, C.c_int32]),
     "tcr_train_step": (C.c_int, [C.c_void_p, C.POINTER(TcrStepArgs), C.c_void_p]),
+    "tcr_set_trainable": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "tcr_train_step_host": (C.c_int, [C.c_void_p, C.POINTER(TcrStepArgs), C.c_int32, C.c_void_p, C.POINTER(C.c_float),
                                       C.POINTER(C.c_int64)]),
     "tcr_host_flush": (C.c_int, [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int64)]),

@@ -443,6 +443,7 @@ extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
 
 static void hostfeed_destroy(tcr_handle* h);
 static void frontend_ahead_destroy(tcr_handle* h);
+static int handle_streams_sync(tcr_handle* h);
 
 extern "C" int tcr_destroy(tcr_handle* h) {
   if (!h) return TCR_OK;
@@ -654,6 +655,8 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
     return fail(TCR_ERR_INVALID, "apply_update with Adam / RMSProp needs slots2");
   if (a->optimizer == TCR_OPT_ADAM && a->beta1_power == 1.0f)
     return fail(TCR_ERR_INVALID, "beta1_power == 1: Adam's step size lr*sqrt(1-beta2_power)/(1-beta1_power) is undefined");
+  if (a->ema && !(a->ema_decay >= 0.0f && a->ema_decay <= 1.0f))
+    return fail(TCR_ERR_INVALID, "ema_decay %g outside [0, 1]", (double)a->ema_decay);
   TCR_TRY(check_n(h, a->n));
   cudaStream_t s = (cudaStream_t)stream;
   const float* feat = a->input;
@@ -703,12 +706,14 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
 #endif
   }
   const int resident = resident_mode(h);
-  if (resident == kResidentOff) net_weight_transpose(h, a->params, s);   // the resident forward kernel writes the transposed banks itself
+  // the resident forward kernel writes the transposed banks itself; a head-only step reads none
+  if (resident == kResidentOff && h->bwd_phases > 0) net_weight_transpose(h, a->params, s);
   int rc = resident != kResidentOff ? resident_forward(h, feat, a, s)
                                     : net_forward(h, feat, a->params, nullptr, a->n, true, a->dropout_seed, a->dropout_mask, a->onehot,
                                                   a->weight_decay, a->logits, a->probs, nullptr, /*backward=*/true, s);
   if (rc) return fail(rc, "forward launch failed: %s", g_err);
-  rc = resident == kResidentFwdBwdData ? resident_backward_data(h, feat, a, s) : net_backward_data(h, a->params, a->n, s);
+  rc = resident == kResidentFwdBwdData && h->bwd_phases > 0 ? resident_backward_data(h, feat, a, s)
+                                                            : net_backward_data(h, a->params, a->n, s);
   if (rc) return fail(rc, "backward launch failed: %s", g_err);
   rc = net_weight_gradients(h, feat, a->n, s);
   if (rc) return fail(rc, "weight-gradient launch failed: %s", g_err);
@@ -729,6 +734,34 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
 }
 
 extern "C" int tcr_train_step(tcr_handle* h, const tcr_step_args* a, tcr_stream stream) { return train_step_impl(h, a, stream, nullptr); }
+
+extern "C" int tcr_set_trainable(tcr_handle* h, const int32_t* flags, int32_t count) {
+  if (!h) return fail(TCR_ERR_INVALID, "NULL handle");
+  const int rows = 3 * (int)h->convs.size() + 2;      // trainable rows of the table: per conv weights / beta / gamma, fc, fc2
+  std::vector<int> want;
+  if (flags) {
+    if (count != rows) return fail(TCR_ERR_INVALID, "tcr_set_trainable: %d flags for %d trainable variables", count, rows);
+    int any = 0;
+    for (int i = 0; i < rows; ++i) {
+      want.push_back(flags[i] ? 1 : 0);
+      any |= want.back();
+    }
+    if (!any) return fail(TCR_ERR_INVALID, "tcr_set_trainable: no variable is trained");
+  }
+  // The plans are rewritten in place on the handle's device.  Steps of this handle on the caller's stream must have finished
+  // (include/tcr_b200.h); the handle's own streams (front-end ahead, host-feed copies) are drained here.
+  int prev = 0;
+  TCR_CUDA(cudaGetDevice(&prev));
+  if (prev != h->cfg.device) TCR_CUDA(cudaSetDevice(h->cfg.device));
+  int rc = handle_streams_sync(h);
+  if (!rc) {
+    h->train_rows = want;
+    rc = build_trainable_plans(h);
+    if (rc) rc = fail(rc, "tcr_set_trainable: plan upload failed");
+  }
+  if (prev != h->cfg.device) cudaSetDevice(prev);
+  return rc;
+}
 
 // ------------------------------------------------------------------------------------------------
 // Host-buffer training step: the `feed_dict` / input-pipeline side of session.run(train_op)
@@ -767,6 +800,16 @@ static void hostfeed_destroy(tcr_handle* h) {
   if (f->copy) cudaStreamDestroy(f->copy);
   delete f;
   h->hostfeed = nullptr;
+}
+
+// Waits for the work on the streams the handle owns: the host feed's copy stream and the front-end's own stream.
+static int handle_streams_sync(tcr_handle* h) {
+  const HostFeedState* f = (const HostFeedState*)h->hostfeed;
+  if (f && f->copy) TCR_CUDA(cudaStreamSynchronize(f->copy));
+#ifndef TCR_EMU
+  if (h->fe_stream) TCR_CUDA(cudaStreamSynchronize((cudaStream_t)h->fe_stream));
+#endif
+  return TCR_OK;
 }
 
 static int hostfeed_get(tcr_handle* h, HostFeedState** out) {

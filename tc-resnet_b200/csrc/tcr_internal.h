@@ -144,6 +144,7 @@ struct OptSegment {         // one trainable variable
   const float* part;        // partial sums [R][numel] (weights) or bsum row (gamma/beta), may be null (fc2)
   int R;                    // number of partials to add
   int decay;                // 1: add weight_decay * w
+  int train;                // 0: frozen (tcr_set_trainable): gradient 0, no update; still in sum(w^2) when decay
 };
 struct MovingSegment {      // one BN layer
   int64_t mm_off, mv_off; int c;

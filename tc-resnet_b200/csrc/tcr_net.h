@@ -40,6 +40,20 @@ int net_weight_gradients(tcr_handle* h, const float* feat, int n, cudaStream_t s
 // Gradient finalisation (+ weight decay), optional NCCL all-reduce, optimizer update, BN moving averages, losses.
 int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s);
 
+// Host-side plans that follow the trainable set (tcr_set_trainable, h->train_rows): optimizer segments (tcr_optim.cu), the
+// grouped weight-gradient table and the depth of the backward-data chain (tcr_net_bwd.cu).
+int build_opt_segments(tcr_handle* h);
+int build_dw_table(tcr_handle* h);
+int plan_bwd_phases(const tcr_handle* h);
+inline int build_trainable_plans(tcr_handle* h) {
+  int frozen = 0;
+  for (int f : h->train_rows) frozen += f ? 0 : 1;
+  h->frozen_rows = frozen;
+  h->bwd_phases = plan_bwd_phases(h);
+  const int rc = build_dw_table(h);
+  return rc ? rc : build_opt_segments(h);
+}
+
 int launch_loss_only(tcr_handle* h, const float* params, float weight_decay, int n, float* losses, cudaStream_t s);
 int head_groups(int n);
 

@@ -415,12 +415,15 @@ void plan_bwd_weight(tcr_handle* h) {
   }
 }
 
-// Device table of the grouped weight-gradient launch (pointers are workspace addresses: static per handle).
+// Device table of the grouped weight-gradient launch (pointers are workspace addresses: static per handle).  Only the layers
+// whose weights are trained (tcr_set_trainable) are in it; each keeps its own row partition (plan_bwd_weight), so its partial
+// sums, and its gradient, are those of the full table.
 int build_dw_table(tcr_handle* h) {
   std::vector<DwLayer> tab;
   int cta = 0;
   size_t smem = 0;
   auto add = [&](ConvPlan& cv, const float* xd, const float* xb, int xk, const float* dz, int mask) {
+    if (!h->conv_w_trained((int)(&cv - &h->convs[0]))) return;
     DwLayer L;
     L.x_data = xd; L.x_bnf = xb; L.x_kind = xk;
     L.dz = dz; L.y = cv.y; L.bnf = cv.bnf; L.bsum = cv.bsum; L.mask_relu = mask;
@@ -448,12 +451,33 @@ int build_dw_table(tcr_handle* h) {
   h->dw_ctas = cta;
   h->dw_smem = smem;
   h->n_dw_layers = (int)tab.size();
-  void* p = nullptr;
-  if (cudaMalloc(&p, tab.size() * sizeof(DwLayer)) != cudaSuccess) return TCR_ERR_CUDA;
-  h->allocs.push_back(p);
-  h->d_dw_layers = (DwLayer*)p;
-  if (cudaMemcpy(p, tab.data(), tab.size() * sizeof(DwLayer), cudaMemcpyHostToDevice) != cudaSuccess) return TCR_ERR_CUDA;
+  h->dw_conv0 = h->conv_w_trained(0) ? 1 : 0;
+  if (!h->d_dw_layers) {             // sized for every layer: a later tcr_set_trainable rewrites it in place
+    void* p = nullptr;
+    if (cudaMalloc(&p, h->convs.size() * sizeof(DwLayer)) != cudaSuccess) return TCR_ERR_CUDA;
+    h->allocs.push_back(p);
+    h->d_dw_layers = (DwLayer*)p;
+  }
+  if (!tab.empty() && cudaMemcpy(h->d_dw_layers, tab.data(), tab.size() * sizeof(DwLayer), cudaMemcpyHostToDevice) != cudaSuccess)
+    return TCR_ERR_CUDA;
   return 0;
+}
+
+// Backward-data phases a step runs: 2 per block from the last block down ((1) conv_b -> g of conv_a, (2) conv_a + shortcut ->
+// gradient at the block input), only as deep as the lowest conv with a trained variable needs.  conv_b / down of block i read
+// gblk_i (phase (2) of block i + 1), conv_a of block i phase (1) of block i, conv0 phase (2) of block 0.  0: only fc / fc2.
+// The last block's conv_b / down take phase (1) as well: the head leaves their BatchNorm-backward sums as records, and the
+// resident kernel publishes them (with its own summation order) when it starts.
+int plan_bwd_phases(const tcr_handle* h) {
+  const int nb = (int)h->blocks.size();
+  int phases = h->conv_any_trained(0) ? 2 * nb : 0;
+  for (int i = 0; i < nb; ++i) {
+    const BlockPlan& b = h->blocks[(size_t)i];
+    const int above = 2 * (nb - 1 - i);
+    if (h->conv_any_trained(b.b) || (b.down >= 0 && h->conv_any_trained(b.down))) phases = std::max(phases, std::max(above, 1));
+    if (h->conv_any_trained(b.a)) phases = std::max(phases, above + 1);
+  }
+  return phases;
 }
 
 template <int K, bool WSMEM>
@@ -514,8 +538,25 @@ int net_weight_transpose(tcr_handle* h, const float* params, cudaStream_t s) {
   return 0;
 }
 
+// BatchNorm-backward sums of one layer from the per-cluster records its producer left, published to ConvPlan::bsum.  A truncated
+// backward-data chain (tcr_set_trainable) leaves the records of its lowest layers without the consumer launch that would
+// publish them; this is that consumer's prologue (bsum_build with the same 256 threads, hence the same bits).
+__global__ void __launch_bounds__(kThreads) bsum_publish_kernel(BsumSrc bs, int C) {
+  pdl_wait();
+  __shared__ float sb[kThreads], scratch[kThreads];
+  bsum_build(bs, bs.bsum, C, sb, scratch, true);
+}
+static int publish_bsums(tcr_handle* h, int l, cudaStream_t s) {
+  if (!h->conv_any_trained(l)) return 0;
+  const ConvPlan& cv = h->convs[(size_t)l];
+  TCR_LAUNCH("records_sum", bsum_publish_kernel, dim3(1), dim3(kThreads), 0, s, bsum_src(h, cv), cv.cout);
+  return 0;
+}
+
 int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s) {
-  for (int i = (int)h->blocks.size() - 1; i >= 0; --i) {
+  const int nb = (int)h->blocks.size(), phases = h->bwd_phases;
+  int done = 0;
+  for (int i = nb - 1; i >= 0 && done < phases; --i) {
     BlockPlan& b = h->blocks[i];
     ConvPlan& ca = h->convs[b.a];
     ConvPlan& cb = h->convs[b.b];
@@ -532,6 +573,11 @@ int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s)
       if (rc) return rc;
       ca.b_gc = gc;
       if (sync_bn_on(h) && (rc = sync_records(h, ca.bpart, gc, 2 * ca.cout, ca.bsync, s))) return rc;
+    }
+    if (++done == phases) {          // truncated after (1): conv_a's records and the shortcut conv's are still unpublished
+      int rc = publish_bsums(h, b.a, s);
+      if (!rc && b.down >= 0) rc = publish_bsums(h, b.down, s);
+      return rc;
     }
     // (2) conv_a (+ down conv | identity): dx is the gradient at the block input
     {
@@ -576,21 +622,31 @@ int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s)
         if (sync_bn_on(h) && (rc = sync_records(h, h->convs[0].bpart, gc, 2 * h->convs[0].cout, h->convs[0].bsync, s))) return rc;
       }
     }
+    if (++done == phases && i > 0) {  // truncated after (2): the previous block's conv_b / shortcut records are unpublished
+      const BlockPlan& pb = h->blocks[i - 1];
+      int rc = publish_bsums(h, pb.b, s);
+      if (!rc && pb.down >= 0) rc = publish_bsums(h, pb.down, s);
+      return rc;
+    }
   }
+  // conv0's records: its weight-gradient CTAs sum them (net_weight_gradients); without its weights in that launch, here
+  if (phases == 2 * nb && !h->dw_conv0) return publish_bsums(h, 0, s);
   return 0;
 }
 
 // weight gradients: every layer's inputs are final now -> one grouped launch over all layers
 int net_weight_gradients(tcr_handle* h, const float* feat, int n, cudaStream_t s) {
+  if (h->dw_ctas == 0) return 0;     // no conv weight is trained
   {
     auto kfn = dw_grouped_kernel;
 #ifndef TCR_EMU
     static SmemOptIn optin;
     if (optin.ensure(kfn, h->dw_smem) != cudaSuccess) return TCR_ERR_CUDA;
 #endif
-    // conv0's BatchNorm-backward sums have no backward-data consumer: its weight-gradient CTAs add the records themselves
+    // conv0's BatchNorm-backward sums have no backward-data consumer: its weight-gradient CTAs add the records themselves.
+    // Row 0 of a table without conv0 is a layer whose sums are published: it reads them like every other row.
     const ConvPlan& c0 = h->convs[0];
-    const BsumSrc bs0 = bsum_src(h, c0);
+    const BsumSrc bs0 = h->dw_conv0 ? bsum_src(h, c0) : BsumSrc{nullptr, 0, nullptr};
     const float inv_scale = sync_bn_on(h) ? 1.0f / (float)h->world : 1.0f;         // SyncBN: BatchNorm-backward means over the global rows
     TCR_LAUNCH("dw_grouped", kfn, dim3(h->dw_ctas), dim3(kDwThreads), h->dw_smem, s, h->d_dw_layers, h->n_dw_layers, n, feat, h->d_timeline, bs0,
                inv_scale);

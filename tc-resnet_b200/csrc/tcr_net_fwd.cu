@@ -383,8 +383,6 @@ static int ws_alloc(tcr_handle* h, T** p, size_t count) {
   } while (0)
 
 void plan_bwd_weight(tcr_handle* h);   // tcr_net_bwd.cu
-int build_opt_segments(tcr_handle* h); // tcr_optim.cu
-int build_dw_table(tcr_handle* h);     // tcr_net_bwd.cu
 
 int net_alloc_workspace(tcr_handle* h) {
   const size_t N = (size_t)h->cfg.max_batch;
@@ -428,9 +426,7 @@ int net_alloc_workspace(tcr_handle* h) {
     cudaMemset(h->d_timeline, 0, sizeof(long long) * 16 * 8192);
   }
   if (cudaMallocHost((void**)&h->h_hyper, sizeof(Hyper)) != cudaSuccess) return TCR_ERR_CUDA;
-  int rc = build_dw_table(h);
-  if (rc) return rc;
-  return build_opt_segments(h);
+  return build_trainable_plans(h);
 }
 
 // Thread-block cluster size of the conv / head launches: 8 CTAs add their BatchNorm partial sums through distributed shared

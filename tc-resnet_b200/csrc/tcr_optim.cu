@@ -29,6 +29,7 @@ __device__ __forceinline__ int find_segment(const OptSegment* segs, int nsegs, i
   return lo;
 }
 
+template <bool kSubset>
 __device__ __forceinline__ void grad_finalize_body(const GradArgs& a, const int vb, float* s_red) {
   const OptSegment* __restrict__ segs = a.segs;
   const int nsegs = a.nsegs, fc_seg = a.fc_seg, fc_R = a.fc_R;
@@ -47,7 +48,7 @@ __device__ __forceinline__ void grad_finalize_body(const GradArgs& a, const int 
     const float* part = si == fc_seg ? fc_part : sg.part;
     const int R = si == fc_seg ? fc_R : sg.R;
     float g = 0.f;
-    if (part) {                      // fixed summation order (deterministic); many loads in flight: the fc partials come one per
+    if (part && (!kSubset || sg.train)) {                    // fixed summation order (deterministic); many loads in flight: the fc partials come one per
       float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};      // CTA of the resident forward kernel (148 records), and a
       int r = 0;                                                    // dependent round trip per 8 records made them the kernel's tail
       for (; r + 32 <= R; r += 32) {
@@ -69,11 +70,11 @@ __device__ __forceinline__ void grad_finalize_body(const GradArgs& a, const int 
     if (sg.decay) {
       const float w = params[p];
       g = fmaf(weight_decay, w, g);
-      w2 = w * w;
+      w2 = w * w;                    // frozen weights too: total_loss keeps the decay of every weight (factory/audio_nets.py:175-182)
     } else {
       g *= a.bn_grad_scale;          // gamma / beta (the only segments without decay)
     }
-    grads[p] = g;
+    grads[p] = !kSubset || sg.train ? g : 0.f;
   }
   w2 = warp_sum(w2);
   if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = w2;
@@ -84,10 +85,12 @@ __device__ __forceinline__ void grad_finalize_body(const GradArgs& a, const int 
     l2part[vb] = s;
   }
 }
+// kSubset: some segments are frozen (tcr_set_trainable); the default instantiation is the code without the check
+template <bool kSubset>
 __global__ void __launch_bounds__(kOptThreads) grad_finalize_kernel(GradArgs a) {
   pdl_wait();
   __shared__ float s_red[kOptThreads / 32];
-  grad_finalize_body(a, (int)blockIdx.x, s_red);
+  grad_finalize_body<kSubset>(a, (int)blockIdx.x, s_red);
 }
 
 struct UpdateArgs {
@@ -110,7 +113,14 @@ struct UpdateArgs {
   float* slots2;                                       // Adam v / RMSProp mom (`slots`: Adam m / RMSProp ms)
   float beta1, beta2, epsilon, rho;
   float beta1_power, beta2_power;                      // Adam: beta^t before this step
+  // trainable subset / weight EMA (after the fields above: the default instantiations read the same parameter offsets)
+  const OptSegment* segs; int nsegs;                   // kUpdSubset: frozen segments are skipped
+  float* ema; float ema_one_minus;                     // kUpdEma: shadow, 1 - ema_decay
 };
+
+// Variants of the update kernel (template flags): the default step instantiates neither, so its code is what it was.
+constexpr int kUpdSubset = 1;        // some variables are frozen (tcr_set_trainable)
+constexpr int kUpdEma = 2;           // tcr_step_args::ema is set
 
 // System-scope flag accesses for the cross-GPU arrival barrier.
 __device__ __forceinline__ void st_release_sys(unsigned* p, unsigned v) {
@@ -130,7 +140,7 @@ __device__ __forceinline__ unsigned ld_acquire_sys(const unsigned* p) {
 #endif
 }
 
-template <int kOpt>
+template <int kOpt, int kVar>
 __global__ void __launch_bounds__(kOptThreads) update_kernel(UpdateArgs a) {
   pdl_wait();
   if (a.p2p_world > 1) {
@@ -160,11 +170,14 @@ __global__ void __launch_bounds__(kOptThreads) update_kernel(UpdateArgs a) {
     }
     const float g = gsum * a.grad_scale;
     if (a.grads_out) a.grads_out[p] = g;
-    if (a.apply) {
+    bool trained = true;
+    if constexpr ((kVar & kUpdSubset) != 0) trained = a.segs[find_segment(a.segs, a.nsegs, p)].train != 0;
+    if (a.apply && trained) {
+      float w;
       if constexpr (kOpt == TCR_OPT_MOMENTUM) {
         const float m = fmaf(a.slots[p], a.momentum, g);     // accum = accum * momentum + grad
         a.slots[p] = m;
-        a.params[p] = a.params[p] - a.lr * m;                // var -= lr * accum
+        w = a.params[p] - a.lr * m;                          // var -= lr * accum
       } else if constexpr (kOpt == TCR_OPT_ADAM) {
         // IEEE sqrtf and division (the library is built without fast-math): alpha is the same bits in every thread
         const float alpha = a.lr * sqrtf(1.f - a.beta2_power) / (1.f - a.beta1_power);
@@ -173,7 +186,7 @@ __global__ void __launch_bounds__(kOptThreads) update_kernel(UpdateArgs a) {
         v += (g * g - v) * (1.f - a.beta2);
         a.slots[p] = m;
         a.slots2[p] = v;
-        a.params[p] = a.params[p] - (m * alpha) / (sqrtf(v) + a.epsilon);
+        w = a.params[p] - (m * alpha) / (sqrtf(v) + a.epsilon);
       } else {
         static_assert(kOpt == TCR_OPT_RMSPROP, "unknown optimizer");
         float ms = a.slots[p];
@@ -181,7 +194,12 @@ __global__ void __launch_bounds__(kOptThreads) update_kernel(UpdateArgs a) {
         const float mom = a.slots2[p] * a.momentum + (g * a.lr) / sqrtf(ms + a.epsilon);
         a.slots[p] = ms;
         a.slots2[p] = mom;
-        a.params[p] = a.params[p] - mom;
+        w = a.params[p] - mom;
+      }
+      a.params[p] = w;
+      if constexpr ((kVar & kUpdEma) != 0) {               // ExponentialMovingAverage.apply after the train op, on the new weight
+        const float s = a.ema[p];
+        a.ema[p] = s - (s - w) * a.ema_one_minus;            // assign_moving_average, zero_debias=False
       }
     }
   }
@@ -253,24 +271,29 @@ __global__ void __launch_bounds__(1024) loss_only_kernel(const OptSegment* __res
 }
 
 
+// One segment per trainable row of the table, in table order; rebuilt by tcr_set_trainable (the `train` flags).
 int build_opt_segments(tcr_handle* h) {
   std::vector<OptSegment> segs;
   std::vector<MovingSegment> msegs;
   for (auto& cv : h->convs) {
-    segs.push_back(OptSegment{cv.w_off, cv.wnumel(), cv.dwpart, cv.dw_R, 1});
-    segs.push_back(OptSegment{cv.beta_off, cv.cout, cv.bsum, 1, 0});             // d beta  = sum dz
-    segs.push_back(OptSegment{cv.gamma_off, cv.cout, cv.bsum + cv.cout, 1, 0});  // d gamma = sum dz * xhat
+    segs.push_back(OptSegment{cv.w_off, cv.wnumel(), cv.dwpart, cv.dw_R, 1, 1});
+    segs.push_back(OptSegment{cv.beta_off, cv.cout, cv.bsum, 1, 0, 1});             // d beta  = sum dz
+    segs.push_back(OptSegment{cv.gamma_off, cv.cout, cv.bsum + cv.cout, 1, 0, 1});  // d gamma = sum dz * xhat
     msegs.push_back(MovingSegment{cv.mm_off, cv.mv_off, cv.cout, cv.bnf, cv.var, cv.t_out});
   }
-  segs.push_back(OptSegment{h->fc_off, (int64_t)h->c_last * h->cfg.num_classes, h->d_dwfc_part, 1, 1});
-  segs.push_back(OptSegment{h->fc2_off, (int64_t)h->c_last * 2, nullptr, 0, 1});   // dead "ranges" head: decay only
+  segs.push_back(OptSegment{h->fc_off, (int64_t)h->c_last * h->cfg.num_classes, h->d_dwfc_part, 1, 1, 1});
+  segs.push_back(OptSegment{h->fc2_off, (int64_t)h->c_last * 2, nullptr, 0, 1, 1});   // dead "ranges" head: decay only
+  for (size_t i = 0; i < segs.size(); ++i) segs[i].train = h->row_trained((int)i) ? 1 : 0;
   h->n_segs = (int)segs.size();
   h->n_msegs = (int)msegs.size();
   void* p = nullptr;
-  if (cudaMalloc(&p, segs.size() * sizeof(OptSegment)) != cudaSuccess) return TCR_ERR_CUDA;
-  h->allocs.push_back(p);
-  h->d_segs = (OptSegment*)p;
-  if (cudaMemcpy(p, segs.data(), segs.size() * sizeof(OptSegment), cudaMemcpyHostToDevice) != cudaSuccess) return TCR_ERR_CUDA;
+  if (!h->d_segs) {
+    if (cudaMalloc(&p, segs.size() * sizeof(OptSegment)) != cudaSuccess) return TCR_ERR_CUDA;
+    h->allocs.push_back(p);
+    h->d_segs = (OptSegment*)p;
+  }
+  if (cudaMemcpy(h->d_segs, segs.data(), segs.size() * sizeof(OptSegment), cudaMemcpyHostToDevice) != cudaSuccess) return TCR_ERR_CUDA;
+  if (h->d_msegs) return 0;
   if (cudaMalloc(&p, msegs.size() * sizeof(MovingSegment)) != cudaSuccess) return TCR_ERR_CUDA;
   h->allocs.push_back(p);
   h->d_msegs = (MovingSegment*)p;
@@ -280,6 +303,17 @@ int build_opt_segments(tcr_handle* h) {
 
 static int fc_segment(const tcr_handle* h) { return (int)h->convs.size() * 3; }
 
+template <int kOpt>
+static int launch_update(int var, const UpdateArgs& u, int grid, cudaStream_t s) {
+  switch (var) {
+    case kUpdSubset: TCR_LAUNCH("update", (update_kernel<kOpt, kUpdSubset>), dim3(grid), dim3(kOptThreads), 0, s, u); break;
+    case kUpdEma: TCR_LAUNCH("update", (update_kernel<kOpt, kUpdEma>), dim3(grid), dim3(kOptThreads), 0, s, u); break;
+    case kUpdSubset | kUpdEma: TCR_LAUNCH("update", (update_kernel<kOpt, kUpdSubset | kUpdEma>), dim3(grid), dim3(kOptThreads), 0, s, u); break;
+    default: TCR_LAUNCH("update", (update_kernel<kOpt, 0>), dim3(grid), dim3(kOptThreads), 0, s, u); break;
+  }
+  return 0;
+}
+
 int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s) {
   const int blocks = (int)((h->n_train + kOptThreads - 1) / kOptThreads);
   if (blocks > 4096) { set_error("parameter count too large for the l2 partial buffer"); return TCR_ERR_UNSUPPORTED; }
@@ -288,7 +322,8 @@ int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s) {
   float* grads = p2p ? h->p2p.grads + (size_t)(h->p2p.step & 1u) * h->n_train : h->d_grads;
   GradArgs ga{h->d_segs, h->n_segs, h->n_train, fc_segment(h), h->d_dwfc_part, h->fc_records, a->params, a->weight_decay,
               grads, h->d_l2part, sync_bn_on(h) ? 1.0f / (float)h->world : 1.0f};
-  TCR_LAUNCH("grad_finalize", grad_finalize_kernel, dim3(blocks), dim3(kOptThreads), 0, s, ga);
+  if (h->frozen_rows > 0) TCR_LAUNCH("grad_finalize", grad_finalize_kernel<true>, dim3(blocks), dim3(kOptThreads), 0, s, ga);
+  else TCR_LAUNCH("grad_finalize", grad_finalize_kernel<false>, dim3(blocks), dim3(kOptThreads), 0, s, ga);
   if (!p2p && h->comm && h->world > 1) {
     int rc = comm_allreduce_sum(h, h->d_grads, h->n_train, s);
     if (rc) return rc;
@@ -312,13 +347,15 @@ int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s) {
   u.slots2 = a->slots2;
   u.beta1 = a->beta1; u.beta2 = a->beta2; u.epsilon = a->epsilon; u.rho = a->rho;
   u.beta1_power = a->beta1_power; u.beta2_power = a->beta2_power;
-  const dim3 grid(blocks + h->n_msegs + 1);
+  u.segs = h->d_segs; u.nsegs = h->n_segs;
+  u.ema = a->ema;
+  u.ema_one_minus = 1.0f - a->ema_decay;   // fp32, as TF forms 1 - decay from the float32 decay tensor (moving_averages.py)
+  const int var = (h->frozen_rows > 0 ? kUpdSubset : 0) | (a->ema ? kUpdEma : 0);
   switch (a->optimizer) {            // the kind was validated by train_step_impl
-    case TCR_OPT_ADAM: TCR_LAUNCH("update", update_kernel<TCR_OPT_ADAM>, grid, dim3(kOptThreads), 0, s, u); break;
-    case TCR_OPT_RMSPROP: TCR_LAUNCH("update", update_kernel<TCR_OPT_RMSPROP>, grid, dim3(kOptThreads), 0, s, u); break;
-    default: TCR_LAUNCH("update", update_kernel<TCR_OPT_MOMENTUM>, grid, dim3(kOptThreads), 0, s, u); break;
+    case TCR_OPT_ADAM: return launch_update<TCR_OPT_ADAM>(var, u, blocks + h->n_msegs + 1, s);
+    case TCR_OPT_RMSPROP: return launch_update<TCR_OPT_RMSPROP>(var, u, blocks + h->n_msegs + 1, s);
+    default: return launch_update<TCR_OPT_MOMENTUM>(var, u, blocks + h->n_msegs + 1, s);
   }
-  return 0;
 }
 
 int launch_loss_only(tcr_handle* h, const float* params, float weight_decay, int n, float* losses, cudaStream_t s) {

@@ -77,6 +77,11 @@ struct tcr_handle {
   tcr::OptSegment* d_segs = nullptr; int n_segs = 0;
   tcr::MovingSegment* d_msegs = nullptr; int n_msegs = 0;
   tcr::DwLayer* d_dw_layers = nullptr; int n_dw_layers = 0; int dw_ctas = 0; size_t dw_smem = 0;
+  // trainable subset (tcr_set_trainable): one flag per trainable row of `table`; the plans above are rebuilt from it
+  std::vector<int> train_rows;
+  int frozen_rows = 0;               // > 0: the update kernel checks each parameter's segment
+  int dw_conv0 = 1;                  // conv0's weights are in the grouped weight-gradient table
+  int bwd_phases = 0;                // backward-data phases (2 per block, from the last block down) the step runs
   std::vector<void*> allocs;
   int64_t workspace_bytes = 0;
   // data-parallel
@@ -101,4 +106,9 @@ struct tcr_handle {
   int fc_records = 0;                // per-CTA records of the fc weight gradient left by the last head launch
   unsigned* d_gridbar = nullptr;    // arrival counter of the resident kernel's grid barrier (monotonic, never reset)
   long long* d_timeline = nullptr;   // TCR_DEBUG_TIMELINE=1: per-CTA phase stamps (fwd kernels: 8 slots per CTA; dw: after)
+
+  // Trainable rows in table order: conv l -> 3l (weights), 3l + 1 (beta), 3l + 2 (gamma); then fc, fc2.
+  bool row_trained(int row) const { return train_rows.empty() || train_rows[(size_t)row] != 0; }
+  bool conv_w_trained(int l) const { return row_trained(3 * l); }
+  bool conv_any_trained(int l) const { return row_trained(3 * l) || row_trained(3 * l + 1) || row_trained(3 * l + 2); }
 };

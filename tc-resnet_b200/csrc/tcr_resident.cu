@@ -65,6 +65,7 @@ struct ResCall {                     // per call
   float* logits; float* probs;
   int n; unsigned bar_base; float inv_n;
   long long* tl;                     // debug timeline (TCR_DEBUG_TIMELINE=1): [cta][32] globaltimer stamps, else null
+  int phases;                        // backward kernel: phases to run from the last block down (tcr_handle::bwd_phases, >= 1)
 };
 
 __device__ __forceinline__ void res_stamp(const ResCall& c, int slot) {
@@ -498,6 +499,8 @@ __device__ __noinline__ void res_bwd_epilogue(const float* dxs, int rcap, int KS
   __syncthreads();
 }
 
+// kTrunc: the chain stops after c.phases phases (tcr_set_trainable); the full chain's instantiation has no phase count in it
+template <bool kTrunc>
 __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __grid_constant__ ResProgram P, const __grid_constant__ ResCall c) {
   TCR_DYNAMIC_SMEM(smem_raw);
   float* smem = reinterpret_cast<float*>(smem_raw);
@@ -548,8 +551,8 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
     const BsDst sd = Dd ? BsDst{bsr + Dd->bs, Dd->bsum, Dd->cout} : sa;
     res_bsums(Lb.brec, sa, Dd ? Dd->brec : nullptr, sd, Dd ? 2 : 1, G, red, cta == 0);
   }
-  int slot = 1;
-  for (int bi = nb - 1; bi >= 0; --bi) {
+  int slot = 1, done = 0;            // done: phases finished; each ends with the published sums of the layer(s) it produced
+  for (int bi = nb - 1; bi >= 0 && (!kTrunc || done < c.phases); --bi) {
     const RBlock& B = P.blk[bi];
     const RConv& La = P.conv[B.a];
     const RConv& Lb = P.conv[B.b];
@@ -574,20 +577,22 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
       gbar_arrive(P.bar);
       target += (unsigned)G;
       // ---- nobody waits for the rest of this phase: the next phase's (conv_a) tensors and bank(s) travel during the barrier ----
-      const int Ca = La.cin, Rin = Ue * La.t_in;
-      res_fetch(ysr, La.y + (size_t)u0 * B.t * C, R * (C >> 2));
-      if (Dd) res_fetch(ysr + P.umax * B.t * C, Dd->y + (size_t)u0 * B.t * C, R * (C >> 2));
-      {                                 // y / out of the layer(s) below into ypr (the epilogue has consumed y_a)
-        const int n4 = Rin * (Ca >> 2), cap = P.umax * La.t_in * Ca;
-        if (bi > 0) {
-          const RBlock& Bp = P.blk[bi - 1];
-          res_fetch(ypr, P.conv[Bp.b].y + (size_t)u0 * La.t_in * Ca, n4);
-          res_fetch(ypr + cap, (Bp.down >= 0 ? P.conv[Bp.down].y : Bp.out) + (size_t)u0 * La.t_in * Ca, n4);
-        } else {
-          res_fetch(ypr, P.conv[0].y + (size_t)u0 * La.t_in * Ca, n4);
+      if (!kTrunc || ++done < c.phases) {
+        const int Ca = La.cin, Rin = Ue * La.t_in;
+        res_fetch(ysr, La.y + (size_t)u0 * B.t * C, R * (C >> 2));
+        if (Dd) res_fetch(ysr + P.umax * B.t * C, Dd->y + (size_t)u0 * B.t * C, R * (C >> 2));
+        {                               // y / out of the layer(s) below into ypr (the epilogue has consumed y_a)
+          const int n4 = Rin * (Ca >> 2), cap = P.umax * La.t_in * Ca;
+          if (bi > 0) {
+            const RBlock& Bp = P.blk[bi - 1];
+            res_fetch(ypr, P.conv[Bp.b].y + (size_t)u0 * La.t_in * Ca, n4);
+            res_fetch(ypr + cap, (Bp.down >= 0 ? P.conv[Bp.down].y : Bp.out) + (size_t)u0 * La.t_in * Ca, n4);
+          } else {
+            res_fetch(ypr, P.conv[0].y + (size_t)u0 * La.t_in * Ca, n4);
+          }
         }
+        res_load_bank(smem + P.b_w, La.wT, (unsigned)(La.k * La.cin * La.cout), Dd ? Dd->wT : nullptr, Dd ? (unsigned)(Dd->cin * Dd->cout) : 0u, wbar);
       }
-      res_load_bank(smem + P.b_w, La.wT, (unsigned)(La.k * La.cin * La.cout), Dd ? Dd->wT : nullptr, Dd ? (unsigned)(Dd->cin * Dd->cout) : 0u, wbar);
       res_stamp(c, slot + 3);
       gbar_wait(P.bar, target);
       res_stamp(c, slot + 4);
@@ -595,6 +600,7 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
       res_bsums(La.brec, sa, nullptr, sa, 1, G, red, cta == 0);
       slot += 5;
     }
+    if (kTrunc && done == c.phases) break;
     // =============== phase Ba: conv_a (k 9, stride S) + shortcut conv / identity: gradient at the block input ===============
     {
       const int C = B.c, Ca = La.cin, S = La.stride, COS = chan_stride(C);
@@ -630,7 +636,7 @@ __global__ void __launch_bounds__(kResThreads, 1) resident_bwd_kernel(const __gr
       gbar_arrive(P.bar);
       target += (unsigned)G;
       // ---- nobody waits for the rest of this phase: the next phase's tensors (ysr and ypr are dead) and bank travel ----
-      if (bi > 0) {
+      if (kTrunc ? ++done < c.phases : bi > 0) {   // (truncated: done < phases implies bi > 0)
         const RBlock& Bp = P.blk[bi - 1];
         const RConv& Lpb = P.conv[Bp.b];
         res_fetch(ysr, Lpb.y + (size_t)u0 * Bp.t * Bp.c, Ue * Bp.t * (Bp.c >> 2));
@@ -876,14 +882,15 @@ static ResidentState* resident_state(tcr_handle* h) {
 #ifndef TCR_EMU
   if (S->smem_f > 227 * 1024) return S;
   // the opt-in limit is a property of the FUNCTION, shared by every handle of the process: it is only ever raised
-  static SmemOptIn optin_f, optin_b;
+  static SmemOptIn optin_f, optin_b, optin_t;
   if (optin_f.ensure(resident_fwd_kernel, S->smem_f) != cudaSuccess) return S;
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resident_fwd_kernel, kResThreads, S->smem_f) != cudaSuccess || per_sm < 1) return S;
   if (want == kResidentFwdBwdData) {
     if (S->smem_b > 227 * 1024 ||
-        optin_b.ensure(resident_bwd_kernel, S->smem_b) != cudaSuccess ||
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resident_bwd_kernel, kResThreads, S->smem_b) != cudaSuccess || per_sm < 1)
+        optin_b.ensure(resident_bwd_kernel<false>, S->smem_b) != cudaSuccess || optin_t.ensure(resident_bwd_kernel<true>, S->smem_b) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resident_bwd_kernel<false>, kResThreads, S->smem_b) != cudaSuccess || per_sm < 1 ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, resident_bwd_kernel<true>, kResThreads, S->smem_b) != cudaSuccess || per_sm < 1)
       want = kResidentFwd;
   }
 #endif
@@ -961,16 +968,19 @@ int resident_forward(tcr_handle* h, const float* feat, const tcr_step_args* a, c
 }
 
 // The backward-data chain as the resident kernel.  It leaves every layer's masked gradient (ConvPlan::g, BlockPlan::gblk) and
-// the published BatchNorm-backward sums, i.e. what the conv_bwd_data launches of net_backward_data leave.
+// the published BatchNorm-backward sums, i.e. what the conv_bwd_data launches of net_backward_data leave, down to the depth
+// the trainable set needs (tcr_handle::bwd_phases; the caller launches nothing when that is 0).
 int resident_backward_data(tcr_handle* h, const float* feat, const tcr_step_args* a, cudaStream_t s) {
   ResidentState* S = resident_state(h);
   const int G = std::min(S->grid_max, a->n);
   ResCall c = res_call(h, feat, a);
   c.tl = h->d_timeline ? h->d_timeline + 148 * 32 : nullptr;
   c.bar_base = S->bar_next;
-  S->bar_next += (unsigned)G * (unsigned)(2 * h->blocks.size());
+  c.phases = h->bwd_phases;                           // the chain stops at the lowest conv with a trained variable
+  S->bar_next += (unsigned)G * (unsigned)c.phases;    // one grid barrier per phase run
   for (auto& cv : h->convs) cv.b_gc = 0;              // every layer's sums are published: nobody sums records afterwards
-  return res_launch(h, "resident_bwd_data", resident_bwd_kernel, G, S->smem_b, c, s);
+  const bool full = c.phases == 2 * (int)h->blocks.size();
+  return res_launch(h, "resident_bwd_data", full ? resident_bwd_kernel<false> : resident_bwd_kernel<true>, G, S->smem_b, c, s);
 }
 
 }  // namespace tcr

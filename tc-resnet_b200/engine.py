@@ -94,6 +94,7 @@ class Engine:
         self.frames, self.features = int(self.info.frames), int(self.info.features)
         self.num_classes = int(num_classes)
         self.table = self._read_table()
+        self.trained = set(self.trainable_names)
         self.world_size = 1
 
     # ------------------------------------------------------------------ plumbing
@@ -157,6 +158,41 @@ class Engine:
         second = torch.zeros(self.num_trainable, dtype=torch.float32, device=self.device) if OPTIMIZER_SLOT_NAMES[kind][1] else None
         return first, second
 
+    @property
+    def trainable_names(self):
+        """Names of the trainable variables in table order (tf.trainable_variables() order)."""
+        return [d["name"] for d in self.table if d["trainable"]]
+
+    def set_trainable(self, names_or_mask=None):
+        """The variables the training steps train (--trainable_scopes, tcr_set_trainable): None = all (the default), an iterable of
+        variable names, or one bool per trainable variable in table order.  Frozen variables get a zero gradient and keep their
+        values and optimizer slots; the step skips the backward work only they needed.  Returns the set of trained names."""
+        names = self.trainable_names
+        torch.cuda.current_stream(self.device).synchronize()      # the plans are rewritten in place: no step may be queued
+        if names_or_mask is None:
+            L.check(self.lib, self.lib.tcr_set_trainable(self._h, None, 0), "tcr_set_trainable")
+            self.trained = set(names)
+            return self.trained
+        sel = list(names_or_mask)
+        if sel and all(isinstance(x, (bool, np.bool_)) for x in sel):
+            if len(sel) != len(names):
+                raise ValueError(f"{len(sel)} flags for {len(names)} trainable variables")
+            mask = [bool(x) for x in sel]
+        else:
+            unknown = set(sel) - set(names)
+            if unknown:
+                raise KeyError(f"not trainable variables of this model: {sorted(unknown)}")
+            mask = [n in set(sel) for n in names]
+        flags = (C.c_int32 * len(mask))(*[int(m) for m in mask])
+        L.check(self.lib, self.lib.tcr_set_trainable(self._h, flags, len(mask)), "tcr_set_trainable")
+        self.trained = {n for n, m in zip(names, mask) if m}
+        return self.trained
+
+    def new_ema(self, params: torch.Tensor) -> torch.Tensor:
+        """Flat shadow buffer for tcr_step_args::ema, initialised to `params` (TF initialises each `<var>/ExponentialMovingAverage`
+        to the variable's initial value)."""
+        return params.detach().clone().contiguous()
+
     def variables_to_dict(self, params: torch.Tensor, moving: Optional[torch.Tensor] = None) -> Dict[str, np.ndarray]:
         """{TF variable name: ndarray} — the reference's `var_names_to_values` form (helper/trainer.py:145-154)."""
         p = params.detach().cpu().numpy()
@@ -169,10 +205,13 @@ class Engine:
         return out
 
     def variables_from_dict(self, values: Dict[str, np.ndarray], params: torch.Tensor, moving: Optional[torch.Tensor] = None,
-                            strict: bool = True):
+                            strict: bool = True, only=None):
+        """only: predicate on names; the variables it rejects are skipped (neither read nor required)."""
         p = params.detach().cpu().numpy().copy()
         m = moving.detach().cpu().numpy().copy() if moving is not None else None
         for d in self.table:
+            if only is not None and not only(d["name"]):
+                continue
             if d["name"] not in values:
                 if strict:
                     raise KeyError(d["name"])
@@ -234,7 +273,8 @@ class Engine:
                    want_outputs: bool = False, want_grads: bool = False, apply_update: bool = True,
                    losses: Optional[torch.Tensor] = None, clips: Optional[torch.Tensor] = None,
                    background: Optional[torch.Tensor] = None, input_resident: bool = False, *,
-                   optimizer: Optional[dict] = None, slots2: Optional[torch.Tensor] = None):
+                   optimizer: Optional[dict] = None, slots2: Optional[torch.Tensor] = None,
+                   ema: Optional[torch.Tensor] = None, ema_decay: float = 0.999):
         """optimizer: None or dict(kind="mom" | "gd") for the momentum step (`momentum`), dict(kind="adam", beta1=, beta2=,
         epsilon=, beta1_power=, beta2_power=) or dict(kind="rmsprop", decay=, momentum=, epsilon=) (missing hyper-parameters
         take TF's defaults, OPTIMIZER_DEFAULTS).  Adam / RMSProp keep their second slot in `slots2` (new_optimizer_state);
@@ -242,7 +282,9 @@ class Engine:
         clips (uint8 CUDA tensor of n packed tcr_augment_clip records) + int16 `inputs` [n, stride]: the step starts with
         the device input stage (decode, shift, background mix, clip) instead of taking decoded fp32 samples.
         input_resident=True: `inputs` is final when the call is made (nothing queued on the current stream writes it); the
-        front-end then runs ahead on the library's own stream and overlaps the previous step's tail (tcr_step_args::input_resident)."""
+        front-end then runs ahead on the library's own stream and overlaps the previous step's tail (tcr_step_args::input_resident).
+        ema (new_ema) / ema_decay: after the update, the shadow of every trained parameter moves toward the new weight
+        (tf.train.ExponentialMovingAverage(ema_decay).apply(variables_to_train), tcr_step_args::ema)."""
         n = inputs.shape[0]
         a = L.TcrStepArgs()
         if clips is not None:
@@ -267,6 +309,7 @@ class Engine:
         a.apply_update = int(apply_update)
         a.input_resident = int(bool(input_resident))
         _set_optimizer(a, optimizer, self._ptr(slots2))
+        a.ema, a.ema_decay = self._ptr(ema), float(ema_decay)
         L.check(self.lib, self.lib.tcr_train_step(self._h, C.byref(a), self._stream), "tcr_train_step")
         return out
 
@@ -369,8 +412,8 @@ class HostFeed:
     def submit(self, h_inputs: torch.Tensor, h_onehot: torch.Tensor, params, slots, moving, learning_rate, momentum=0.9,
                weight_decay=1e-4, dropout_seed=0, input_is_features=False, h_clips: Optional[torch.Tensor] = None,
                background: Optional[torch.Tensor] = None, *, optimizer: Optional[dict] = None,
-               slots2: Optional[torch.Tensor] = None):
-        """optimizer / slots2: as Engine.train_step; the values (Adam's powers included) are captured with this call.
+               slots2: Optional[torch.Tensor] = None, ema: Optional[torch.Tensor] = None, ema_decay: float = 0.999):
+        """optimizer / slots2 / ema / ema_decay: as Engine.train_step; the values (Adam's powers included) are captured with this call.
         h_clips (pinned uint8 tensor of n packed tcr_augment_clip records, datasets/device_input_stage.py) with int16
         h_inputs [n, stride]: the wav files' samples and the per-clip draws cross the bus; the input stage runs on the device
         (`background`: the CUDA-resident bank)."""
@@ -388,6 +431,7 @@ class HostFeed:
         a.learning_rate, a.momentum, a.weight_decay = float(learning_rate), float(momentum), float(weight_decay)
         a.dropout_seed, a.apply_update = int(dropout_seed), 1
         _set_optimizer(a, optimizer, eng._ptr(slots2))
+        a.ema, a.ema_decay = eng._ptr(ema), float(ema_decay)
         L.check(eng.lib, eng.lib.tcr_train_step_host(eng._h, C.byref(a), self.lag, eng._stream, self._out, C.byref(self._step)),
                 "tcr_train_step_host")
         return self._result()

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from ..common import utils
+from ..common.model_loader import EMA_SUFFIX
 from ..datasets import preprocessor_factory
 from ..engine import OPTIMIZER_DEFAULTS, OPTIMIZER_SLOT_NAMES, Engine
 from ..runtime import InvalidArgumentError, Node
@@ -37,6 +38,7 @@ class AudioNetModel(TFModel):
         self.optimizer = dict(kind="mom", momentum=0.9)            # set by the trainer (build_optimizer -> set_optimizer)
         self.slots2 = None                                          # Adam v / RMSProp mom (`slots`: the first slot)
         self.beta1_power = self.beta2_power = None                  # Adam's beta^t before the next step (np.float32)
+        self.ema, self.ema_decay = None, 0.999                      # --use_ema: flat shadow of the trained variables
         self.lr_schedule = lambda step: getattr(args, "learning_rate", 1e-4)
         self.var_names_to_values = None                            # in-memory weight injection hook (trainer.py:145-154)
         self.endpoints_loss: Dict[str, Node] = {}
@@ -174,27 +176,54 @@ class AudioNetModel(TFModel):
             self.beta1_power = np.float32(self.beta1_power * np.float32(self._opt("beta1")))
             self.beta2_power = np.float32(self.beta2_power * np.float32(self._opt("beta2")))
 
+    # ------------------------------------------------------------------ trainable subset and weight EMA
+    def set_trainable(self, names=None):
+        """Trains only `names` (None: every trainable variable); see Engine.set_trainable."""
+        self.flush_feed()
+        return self.engine.set_trainable(names)
+
+    def enable_ema(self, decay: float):
+        """--use_ema: the shadow `<var>/ExponentialMovingAverage` of every trained variable, starting from the variables' CURRENT
+        values (the trainer calls this before the restore: TF initialises a shadow from its variable's initializer)."""
+        self.ema, self.ema_decay = self.engine.new_ema(self.params), float(decay)
+
+    def _trained(self):
+        trained = getattr(self.engine, "trained", None)
+        return trained if trained is not None else {d["name"] for d in self.engine.table if d["trainable"]}
+
     # ------------------------------------------------------------------ variables by TF name
     def get_variables(self, with_slots=True) -> Dict[str, np.ndarray]:
-        """{TF name: array}: the variables, and with_slots the optimizer state under TF's names (`<var>/Momentum`;
-        `<var>/Adam`, `<var>/Adam_1`, beta1_power, beta2_power; `<var>/RMSProp`, `<var>/RMSProp_1`)."""
+        """{TF name: array}: the variables, the shadows `<var>/ExponentialMovingAverage` of the trained ones with --use_ema, and
+        with_slots the optimizer state under TF's names (`<var>/Momentum`; `<var>/Adam`, `<var>/Adam_1`, beta1_power,
+        beta2_power; `<var>/RMSProp`, `<var>/RMSProp_1`).  Slots and shadows exist for the trained variables only, as TF
+        creates them for var_list alone."""
         self.flush_feed()
         out = self.engine.variables_to_dict(self.params, self.moving)
+        trained = self._trained()
         if with_slots:
             names = OPTIMIZER_SLOT_NAMES[self.optimizer["kind"]]
             for suffix, buf in zip(names, (self.slots, self.slots2)):
                 if suffix is not None:
                     for k, v in self.engine.variables_to_dict(buf).items():
-                        out[f"{k}/{suffix}"] = v
+                        if k in trained:
+                            out[f"{k}/{suffix}"] = v
             if self.optimizer["kind"] == "adam":
                 out["beta1_power"], out["beta2_power"] = np.float32(self.beta1_power), np.float32(self.beta2_power)
+        if self.ema is not None:
+            for k, v in self.engine.variables_to_dict(self.ema).items():
+                if k in trained:
+                    out[k + EMA_SUFFIX] = v
         return out
 
-    def set_variables(self, values: Dict[str, np.ndarray], strict=True):
+    def set_variables(self, values: Dict[str, np.ndarray], strict=True, restore=None):
         """Variables by TF name; the optimizer state of the current kind is optional (slots and powers that are absent keep
-        their values)."""
+        their values).  With --use_ema the shadows of the trained variables are restored under their own names, and a missing
+        one is an error when `strict` (it keeps its initial value otherwise).  restore: predicate on names
+        (model_loader.restore_filter); the names it rejects are neither restored nor required."""
         self.flush_feed()
-        self.engine.variables_from_dict(values, self.params, self.moving, strict=strict)
+        if restore is not None:
+            values = {k: v for k, v in values.items() if restore(k)}
+        self.engine.variables_from_dict(values, self.params, self.moving, strict=strict, only=restore)
         names = OPTIMIZER_SLOT_NAMES[self.optimizer["kind"]]
         for suffix, buf in zip(names, (self.slots, self.slots2)):
             if suffix is None:
@@ -203,6 +232,14 @@ class AudioNetModel(TFModel):
             slots = {k[:-len(tail)]: v for k, v in values.items() if k.endswith(tail)}
             if slots:
                 self.engine.variables_from_dict(slots, buf, None, strict=False)
+        if self.ema is not None:
+            wanted = [n for n in sorted(self._trained()) if restore is None or restore(n + EMA_SUFFIX)]
+            missing = [n + EMA_SUFFIX for n in wanted if n + EMA_SUFFIX not in values]
+            if strict and missing:
+                raise KeyError(f"checkpoint has no {missing[0]} (--ignore_missing_vars keeps the initial value)")
+            shadows = {n: values[n + EMA_SUFFIX] for n in wanted if n + EMA_SUFFIX in values}
+            if shadows:
+                self.engine.variables_from_dict(shadows, self.ema, None, strict=False)
         if self.optimizer["kind"] == "adam":
             if "beta1_power" in values:
                 self.beta1_power = np.float32(np.asarray(values["beta1_power"], np.float32).reshape(()))
@@ -252,7 +289,7 @@ class AudioNetModel(TFModel):
         lr = float(self.lr_schedule(self.global_step))
         r = self._feed.submit(pinned[0], pinned[1], self.params, self.slots, self.moving, lr, self.optimizer.get("momentum") or 0.0,
                               self.args.weight_decay, dropout_seed=self._dropout_seed(), optimizer=self._step_optimizer(),
-                              slots2=self.slots2)
+                              slots2=self.slots2, ema=self.ema, ema_decay=self.ema_decay)
         self._advance_optimizer()
         self.global_step += 1
         self._feed_steps.append(self.global_step)
@@ -292,7 +329,7 @@ class AudioNetModel(TFModel):
             out = self.engine.train_step(self._d_wav, self._d_hot, self.params, self.slots, self.moving, lr,
                                          self.optimizer.get("momentum") or 0.0, wd, dropout_seed=self._dropout_seed(),
                                          want_outputs=bool(names & {"outputs", "logits"}), optimizer=self._step_optimizer(),
-                                         slots2=self.slots2)
+                                         slots2=self.slots2, ema=self.ema, ema_decay=self.ema_decay)
             self._advance_optimizer()
             self.global_step += 1
             vals["train_op"], vals["learning_rate"] = None, np.float32(lr)

@@ -9,6 +9,7 @@ import sys
 from pathlib import Path
 
 from ..common import checkpoint as ckpt
+from ..common import model_loader
 from ..common.utils import get_logger
 from ..metrics.manager import AudioMetricManager
 from .base import AudioBase
@@ -28,13 +29,27 @@ class Evaluator:
         self.watch_path = p if p.is_dir() else p.parent
         self.best = {}
 
+    def restore_values(self, values):
+        """(values, restore predicate) for set_variables: the checkpoint filtered by --checkpoint_{include,exclude}_scopes
+        (common/model_loader.py:42-83), or with --use_ema every trainable variable taken from its shadow
+        (helper/evaluator.py:41-48).  The reference crashes on --use_ema together with a scope filter (model_loader.py:76-80
+        calls .op.name on the dict's string keys); that combination is rejected here (SURVEY.md section 9)."""
+        include = getattr(self.args, "checkpoint_include_scopes", "")
+        exclude = getattr(self.args, "checkpoint_exclude_scopes", "")
+        if getattr(self.args, "use_ema", False):
+            if model_loader.split_strip(include) or model_loader.split_strip(exclude):
+                raise ValueError("--use_ema cannot be combined with --checkpoint_include_scopes / --checkpoint_exclude_scopes")
+            return model_loader.ema_restore_values(values, self.model.engine.trainable_names), None
+        return values, model_loader.restore_filter(include, exclude)
+
     def build_evaluation_step(self, checkpoint_path):
         return ckpt.checkpoint_step(checkpoint_path)
 
     def evaluate_once(self, checkpoint_path):
         self.log.info("Evaluation started")
         self.setup_dataset_iterator()
-        self.model.set_variables(ckpt.load(checkpoint_path), strict=not self.args.ignore_missing_vars)
+        values, restore = self.restore_values(ckpt.load(checkpoint_path))
+        self.model.set_variables(values, strict=not self.args.ignore_missing_vars, restore=restore)
         step = self.build_evaluation_step(str(checkpoint_path))
         self.model.global_step = step
         metrics = self.run_evaluation(step, is_training=False)

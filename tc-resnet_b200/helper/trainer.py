@@ -6,6 +6,7 @@ What changes underneath: `build_train_op` does not assemble a gradient graph (sl
 tf.train.piecewise_constant(global_step, boundaries, lr_list) (:135) evaluated on the host per step.
 Optimizers: all four choices of --optimizer run on the CUDA path: "adam" (the default), "rmsprop", "mom" and "gd"
 (= momentum 0), with TF 1.13's defaults for whatever --momentum / --optimizer_decay / --optimizer_epsilon leave unset.
+--trainable_scopes, --use_ema / --ema_decay and --checkpoint_{include,exclude}_scopes run on the same step (common/model_loader.py).
 """
 from __future__ import annotations
 
@@ -14,6 +15,7 @@ import time
 from pathlib import Path
 
 from ..common import checkpoint as ckpt
+from ..common import model_loader
 from ..common import utils
 from ..metrics.manager import AudioMetricManager
 from ..runtime import InvalidArgumentError, Node, no_op
@@ -87,23 +89,28 @@ class TrainerBase:
         raise NotImplementedError
 
     def build_train_op(self, total_loss, optimizer, trainable_scopes, global_step, gradient_multipliers=None):
-        if trainable_scopes:
-            raise NotImplementedError("--trainable_scopes (partial training) is not supported by the fused step")
-        if self.args.use_ema:
-            raise NotImplementedError("--use_ema is not supported by the fused step")
+        """create_train_op(variables_to_train=...) (+ ExponentialMovingAverage.apply behind it with --use_ema), :199-222: the
+        engine is told which variables the fused step trains, and the EMA shadow starts from the variables' initial values
+        (before the restore, as TF's var.initialized_value())."""
+        trained = model_loader.variables_to_train(trainable_scopes, self.model.engine.trainable_names, self.log)
+        self.model.set_trainable(None if len(trained) == len(self.model.engine.trainable_names) else trained)
         self.model.set_optimizer(optimizer)          # before the restore: the checkpoint may carry the optimizer's state
+        if self.args.use_ema:
+            self.model.enable_ema(self.args.ema_decay)
         return Node("train_op")
 
     def routine_restore_and_initialize(self, checkpoint_path=None):
         checkpoint_path = self.args.checkpoint_path if checkpoint_path is None else checkpoint_path
         values = getattr(self.model, "var_names_to_values", None)
+        restore = model_loader.restore_filter(getattr(self.args, "checkpoint_include_scopes", ""),
+                                              getattr(self.args, "checkpoint_exclude_scopes", ""))
         if values is not None:
             self.model.set_variables(values, strict=False)
             self.log.info("Restore from Memory")
         elif not checkpoint_path:
             self.log.info("Initialize global / local variables")
         else:
-            self.model.set_variables(ckpt.load(checkpoint_path), strict=not self.args.ignore_missing_vars)
+            self.model.set_variables(ckpt.load(checkpoint_path), strict=not self.args.ignore_missing_vars, restore=restore)
             self.log.info(f"Restored {checkpoint_path}")
 
     def setup_trainer(self):
