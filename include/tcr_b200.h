@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 8
+#define TCR_ABI_VERSION 9
 
 enum {
   TCR_OK = 0,
@@ -112,6 +112,7 @@ typedef struct tcr_param_desc {
 } tcr_param_desc;
 
 struct tcr_augment_clip;
+struct tcr_dataset;
 /* Arguments of one training step == one `session.run(train_op)` of helper/trainer.py:312-321. */
 typedef struct tcr_step_args {
   const float* input;        /* wav [n, clip_samples] in [-1,1], features [n,T,F], or (cast) int16 PCM: see TCR_INPUT_* */
@@ -171,6 +172,16 @@ typedef struct tcr_step_args {
    * Rejected with TCR_ERR_INVALID: ema_decay outside [0, 1] when ema is set. */
   float*       ema;          /* flat shadow `<var>/ExponentialMovingAverage` [num_trainable], updated in place */
   float        ema_decay;    /* 0.999 (--ema_decay) */
+  /* Resident dataset input (ABI 9, see tcr_dataset).  NULL (zero-initialised): the step reads `input` and `onehot` as above.
+   * Otherwise the input stage gathers rows [dataset_position, dataset_position + n) of the dataset's order from the clip bank,
+   * augments them with draws keyed by (dataset_seed, dataset_epoch, position) and writes their one-hot labels into a workspace
+   * buffer; `input`, `input_is_features`, `onehot`, `clips`, `background` and `pcm_stride` are ignored.  The bank is final when
+   * the step is submitted, so input_resident = 1 is valid.  Rejected with TCR_ERR_INVALID: dataset_position < 0 or
+   * dataset_position + n > order_length.  tcr_train_step only: tcr_train_step_host rejects it. */
+  const struct tcr_dataset* dataset;   /* host pointer to the caller's description, read during the call */
+  int64_t      dataset_position;
+  int64_t      dataset_epoch;
+  uint64_t     dataset_seed;
 } tcr_step_args;
 
 int         tcr_abi_version(void);
@@ -220,6 +231,53 @@ int tcr_augment_pcm16(tcr_handle* h, const int16_t* pcm, int64_t pcm_stride, con
  * does not fit is not mixed (instead of reading past the bank).  0 (default): offsets are trusted.  The host stage pads
  * recordings shorter than a clip, as augmentation_factory.py:60-75 does. */
 int tcr_set_background_samples(tcr_handle* h, int64_t samples);
+
+/* A dataset split resident in device memory (ABI 9): every clip decoded once into one int16 bank, each batch gathered and
+ * augmented on the device with random draws made in the kernel, so the host does no work per batch (the per-file tf.data map of
+ * datasets/audio_data_wrapper.py:37-58 and datasets/augmentation_factory.py:30-211).  Every pointer is device memory owned by
+ * the caller; the struct itself is host memory and is read during the call only.
+ *
+ * Row i of a batch at `position` is clip clips[order[position + i]]: its `length` samples from samples[offset], cropped to
+ * clip_samples and zero-padded, then shifted, mixed and clipped exactly as tcr_augment_pcm16 does.  The draws of the row at
+ * global position p (an index into `order`) are, with key = splitmix64(seed, epoch) and z_k = splitmix64(key, 8 p + k),
+ * splitmix64(s, i) the SplitMix64 output of the state s + 0x9E3779B97F4A7C15 * (i + 1) and u(z) = (z >> 40) / 2^24 in fp32:
+ *   shift      z0 % (2 S) - S, S = int(0.1 * clip_samples)                       (`shift` set and S > 0; else 0)
+ *   recording  b = z1 % num_background, crop z2 % (length_b - clip_samples + 1)  (`mix` set and num_background > 0)
+ *   mixed      is_training && u(z3) < background_frequency
+ *   volume     u(z4) * background_max_volume in fp32 when mixed, else 0 (the recording is then not read: 0 * x + y == y)
+ * The draws depend on the global position, not on the caller's rank or batch size, so data-parallel ranks reading their rows
+ * at position + rank * n get the rows and draws of one device running the global batch.  No read leaves `samples` or
+ * `background`: an order entry outside [0, num_clips) is a silent row with an all-zero one-hot row, a clip whose samples lie
+ * outside the bank is read only as far as it lies inside, a label outside [0, num_classes) gives an all-zero one-hot row and a
+ * crop that does not fit `background_samples` is not mixed. */
+typedef struct tcr_dataset_clip {
+  int64_t offset;      /* first sample of the clip in `samples` */
+  int32_t length;      /* samples stored, at most clip_samples; 0 for a silent sample (the "" filename) */
+  int32_t label;       /* class index of the one-hot row */
+} tcr_dataset_clip;
+typedef struct tcr_dataset {
+  const int16_t*          samples;            /* the clip bank: every clip's int16 samples back to back */
+  int64_t                 num_samples;
+  const tcr_dataset_clip* clips;              /* [num_clips] */
+  int64_t                 num_clips;
+  const int32_t*          order;              /* [order_length] clip indices: the epoch's shuffled order */
+  int64_t                 order_length;
+  const float*            background;         /* concatenated background recordings, each at least clip_samples long */
+  int64_t                 background_samples;
+  const int64_t*          background_table;   /* [num_background][2]: start and length of each recording in `background` */
+  int32_t                 num_background;
+  int32_t                 shift;              /* 1: anchored_slice_or_pad_with_shift */
+  int32_t                 mix;                /* 1: draw a recording and mix it in */
+  int32_t                 is_training;        /* 0: volume 0, as the evaluation graph */
+  float                   background_frequency;    /* 0.8 */
+  float                   background_max_volume;   /* 0.1 */
+} tcr_dataset;
+/* One batch of a resident dataset: rows [position, position + n) of its order, gathered and augmented (see tcr_dataset) into
+ * wav_out [n, clip_samples] (16-byte aligned) and their one-hot labels into onehot_out [n, num_classes], in one launch.
+ * For evaluation and inspection; a training step takes the dataset itself (tcr_step_args::dataset).
+ * TCR_ERR_INVALID: position < 0 or position + n > order_length, a NULL pointer. */
+int tcr_dataset_batch(tcr_handle* h, const tcr_dataset* desc, int64_t position, int64_t epoch, uint64_t seed, int32_t n,
+                      float* wav_out, float* onehot_out, tcr_stream stream);
 
 /* Forward pass.  is_training == 0: evaluate_audio.py path (BN moving statistics, dropout identity;
  * helper/base.py:52-125).  is_training == 1: the training graph's forward (batch statistics, dropout)

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtcr_b200.so")
 
 TCR_MODEL_TCRESNET8 = 8
 TCR_MODEL_TCRESNET14 = 14
-ABI_VERSION = 8         # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
+ABI_VERSION = 9        # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
 TCR_INPUT_WAV_F32, TCR_INPUT_FEATURES, TCR_INPUT_WAV_PCM16 = 0, 1, 2
 TCR_OPT_MOMENTUM, TCR_OPT_ADAM, TCR_OPT_RMSPROP = 0, 1, 2
 TCR_FEATURE_MFCC = 0
@@ -73,6 +73,16 @@ class TcrStepArgs(C.Structure):
         ("optimizer", C.c_int32), ("slots2", C.c_void_p), ("beta1", C.c_float), ("beta2", C.c_float),
         ("epsilon", C.c_float), ("rho", C.c_float), ("beta1_power", C.c_float), ("beta2_power", C.c_float),
         ("ema", C.c_void_p), ("ema_decay", C.c_float),
+        ("dataset", C.c_void_p), ("dataset_position", C.c_int64), ("dataset_epoch", C.c_int64), ("dataset_seed", C.c_uint64),
+    ]
+
+
+class TcrDataset(C.Structure):
+    _fields_ = [
+        ("samples", C.c_void_p), ("num_samples", C.c_int64), ("clips", C.c_void_p), ("num_clips", C.c_int64),
+        ("order", C.c_void_p), ("order_length", C.c_int64), ("background", C.c_void_p), ("background_samples", C.c_int64),
+        ("background_table", C.c_void_p), ("num_background", C.c_int32), ("shift", C.c_int32), ("mix", C.c_int32),
+        ("is_training", C.c_int32), ("background_frequency", C.c_float), ("background_max_volume", C.c_float),
     ]
 
 
@@ -90,6 +100,8 @@ SYMBOLS = {
     "tcr_mfcc_forward_pcm16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
     "tcr_set_background_samples": (C.c_int, [C.c_void_p, C.c_int64]),
     "tcr_augment_pcm16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "tcr_dataset_batch": (C.c_int, [C.c_void_p, C.POINTER(TcrDataset), C.c_int64, C.c_int64, C.c_uint64, C.c_int32, C.c_void_p,
+                                    C.c_void_p, C.c_void_p]),
     "tcr_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                               C.c_uint64, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_void_p]),

@@ -563,6 +563,46 @@ extern "C" int tcr_set_background_samples(tcr_handle* h, int64_t samples) {
   return TCR_OK;
 }
 
+// The host-side half of the bounds of a resident-dataset batch: the rows it reads from the order, and the pointers the kernel
+// dereferences.  The kernel clamps what the tables themselves contain (tcr_augment.cu).
+static int dataset_check(const tcr_handle* h, const tcr_dataset* d, int64_t position, int32_t n) {
+  if (!d || !d->clips || !d->order || (d->num_samples > 0 && !d->samples)) return fail(TCR_ERR_INVALID, "dataset: NULL pointer");
+  if (d->num_samples < 0 || d->num_clips < 0 || d->order_length < 0 || d->background_samples < 0 || d->num_background < 0)
+    return fail(TCR_ERR_INVALID, "dataset: negative size");
+  if (position < 0 || position + (int64_t)n > d->order_length)
+    return fail(TCR_ERR_INVALID, "dataset: rows [%lld, %lld) outside the order of %lld entries", (long long)position,
+                (long long)(position + n), (long long)d->order_length);
+  if (d->mix && d->num_background > 0 && (!d->background || !d->background_table))
+    return fail(TCR_ERR_INVALID, "dataset: mixing needs the background bank and its table");
+  (void)h;
+  return TCR_OK;
+}
+
+// A workspace buffer a step allocates on its first use (the input stage's decoded wav and one-hot buffers), counted in
+// workspace_bytes like the buffers allocated at creation.
+static int lazy_buffer(tcr_handle* h, float*& p, size_t floats) {
+  if (p) return TCR_OK;
+  void* q = nullptr;
+  TCR_CUDA(cudaMalloc(&q, floats * sizeof(float)));
+  h->allocs.push_back(q);
+  h->workspace_bytes += (int64_t)(floats * sizeof(float));
+  p = (float*)q;
+  return TCR_OK;
+}
+
+extern "C" int tcr_dataset_batch(tcr_handle* h, const tcr_dataset* desc, int64_t position, int64_t epoch, uint64_t seed, int32_t n,
+                                 float* wav_out, float* onehot_out, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!h || !wav_out || !onehot_out) return fail(TCR_ERR_INVALID, "NULL argument");
+  TCR_TRY(check_n(h, n));
+  TCR_TRY(dataset_check(h, desc, position, n));
+  if (((uintptr_t)wav_out & 15) != 0) return fail(TCR_ERR_INVALID, "wav_out must be 16-byte aligned");
+  dataset_batch_launch(*desc, position, epoch, seed, wav_out, onehot_out, h->cfg.clip_samples, h->cfg.num_classes, n,
+                       (cudaStream_t)stream);
+  TCR_CUDA(cudaGetLastError());
+  return TCR_OK;
+}
+
 extern "C" int tcr_forward(tcr_handle* h, const float* input, int32_t input_is_features, const float* params,
                            const float* moving, int32_t n, int32_t is_training, uint64_t dropout_seed,
                            const float* dropout_mask, const float* onehot, float weight_decay, float* logits,
@@ -647,7 +687,8 @@ static void frontend_ahead_destroy(tcr_handle* h) {
 // input_event: what the front-end has to wait for when it runs ahead (the host feed's H2D copy), or null
 static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream stream, void* input_event) {
   pdl_chain_reset();
-  if (!h || !a || !a->input || !a->onehot || !a->params) return fail(TCR_ERR_INVALID, "NULL argument");
+  if (!h || !a || !a->params) return fail(TCR_ERR_INVALID, "NULL argument");
+  if (!a->dataset && (!a->input || !a->onehot)) return fail(TCR_ERR_INVALID, "NULL argument");
   if (a->apply_update && (!a->slots || !a->moving)) return fail(TCR_ERR_INVALID, "apply_update needs slots and moving");
   if (a->optimizer != TCR_OPT_MOMENTUM && a->optimizer != TCR_OPT_ADAM && a->optimizer != TCR_OPT_RMSPROP)
     return fail(TCR_ERR_INVALID, "unknown optimizer %d", a->optimizer);
@@ -658,11 +699,13 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
   if (a->ema && !(a->ema_decay >= 0.0f && a->ema_decay <= 1.0f))
     return fail(TCR_ERR_INVALID, "ema_decay %g outside [0, 1]", (double)a->ema_decay);
   TCR_TRY(check_n(h, a->n));
+  if (a->dataset) TCR_TRY(dataset_check(h, a->dataset, a->dataset_position, a->n));
   cudaStream_t s = (cudaStream_t)stream;
   const float* feat = a->input;
   int fe_buf = -1;                   // feature buffer of a front-end that ran ahead
-  if (a->input_is_features != TCR_INPUT_FEATURES) {
-    if (a->input_is_features != TCR_INPUT_WAV_F32 && a->input_is_features != TCR_INPUT_WAV_PCM16) return fail(TCR_ERR_INVALID, "unknown input kind %d", a->input_is_features);
+  tcr_step_args ds_args;             // a resident-dataset step: the rest of the step reads the labels the input stage wrote
+  if (a->dataset || a->input_is_features != TCR_INPUT_FEATURES) {
+    if (!a->dataset && a->input_is_features != TCR_INPUT_WAV_F32 && a->input_is_features != TCR_INPUT_WAV_PCM16) return fail(TCR_ERR_INVALID, "unknown input kind %d", a->input_is_features);
     tcr_stream fs = stream;          // stream of the front-end kernels
     float* featbuf = h->d_feat;
 #ifndef TCR_EMU
@@ -680,16 +723,22 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
     }
 #endif
     h->feat_last = featbuf;
-    if (a->clips) {                  // device input stage first: int16 clips + per-clip draws -> fp32 wav (tcr_augment.cu)
+    if (a->dataset) {                // gather + draws + augment from the resident clip bank, labels alongside (tcr_augment.cu)
+      float*& aug = fe_buf >= 0 ? h->fe_aug : h->d_aug;
+      float*& hot = fe_buf >= 0 ? h->fe_hot[fe_buf] : h->d_hot;
+      TCR_TRY(lazy_buffer(h, aug, (size_t)h->cfg.max_batch * h->cfg.clip_samples));
+      TCR_TRY(lazy_buffer(h, hot, (size_t)h->cfg.max_batch * h->cfg.num_classes));
+      dataset_batch_launch(*a->dataset, a->dataset_position, a->dataset_epoch, a->dataset_seed, aug, hot, h->cfg.clip_samples,
+                           h->cfg.num_classes, a->n, (cudaStream_t)fs);
+      TCR_TRY(mfcc_run(h, aug, 0, featbuf, a->n, fs));
+      ds_args = *a;
+      ds_args.onehot = hot;
+      a = &ds_args;
+    } else if (a->clips) {           // device input stage first: int16 clips + per-clip draws -> fp32 wav (tcr_augment.cu)
       if (a->input_is_features != TCR_INPUT_WAV_PCM16) return fail(TCR_ERR_INVALID, "clips need TCR_INPUT_WAV_PCM16 input");
       const int64_t stride = a->pcm_stride > 0 ? a->pcm_stride : h->cfg.clip_samples;
       float*& aug = fe_buf >= 0 ? h->fe_aug : h->d_aug;       // the ahead path decodes into its own buffer
-      if (!aug) {
-        void* p = nullptr;
-        TCR_CUDA(cudaMalloc(&p, (size_t)h->cfg.max_batch * h->cfg.clip_samples * sizeof(float)));
-        h->allocs.push_back(p);
-        aug = (float*)p;
-      }
+      TCR_TRY(lazy_buffer(h, aug, (size_t)h->cfg.max_batch * h->cfg.clip_samples));
       augment_launch((const int16_t*)a->input, stride, a->clips, a->background, h->background_samples, aug, h->cfg.clip_samples, a->n,
                      (cudaStream_t)fs);
       TCR_TRY(mfcc_run(h, aug, 0, featbuf, a->n, fs));
@@ -845,6 +894,7 @@ static int hostfeed_collect(HostFeedState* f, float* losses_out, int64_t* losses
 extern "C" int tcr_train_step_host(tcr_handle* h, const tcr_step_args* a, int32_t lag, tcr_stream stream, float* losses_out,
                                    int64_t* losses_step) {
   if (!h || !a || !a->input || !a->onehot || !a->params) return fail(TCR_ERR_INVALID, "NULL argument");
+  if (a->dataset) return fail(TCR_ERR_INVALID, "a resident dataset is read by tcr_train_step, not by the host-buffer step");
   if (lag < 0 || lag >= kFeedDepth) return fail(TCR_ERR_INVALID, "lag must be in [0, %d]", kFeedDepth - 1);
   TCR_TRY(check_n(h, a->n));
   HostFeedState* f = nullptr;

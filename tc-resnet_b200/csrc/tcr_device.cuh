@@ -246,13 +246,15 @@ __device__ __forceinline__ void tl_stamp(long long* tl, int cta, int slot) {
 __device__ __forceinline__ void tl_stamp(long long*, int, int) {}
 #endif
 
-// Counter-based RNG for dropout (TF's RNG is not reproducible; parity runs inject a mask instead).
-__device__ __forceinline__ float uniform01(uint64_t seed, uint64_t idx) {
+// Counter-based RNG for dropout and the resident dataset's augmentation draws (TF's RNG is not reproducible; parity runs
+// inject a mask instead): SplitMix64's output for the state seed + golden * (idx + 1).
+__host__ __device__ __forceinline__ uint64_t splitmix64(uint64_t seed, uint64_t idx) {
   uint64_t z = seed + 0x9E3779B97F4A7C15ull * (idx + 1);
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  z = z ^ (z >> 31);
-  return (float)(z >> 40) * (1.0f / 16777216.0f);   // [0,1)
+  return z ^ (z >> 31);
 }
+__device__ __forceinline__ float uniform01(uint64_t z) { return (float)(z >> 40) * (1.0f / 16777216.0f); }   // [0,1), 24 bits
+__device__ __forceinline__ float uniform01(uint64_t seed, uint64_t idx) { return uniform01(splitmix64(seed, idx)); }
 
 }  // namespace tcr

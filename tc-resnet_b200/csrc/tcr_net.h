@@ -19,6 +19,9 @@ int cluster_size(tcr_handle* h);
 StatSrc stat_src(const tcr_handle* h, const ConvPlan& cv, const float* params, int n);
 int augment_launch(const int16_t* pcm, int64_t pcm_stride, const tcr_augment_clip* clips, const float* background, int64_t background_samples,
                    float* out, int clip, int n, cudaStream_t s);
+// Rows [position, position + n) of a resident dataset's order: gather + draws + augment into out [n][clip], labels into onehot
+int dataset_batch_launch(const tcr_dataset& ds, int64_t position, int64_t epoch, uint64_t seed, float* out, float* onehot, int clip,
+                         int classes, int n, cudaStream_t s);
 int eval_accumulate_launch(const float* scores, const float* onehot, int n, int classes, int topk, int64_t* counts, cudaStream_t s);
 int net_weight_transpose(tcr_handle* h, const float* params, cudaStream_t s);
 int sync_records(tcr_handle* h, const float* part, int gc, int cols, float* out, cudaStream_t s);   // SyncBN: sum records, all-reduce

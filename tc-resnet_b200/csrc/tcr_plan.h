@@ -65,6 +65,8 @@ struct tcr_handle {
   void* fe_stream = nullptr; float* fe_feat[2] = {nullptr, nullptr}; void* fe_ready[2] = {nullptr, nullptr};
   void* fe_free[2] = {nullptr, nullptr}; long long fe_count = 0;
   float* fe_aug = nullptr;           // the ahead path's own decoded-wav buffer (device input stage)
+  float* fe_hot[2] = {nullptr, nullptr};   // one-hot labels of a resident-dataset step, one per feature buffer of the ahead path
+  float* d_hot = nullptr;            // the same for a resident-dataset step ordered on the caller's stream
   void* fe_gate = nullptr; int fe_gate_valid = 0;   // recorded on the step's stream once the weight gradients are launched: the next
                                      // step's front-end starts behind it, i.e. next to grad_finalize / update, not next to the FMA-bound kernels
   float* feat_last = nullptr;

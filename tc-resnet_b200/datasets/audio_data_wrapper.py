@@ -36,6 +36,7 @@ class AudioDataWrapper(DataWrapperBase):
             if dist.is_available() and dist.is_initialized():
                 self.rank, self.world = dist.get_rank(), dist.get_world_size()
         self.aug_rng = np.random.RandomState(1234 + 7919 * self.rank)
+        self.draw_seed = 1234                           # --device_dataset: draws keyed by global position, the same on every rank
         self.setup()
         self.placeholders = (Node("filenames"), Node("labels_index"))
         self.setup_iterator(session, self.placeholders, self.data)
@@ -50,12 +51,15 @@ class AudioDataWrapper(DataWrapperBase):
         self._order = np.arange(self._num_samples)
         if self.shuffle:
             self.rng.shuffle(self._order)
+        self._epoch = getattr(self, "_epoch", -1) + 1     # key of the device path's draws; a new order goes to the device
+        self._order_changed = True
 
     def get_input_and_output_op(self):
         return (Node("audio_original", [None, self.desired_samples, 1], self),
                 Node("labels", [None, self.num_labels], self))
 
-    def _take_indices(self):
+    def _next_position(self):
+        """Position of this rank's next batch in `_order`: advances the shared cursor, reshuffles when the epoch ends."""
         n = self.batch_size
         window = n * self.world                       # one global batch; every rank advances the shared cursor by it
         if self._cursor + window > self._num_samples:
@@ -64,10 +68,36 @@ class AudioDataWrapper(DataWrapperBase):
             self._cursor = 0
             if self.shuffle:
                 self.rng.shuffle(self._order)
+            self._epoch += 1
+            self._order_changed = True
         lo = self._cursor + self.rank * n
-        idx = self._order[lo:lo + n]
         self._cursor += window
-        return idx
+        return lo
+
+    def _take_indices(self):
+        lo = self._next_position()
+        return self._order[lo:lo + self.batch_size]
+
+    def attach_device(self, engine):
+        """--device_dataset: moves the decoded split to `engine`'s device (DeviceDataset); called once the model's engine exists."""
+        from .device_input_stage import DeviceDataset
+        a = self.args
+        self.device_data = DeviceDataset(
+            engine, self._bank, self._bank_table, self.background_data,
+            shift=a.augmentation_method == "anchored_slice_or_pad_with_shift",
+            mix=a.augmentation_method not in ("no_augmentation", "no_augmentation_audio"),
+            is_training=self.is_training, background_frequency=a.background_frequency, background_max_volume=a.background_max_volume)
+        self._bank = self._bank_table = None          # the host copy is not needed any more
+        return self.device_data
+
+    def next_device_rows(self):
+        """--device_dataset: (position, epoch) of this rank's next batch in the resident order, which is the order the host path
+        takes its indices from; the epoch's order is uploaded when it changed."""
+        lo = self._next_position()
+        if self._order_changed:
+            self.device_data.upload_order(self._order)
+            self._order_changed = False
+        return lo, self._epoch
 
     @staticmethod
     def add_arguments(parser):
@@ -80,6 +110,9 @@ class SingleLabelAudioDataWrapper(AudioDataWrapper):
     def setup(self):
         a = self.args
         self.synthetic = str(a.dataset_path).startswith("synthetic")
+        self.device_data = None
+        if self.synthetic and getattr(a, "device_dataset", False):
+            raise ValueError("--device_dataset reads a dataset from disk; `synthetic:` clips are generated on the host")
         if self.synthetic:
             spec = str(a.dataset_path).split(":")
             self._num_samples = int(spec[1]) if len(spec) > 1 else 4096
@@ -105,6 +138,10 @@ class SingleLabelAudioDataWrapper(AudioDataWrapper):
             self._num_samples = len(self.filenames)
             self.augment = get_audio_augmentation_fn(a.augmentation_method if a.augmentation_method != "no_augmentation"
                                                      else "no_augmentation_audio")
+            if getattr(a, "device_dataset", False):             # decoded once here, moved to the device by attach_device()
+                from .device_input_stage import decode_clip_bank
+                self._bank, self._bank_table = decode_clip_bank(self.filenames, self.labels, self.desired_samples,
+                                                                getattr(a, "num_threads", 8))
         assert a.num_classes == self.num_labels, f"--num_classes {a.num_classes} != {self.num_labels} label directories"
         self.data = (self.filenames, self.labels)
 

@@ -13,15 +13,19 @@ _available_audio_augmentation_methods = ["anchored_slice_or_pad", "anchored_slic
 _available_augmentation_methods = _available_audio_augmentation_methods + ["no_augmentation"]
 
 
-def load_wav_file(filename: str, desired_samples: int) -> np.ndarray:
+def read_wav_pcm16(filename: str) -> np.ndarray:
+    """The int16 samples of a 16-bit PCM wav file, channel 0 only (decode_wav's input, before its 1/32768 scaling)."""
     with wave.open(filename, "rb") as w:
         nch, width, nframes = w.getnchannels(), w.getsampwidth(), w.getnframes()
         raw = w.readframes(nframes)
     if width != 2:
         raise ValueError(f"{filename}: only 16-bit PCM wav is supported")
-    data = np.frombuffer(raw, dtype="<i2").astype(np.float32) / 32768.0
-    if nch > 1:
-        data = data.reshape(-1, nch)[:, 0]
+    data = np.frombuffer(raw, dtype="<i2")
+    return data.reshape(-1, nch)[:, 0] if nch > 1 else data
+
+
+def load_wav_file(filename: str, desired_samples: int) -> np.ndarray:
+    data = read_wav_pcm16(filename).astype(np.float32) / 32768.0
     if desired_samples > 0:
         out = np.zeros(desired_samples, np.float32)
         m = min(desired_samples, data.shape[0])

@@ -11,7 +11,10 @@ from .. import const
 from ..common import utils
 from .augmentation_factory import _available_augmentation_methods
 
-_BOOL_FLAGS = [("has_sub_dataset", False), ("add_null_class", True), ("shuffle", True), ("cache_dataset", False)]
+_BOOL_FLAGS = [("has_sub_dataset", False), ("add_null_class", True), ("shuffle", True), ("cache_dataset", False),
+               # decode the split once into device memory and build every batch there (datasets/device_input_stage.DeviceDataset);
+               # opt-in: it holds the whole split in GPU memory and draws other augmentation random numbers than the host path
+               ("device_dataset", False)]
 
 
 class DataWrapperBase(ABC):

@@ -7,13 +7,19 @@ whole batch in one HBM-bound pass, bit-identical to the host stage (augmentation
 """
 from __future__ import annotations
 
+from concurrent.futures import ThreadPoolExecutor
 from typing import Optional, Sequence
 
 import numpy as np
 import torch
 
+from .. import _lib as L
+from .augmentation_factory import read_wav_pcm16
+
 # tcr_augment_clip (include/tcr_b200.h)
 CLIP_DTYPE = np.dtype([("length", "<i4"), ("shift", "<i4"), ("silent", "<i4"), ("bg_volume", "<f4"), ("bg_offset", "<i8")])
+# tcr_dataset_clip (include/tcr_b200.h)
+DATASET_CLIP_DTYPE = np.dtype([("offset", "<i8"), ("length", "<i4"), ("label", "<i4")])
 
 
 def draw_clips(rng: np.random.RandomState, lengths: Sequence[int], silent: Sequence[bool], clip_samples: int,
@@ -60,3 +66,78 @@ class DeviceInputStage:
 
     def __call__(self, pcm: torch.Tensor, clips: np.ndarray, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         return self.engine.augment(pcm, pack(clips, self.engine.device), self.background, out=out)
+
+
+def decode_clip_bank(filenames: Sequence[str], labels: Sequence[int], clip_samples: int, num_threads: int = 8):
+    """Every clip of a split decoded once, with `num_threads` workers: (int16 bank, DATASET_CLIP_DTYPE table).  A clip keeps at
+    most clip_samples samples (decode_wav's crop); a "" filename (a silent sample) is stored with length 0."""
+    def read(f):
+        return np.zeros(0, np.int16) if f == "" else read_wav_pcm16(f)[:clip_samples]
+    with ThreadPoolExecutor(max(1, int(num_threads))) as ex:
+        clips = list(ex.map(read, filenames))
+    lengths = np.array([c.shape[0] for c in clips], np.int64)
+    table = np.zeros(len(clips), DATASET_CLIP_DTYPE)
+    table["offset"] = np.cumsum(lengths) - lengths
+    table["length"], table["label"] = lengths, np.asarray(labels, np.int64)
+    bank = np.empty(int(lengths.sum()), np.int16)
+    for i in range(len(clips)):
+        bank[table["offset"][i]:table["offset"][i] + lengths[i]] = clips[i]
+        clips[i] = None
+    return bank, table
+
+
+class DeviceDataset:
+    """A split resident in device memory (tcr_dataset, include/tcr_b200.h): the clip bank, its table, the background bank
+    (through DeviceInputStage) and two order buffers.  Each epoch's order is uploaded once, into the buffer the epoch before the
+    last one used; an event recorded when that epoch's last step was submitted guards the overwrite."""
+
+    def __init__(self, engine, bank: np.ndarray, table: np.ndarray, background_data=None, shift: bool = True, mix: bool = True,
+                 is_training: bool = True, background_frequency: float = 0.8, background_max_volume: float = 0.1):
+        self.engine = engine
+        dev = engine.device
+        clip = int(engine.cfg.clip_samples)
+        bg = [np.asarray(b, np.float32).reshape(-1) for b in (background_data or [])]
+        bg_floats = sum(max(b.shape[0], clip) for b in bg)
+        need = bank.nbytes + table.nbytes + 2 * 4 * len(table) + 4 * bg_floats + 16 * len(bg)
+        free, _ = torch.cuda.mem_get_info(dev)
+        if need > free:
+            raise MemoryError(f"--device_dataset: the split needs {need} bytes of device memory, {free} bytes are free")
+        self.num_clips = len(table)
+        self.samples = torch.from_numpy(np.ascontiguousarray(bank, np.int16)).to(dev)
+        self.table = torch.from_numpy(np.frombuffer(np.ascontiguousarray(table, DATASET_CLIP_DTYPE).tobytes(), np.uint8).copy()).to(dev)
+        self.stage = DeviceInputStage(engine, bg)
+        starts = np.cumsum(self.stage.bg_lengths) - np.asarray(self.stage.bg_lengths, np.int64) if bg else np.zeros(0, np.int64)
+        self.bg_table = torch.from_numpy(np.stack([starts, np.asarray(self.stage.bg_lengths, np.int64)], 1).reshape(-1)
+                                         if bg else np.zeros(2, np.int64)).to(dev)
+        # empty, not zeros: the uploads run on their own stream and must not race a fill queued on the current one
+        self.orders = [torch.empty(max(self.num_clips, 1), dtype=torch.int32, device=dev) for _ in range(2)]
+        self._released = [None, None]                 # event: every step that read the buffer has finished
+        self._copy = torch.cuda.Stream(dev)
+        self.current = 1
+        self.desc = L.TcrDataset()
+        d = self.desc
+        d.samples, d.num_samples = self.samples.data_ptr(), self.samples.numel()
+        d.clips, d.num_clips = self.table.data_ptr(), self.num_clips
+        d.background = self.stage.background.data_ptr() if bg else None
+        d.background_samples = int(sum(self.stage.bg_lengths))
+        d.background_table, d.num_background = self.bg_table.data_ptr(), len(bg)
+        d.shift, d.mix, d.is_training = int(bool(shift)), int(bool(mix) and bool(bg)), int(bool(is_training))
+        d.background_frequency, d.background_max_volume = float(background_frequency), float(background_max_volume)
+
+    def upload_order(self, order: np.ndarray):
+        """Makes `order` (the epoch's sample indices) the order the following batches read.  Returns when it is on the device."""
+        stream = torch.cuda.current_stream(self.engine.device)
+        self._released[self.current] = stream.record_event()      # every step reading the current buffer is submitted by now
+        b = self.current ^ 1
+        if self._released[b] is not None:
+            self._released[b].synchronize()
+        with torch.cuda.stream(self._copy):
+            self.orders[b][:len(order)].copy_(torch.from_numpy(np.ascontiguousarray(order, np.int32)))
+        self._copy.synchronize()
+        self.current = b
+        self.desc.order, self.desc.order_length = self.orders[b].data_ptr(), len(order)
+
+    def batch(self, position: int, epoch: int, seed: int, n: int, wav_out: Optional[torch.Tensor] = None,
+              onehot_out: Optional[torch.Tensor] = None):
+        """(wav [n, clip_samples], one-hot [n, classes]) of rows [position, position + n) of the current order (tcr_dataset_batch)."""
+        return self.engine.dataset_batch(self.desc, position, epoch, seed, n, wav_out, onehot_out)

@@ -253,6 +253,16 @@ class Engine:
                                                      self._ptr(out), n, self._stream), "tcr_augment_pcm16")
         return out
 
+    def dataset_batch(self, desc: "L.TcrDataset", position: int, epoch: int, seed: int, n: int,
+                      wav_out: Optional[torch.Tensor] = None, onehot_out: Optional[torch.Tensor] = None):
+        """Rows [position, position + n) of a resident dataset's order (tcr_dataset_batch, datasets/device_input_stage.DeviceDataset),
+        gathered and augmented with the device's draws: (fp32 wav [n, clip_samples], one-hot [n, num_classes])."""
+        wav_out = wav_out if wav_out is not None else self._f32(n, self.cfg.clip_samples)
+        onehot_out = onehot_out if onehot_out is not None else self._f32(n, self.num_classes)
+        L.check(self.lib, self.lib.tcr_dataset_batch(self._h, C.byref(desc), int(position), int(epoch), int(seed), int(n),
+                                                     self._ptr(wav_out), self._ptr(onehot_out), self._stream), "tcr_dataset_batch")
+        return wav_out, onehot_out
+
     def forward(self, inputs: torch.Tensor, params: torch.Tensor, moving: Optional[torch.Tensor] = None,
                 is_training: bool = False, onehot: Optional[torch.Tensor] = None, weight_decay: float = 0.0,
                 dropout_seed: int = 0, dropout_mask: Optional[torch.Tensor] = None, input_is_features: bool = False):
@@ -274,7 +284,8 @@ class Engine:
                    losses: Optional[torch.Tensor] = None, clips: Optional[torch.Tensor] = None,
                    background: Optional[torch.Tensor] = None, input_resident: bool = False, *,
                    optimizer: Optional[dict] = None, slots2: Optional[torch.Tensor] = None,
-                   ema: Optional[torch.Tensor] = None, ema_decay: float = 0.999):
+                   ema: Optional[torch.Tensor] = None, ema_decay: float = 0.999, dataset: Optional["L.TcrDataset"] = None,
+                   position: int = 0, epoch: int = 0, seed: int = 0, n: Optional[int] = None):
         """optimizer: None or dict(kind="mom" | "gd") for the momentum step (`momentum`), dict(kind="adam", beta1=, beta2=,
         epsilon=, beta1_power=, beta2_power=) or dict(kind="rmsprop", decay=, momentum=, epsilon=) (missing hyper-parameters
         take TF's defaults, OPTIMIZER_DEFAULTS).  Adam / RMSProp keep their second slot in `slots2` (new_optimizer_state);
@@ -284,14 +295,21 @@ class Engine:
         input_resident=True: `inputs` is final when the call is made (nothing queued on the current stream writes it); the
         front-end then runs ahead on the library's own stream and overlaps the previous step's tail (tcr_step_args::input_resident).
         ema (new_ema) / ema_decay: after the update, the shadow of every trained parameter moves toward the new weight
-        (tf.train.ExponentialMovingAverage(ema_decay).apply(variables_to_train), tcr_step_args::ema)."""
-        n = inputs.shape[0]
+        (tf.train.ExponentialMovingAverage(ema_decay).apply(variables_to_train), tcr_step_args::ema).
+        dataset (DeviceDataset.desc) with position / epoch / seed and n: the step reads rows [position, position + n) of the resident
+        dataset's order, augmented with the device's draws, and their labels (tcr_step_args::dataset); `inputs` and `onehot` are
+        then None."""
         a = L.TcrStepArgs()
-        if clips is not None:
+        if dataset is not None:
+            assert inputs is None and onehot is None and n is not None
+            a.dataset, a.dataset_position, a.dataset_epoch, a.dataset_seed = C.addressof(dataset), int(position), int(epoch), int(seed)
+        elif clips is not None:
+            n = inputs.shape[0]
             assert inputs.dtype == torch.int16 and inputs.is_cuda and inputs.is_contiguous() and clips.numel() == 24 * n
             a.input, a.input_is_features = inputs.data_ptr(), L.TCR_INPUT_WAV_PCM16
             a.clips, a.background, a.pcm_stride = clips.data_ptr(), self._ptr(background), inputs.shape[1]
         else:
+            n = inputs.shape[0]
             a.input, a.input_is_features = self._input(inputs, input_is_features)
         a.onehot, a.n = self._ptr(onehot), n
         a.params, a.slots, a.moving = self._ptr(params), self._ptr(slots), self._ptr(moving)

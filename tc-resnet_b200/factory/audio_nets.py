@@ -46,6 +46,7 @@ class AudioNetModel(TFModel):
         self._feed, self._feed_last = None, (0, np.float32("nan"), np.float32("nan"))
         self._feed_steps = []                                       # global step numbers of the submitted, not yet reported steps
         self._feed_slots = []
+        self._loss_ring, self._loss_pending, self._loss_submitted = [], [], 0   # --device_dataset: (device, pinned, event) loss slots
         self._counts = None                                        # device int64 [classes^2 + 2] (tcr_eval_accumulate)
 
     # ------------------------------------------------------------------ graph-construction API of the reference
@@ -99,6 +100,8 @@ class AudioNetModel(TFModel):
         self._h_hot = torch.empty(n, a.num_classes, dtype=torch.float32).pin_memory()
         self._d_wav, self._d_hot = self._h_wav.to(dev), self._h_hot.to(dev)
         self._feed_slots = [(torch.empty_like(self._h_wav).pin_memory(), torch.empty_like(self._h_hot).pin_memory()) for _ in range(4)]
+        if getattr(a, "device_dataset", False) and self.dataset is not None and self.dataset.device_data is None:
+            self.dataset.attach_device(self.engine)
         return Node("logits", [None, a.num_classes]), {"ranges": Node("ranges")}
 
     def build_loss(self, logits, scores, labels):
@@ -273,6 +276,8 @@ class AudioNetModel(TFModel):
         lag = int(getattr(self.args, "feed_lag", 2))
         if lag <= 0:
             return None
+        if getattr(self.dataset, "device_data", None) is not None:
+            return self._execute_train_device(lag)
         pinned = self.dataset.next_batch_pinned() if hasattr(self.dataset, "next_batch_pinned") else None
         if pinned is None:
             wav_np, hot_np = self.dataset.next_batch()
@@ -301,11 +306,49 @@ class AudioNetModel(TFModel):
         return {"train_op": None, "learning_rate": np.float32(lr), "global_step": np.int64(self.global_step), "total_loss": total,
                 "model_loss": model, "loss_global_step": np.int64(step)}
 
+    def _execute_train_device(self, lag: int) -> Dict[str, object]:
+        """session.run(train_op) on a resident dataset (--device_dataset): one tcr_train_step that gathers and augments its rows
+        from the clip bank, with the front-end running ahead (input_resident: the bank is final).  Its losses are copied into a
+        ring of lag + 1 pinned slots and reported `lag` calls later, as the host-buffer step reports them."""
+        ds = self.dataset
+        position, epoch = ds.next_device_rows()
+        if not self._loss_ring:
+            dev = self.engine.device
+            self._loss_ring = [(torch.empty(2, dtype=torch.float32, device=dev), torch.empty(2, dtype=torch.float32).pin_memory(),
+                                torch.cuda.Event()) for _ in range(lag + 1)]
+        slot = self._loss_ring[self._loss_submitted % len(self._loss_ring)]     # collected before its reuse: at most lag pending
+        self._loss_submitted += 1
+        lr = float(self.lr_schedule(self.global_step))
+        self.engine.train_step(None, None, self.params, self.slots, self.moving, lr, self.optimizer.get("momentum") or 0.0,
+                               self.args.weight_decay, dropout_seed=self._dropout_seed(), losses=slot[0], input_resident=True,
+                               optimizer=self._step_optimizer(), slots2=self.slots2, ema=self.ema, ema_decay=self.ema_decay,
+                               dataset=ds.device_data.desc, position=position, epoch=epoch, seed=ds.draw_seed, n=self.args.batch_size)
+        slot[1].copy_(slot[0], non_blocking=True)
+        slot[2].record()
+        self._advance_optimizer()
+        self.global_step += 1
+        self._feed_steps.append(self.global_step)
+        self._loss_pending.append(slot)
+        if len(self._loss_pending) > lag:
+            self._collect_loss()
+        step, total, model = self._feed_last
+        return {"train_op": None, "learning_rate": np.float32(lr), "global_step": np.int64(self.global_step), "total_loss": total,
+                "model_loss": model, "loss_global_step": np.int64(step)}
+
+    def _collect_loss(self):
+        _, host, event = self._loss_pending.pop(0)
+        event.synchronize()
+        self._feed_last = (self._feed_steps.pop(0), np.float32(host[0]), np.float32(host[1]))
+        if not np.isfinite(self._feed_last[1]):
+            raise InvalidArgumentError(f"non-finite loss at step {self._feed_last[0]}")
+
     def flush_feed(self):
         """Drain the host-feed pipeline (before anything reads the variables: checkpoints, evaluation, get_variables)."""
         if self._feed is not None:
             for r in self._feed.flush():
                 self._feed_last = (self._feed_steps.pop(0), np.float32(r[1]), np.float32(r[2]))
+        while self._loss_pending:
+            self._collect_loss()
 
     def execute(self, names: Set[str], feed) -> Dict[str, object]:
         if "train_op" in names:
@@ -314,14 +357,20 @@ class AudioNetModel(TFModel):
                 self._last = fast
                 return fast
         self.flush_feed()
-        wav_np, hot_np = self.dataset.next_batch()
-        n = wav_np.shape[0]
-        if n != self.args.batch_size:
-            raise InvalidArgumentError(f"bad batch: {wav_np.shape}")
-        self._h_wav.copy_(torch.from_numpy(wav_np.reshape(n, -1)))
-        self._h_hot.copy_(torch.from_numpy(hot_np))
-        self._d_wav.copy_(self._h_wav, non_blocking=True)
-        self._d_hot.copy_(self._h_hot, non_blocking=True)
+        device_data = getattr(self.dataset, "device_data", None)
+        if device_data is not None:                             # --device_dataset: the batch is built on the device
+            n = self.args.batch_size
+            position, epoch = self.dataset.next_device_rows()
+            device_data.batch(position, epoch, self.dataset.draw_seed, n, self._d_wav, self._d_hot)
+        else:
+            wav_np, hot_np = self.dataset.next_batch()
+            n = wav_np.shape[0]
+            if n != self.args.batch_size:
+                raise InvalidArgumentError(f"bad batch: {wav_np.shape}")
+            self._h_wav.copy_(torch.from_numpy(wav_np.reshape(n, -1)))
+            self._h_hot.copy_(torch.from_numpy(hot_np))
+            self._d_wav.copy_(self._h_wav, non_blocking=True)
+            self._d_hot.copy_(self._h_hot, non_blocking=True)
         wd = self.args.weight_decay
         vals: Dict[str, object] = {}
         if "train_op" in names:
@@ -343,8 +392,14 @@ class AudioNetModel(TFModel):
             self.engine.eval_accumulate(out["probs"], self._d_hot, self._counts, topk=5)
             vals["metric_counts"] = None
         losses = out["losses"].cpu().numpy()                    # the D2H read synchronises the step
-        vals.update(total_loss=losses[0], model_loss=losses[1], global_step=np.int64(self.global_step),
-                    labels=hot_np, audio_original=wav_np)
+        vals.update(total_loss=losses[0], model_loss=losses[1], global_step=np.int64(self.global_step))
+        if device_data is None:
+            vals.update(labels=hot_np, audio_original=wav_np)
+        else:                                                   # copied to the host only when fetched
+            if "labels" in names:
+                vals["labels"] = self._d_hot.cpu().numpy()
+            if "audio_original" in names:
+                vals["audio_original"] = self._d_wav.cpu().numpy()[..., None]
         if "outputs" in names or "logits" in names:
             vals["outputs"], vals["logits"] = out["probs"].cpu().numpy(), out["logits"].cpu().numpy()
         if "audio" in names:
