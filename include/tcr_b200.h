@@ -63,8 +63,8 @@ typedef struct tcr_config {
   int32_t clip_samples;           /* int(sample_rate * clip_duration_ms / 1000) = 16000 */
   int32_t window_size_samples;    /* int(sample_rate * window_size_ms / 1000): 640 (T=49) or 480 (T=98) */
   int32_t window_stride_samples;  /* 320 or 160 */
-  int32_t num_mel_bins;           /* 64 */
-  int32_t num_mfccs;              /* 40 */
+  int32_t num_mel_bins;           /* 64; at most 128 */
+  int32_t num_mfccs;              /* 40; a multiple of 4, at most num_mel_bins (so at most 128); ignored for TCR_FEATURE_LOG_MEL */
   float   lower_edge_hertz;       /* 80 */
   float   upper_edge_hertz;       /* 7600 */
   int32_t feature_kind;           /* TCR_FEATURE_MFCC (power + DCT) | TCR_FEATURE_LOG_MEL (magnitude, no DCT) */

@@ -381,7 +381,9 @@ extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
                 cfg->window_stride_samples, cfg->clip_samples);
   if (cfg->window_size_samples % 4 || cfg->window_stride_samples % 4 || cfg->clip_samples % 4)
     return fail(TCR_ERR_UNSUPPORTED, "window, stride and clip lengths must be multiples of 4 samples (16-byte TMA rows)");
-  if (cfg->num_mel_bins <= 0 || cfg->num_mel_bins > 128 || cfg->num_mfccs <= 0 || cfg->num_mfccs > cfg->num_mel_bins)
+  // num_mfccs only means something to the MFCC front-end: log-mel features with fewer bins than the default 40 coefficients are valid
+  if (cfg->num_mel_bins <= 0 || cfg->num_mel_bins > 128 ||
+      (cfg->feature_kind == TCR_FEATURE_MFCC && (cfg->num_mfccs <= 0 || cfg->num_mfccs > cfg->num_mel_bins)))
     return fail(TCR_ERR_INVALID, "bad num_mel_bins/num_mfccs (%d/%d)", cfg->num_mel_bins, cfg->num_mfccs);
   if (cfg->feature_kind != TCR_FEATURE_MFCC && cfg->feature_kind != TCR_FEATURE_LOG_MEL)
     return fail(TCR_ERR_INVALID, "bad feature_kind %d", cfg->feature_kind);

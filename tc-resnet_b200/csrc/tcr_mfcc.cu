@@ -292,48 +292,54 @@ __global__ void __launch_bounds__(224, (NF2 <= 512) ? 4 : 2) mfcc_kernel(MfccArg
     __syncwarp();
     float* out = a.feat + ((size_t)utt * a.frames + (f0 + f)) * a.features;
     if (a.use_dct) {
-      // DCT: lane (q, g) = (lane / 8, lane % 8) sums mel bins m = q, q + 4, ... for coefficients c = g, g + 8, ...; the four
-      // quarter sums meet through two shuffles.  All 32 lanes stay busy for any coefficient count <= 64.
+      // DCT: lane (q, g) = (lane / 8, lane % 8) sums mel bins m = q, q + 4, ... for coefficients c = c0 + g, c0 + g + 8, ...;
+      // the four quarter sums meet through two shuffles.  A pass covers 64 coefficients (eight per lane), so all 32 lanes
+      // stay busy and the accumulators stay eight registers; more than 64 coefficients (up to 128) take a second pass.
       const int q = lane >> 3, g = lane & 7;
-      float acc[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-      const int nj = (a.features + 7) >> 3;
-      // DCT-II rows are mirror images: D[M-1-m][c] = (-1)^c D[m][c], and c = g + 8 j has the parity of g, so a lane folds
-      // the two halves of the log-mel vector first and walks only M/2 rows (odd M: the middle row is added unfolded).
+      // DCT-II rows are mirror images: D[M-1-m][c] = (-1)^c D[m][c], and c = c0 + g + 8 j has the parity of g (c0 is a
+      // multiple of 64), so a lane folds the two halves of the log-mel vector first and walks only M/2 rows (odd M: the
+      // middle row is added unfolded).
       const int M = a.mel_bins, half = M >> 1;
       const float sgn = (g & 1) ? -1.f : 1.f;
-      if (a.features == 40) {                               // the usual 40 coefficients: five per lane, no bound checks
-#pragma unroll 4
-        for (int m = q; m < half; m += 4) {
-          const float v = fmaf(sgn, lm[M - 1 - m], lm[m]);
-          const float* row = a.dct + m * 40 + g;
+#pragma unroll 1
+      for (int c0 = 0; c0 < a.features; c0 += 64) {
+        float acc[8];
 #pragma unroll
-          for (int j = 0; j < 5; ++j) acc[j] = fmaf(v, __ldg(row + 8 * j), acc[j]);
-        }
-      } else {
+        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+        const int nj = min((a.features - c0 + 7) >> 3, 8);
+        const int cg = c0 + g;                                // this lane's first coefficient of the pass
+        if (a.features == 40) {                             // the usual 40 coefficients: five per lane, no bound checks
 #pragma unroll 4
-        for (int m = q; m < half; m += 4) {
-          const float v = fmaf(sgn, lm[M - 1 - m], lm[m]);
-          const float* row = a.dct + m * a.features + g;
+          for (int m = q; m < half; m += 4) {
+            const float v = fmaf(sgn, lm[M - 1 - m], lm[m]);
+            const float* row = a.dct + m * 40 + g;
+#pragma unroll
+            for (int j = 0; j < 5; ++j) acc[j] = fmaf(v, __ldg(row + 8 * j), acc[j]);
+          }
+        } else {
+#pragma unroll 4
+          for (int m = q; m < half; m += 4) {
+            const float v = fmaf(sgn, lm[M - 1 - m], lm[m]);
+            const float* row = a.dct + m * a.features + cg;
+#pragma unroll
+            for (int j = 0; j < 8; ++j)
+              if (j < nj && cg + 8 * j < a.features) acc[j] = fmaf(v, __ldg(row + 8 * j), acc[j]);
+          }
+        }
+        if ((M & 1) && q == 0) {
+          const float v = lm[half];
+          const float* row = a.dct + half * a.features + cg;
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            if (j < nj && g + 8 * j < a.features) acc[j] = fmaf(v, __ldg(row + 8 * j), acc[j]);
+            if (j < nj && cg + 8 * j < a.features) acc[j] = fmaf(v, __ldg(row + 8 * j), acc[j]);
         }
-      }
-      if ((M & 1) && q == 0) {
-        const float v = lm[half];
-        const float* row = a.dct + half * a.features + g;
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
-          if (j < nj && g + 8 * j < a.features) acc[j] = fmaf(v, __ldg(row + 8 * j), acc[j]);
-      }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        if (j < nj) {
-          acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], 8);
-          acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], 16);
-          if (q == 0 && g + 8 * j < a.features) out[g + 8 * j] = acc[j];
+        for (int j = 0; j < 8; ++j) {
+          if (j < nj) {
+            acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], 8);
+            acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], 16);
+            if (q == 0 && cg + 8 * j < a.features) out[cg + 8 * j] = acc[j];
+          }
         }
       }
     } else {

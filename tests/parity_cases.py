@@ -56,14 +56,76 @@ def check_argmax(logits, ref_logits, err_abs):
     return int((~decided).sum())
 
 
+def reference_features(wav, window, stride, sample_rate=16000, mel=64, mfcc=40, lower=80.0, upper=7600.0, feature_kind=0,
+                       dtype=np.float64):
+    """The oracle front-end of a handle's configuration: MFCCs (feature_kind 0) or the magnitude log-mel spectrogram (1)."""
+    if feature_kind == 0:
+        return O.mfcc(wav, window, stride, mel, mfcc, sample_rate, lower, upper, dtype)
+    return O.log_mel_spectrogram(wav, window, stride, False, mel, sample_rate, lower, upper, dtype)
+
+
+def check_eval(eng, spec, inp, feat, onehot, params, moving, wd, ls, report, tag="eval", is_features=False):
+    """evaluate_audio.py path (moving statistics, dropout identity) against the oracle; the CUDA path gets the variables in fp32."""
+    ev = eng.forward(inp, O.flatten_vars(spec, params), O.flatten_moving(spec, moving), is_features=is_features, onehot_np=onehot, weight_decay=wd)
+    ref_logits, _ = O.forward(spec, params, moving, feat, False)
+    ref_total, ref_model = O.losses(spec, params, ref_logits, onehot, wd, ls)
+    report[f"{tag}_logits"] = rel_err(ev["logits"], ref_logits)
+    assert report[f"{tag}_logits"] <= TOL_LOGITS, report
+    check_argmax(ev["logits"], ref_logits, report[f"{tag}_logits"] * np.abs(ref_logits).max())
+    np.testing.assert_allclose(ev["probs"], O.softmax(ref_logits), rtol=0, atol=2e-5)
+    assert abs(ev["losses"][0] - ref_total) <= 1e-4 * abs(ref_total) + 1e-6
+    assert abs(ev["losses"][1] - ref_model) <= 1e-4 * abs(ref_model) + 1e-6
+
+
+def check_step(eng, spec, inp, feat, onehot, state, lr, mom, wd, keep, mask, ls, report, tag, seed=0, is_features=False,
+               check_f32_floor=False, force_masks=False, feat_f32=None):
+    """One training step of the CUDA path from the flat state (params, moving, slots) against the oracle step started from the
+    same state; returns the CUDA path's post-step state.  feat_f32: the features the fp32 restatement of the oracle starts
+    from (default: the fp64 features rounded to fp32)."""
+    pf_c, mf_c, sf_c = state
+    n = inp.shape[0]
+    p = O.unflatten_vars(spec, pf_c)
+    mv = O.unflatten_moving(spec, mf_c)
+    sl = O.unflatten_vars(spec, sf_c)
+    ts = eng.train_step(inp, onehot, pf_c, sf_c, mf_c, lr, mom, wd, is_features=is_features, mask_np=mask, seed=seed)
+    forced = cuda_relu_masks(eng, spec, n) if force_masks else None
+    p1, mv1, sl1, ref = O.train_step(spec, p, mv, sl, feat, onehot, lr, mom, wd, keep, mask, ls, forced_masks=forced)
+    report[f"train_logits{tag}"] = rel_err(ts["logits"], ref["logits"])
+    report[f"grads{tag}"] = rel_err(ts["grads"], O.flatten_vars(spec, ref["grads"], np.float64))
+    report[f"params{tag}"] = rel_err(ts["params"], O.flatten_vars(spec, p1, np.float64))
+    report[f"slots{tag}"] = rel_err(ts["slots"], O.flatten_vars(spec, sl1, np.float64))
+    report[f"moving{tag}"] = rel_err(ts["moving"], O.flatten_moving(spec, mv1, np.float64))
+    floor = 0.0
+    if check_f32_floor:                      # every step: the fp32 NumPy oracle's own distance to fp64 on this input
+        p32, mv32, sl32 = (O.cast_vars(d, np.float32) for d in (p, mv, sl))
+        f32 = feat.astype(np.float32) if feat_f32 is None else feat_f32
+        _, _, _, r32 = O.train_step(spec, p32, mv32, sl32, f32, onehot, lr, mom, wd, keep, mask, ls)
+        floor = 4 * rel_err(O.flatten_vars(spec, r32["grads"], np.float64), O.flatten_vars(spec, ref["grads"], np.float64))
+        report[f"grads_f32_oracle_floor{tag}"] = floor / 4
+    assert report[f"train_logits{tag}"] <= TOL_LOGITS, report
+    assert report[f"grads{tag}"] <= max(TOL_STATE, floor), report
+    assert report[f"params{tag}"] <= max(TOL_STATE, floor), report
+    assert report[f"slots{tag}"] <= max(TOL_STATE, floor), report
+    assert report[f"moving{tag}"] <= TOL_STATE, report
+    assert abs(ts["losses"][0] - ref["total_loss"]) <= 1e-4 * abs(ref["total_loss"]) + 1e-6
+    assert abs(ts["losses"][1] - ref["model_loss"]) <= 1e-4 * abs(ref["model_loss"]) + 1e-6
+    return ts["params"], ts["moving"], ts["slots"]
+
+
 def run_case(backend, model="TCResNet8", wm=1.0, window=640, stride=320, n=4, keep=1.0, ls=0.0, use_wav=True,
-             steps=1, adversarial=True, max_batch=None, check_f32_floor=False, force_masks=False):
-    t = O.num_frames(16000, window, stride)
-    spec = O.build_spec(model, wm, t)
+             steps=1, adversarial=True, max_batch=None, check_f32_floor=False, force_masks=False, sample_rate=16000, clip=16000,
+             mel=64, mfcc=40, lower=80.0, upper=7600.0, num_classes=12, feature_kind=0, f32_front_end=False):
+    """f32_front_end: with check_f32_floor, the fp32 restatement of the oracle also computes its features in fp32, so the floor
+    includes the front-end's round-off as the gradient amplifies it (log-mel features keep ~1e-5 of it in their quiet bands)."""
+    t = O.num_frames(clip, window, stride)
+    f_in = mfcc if feature_kind == 0 else mel
+    spec = O.build_spec(model, wm, t, f_in=f_in, num_classes=num_classes)
     eng = Engine(backend, model=int(model[len("TCResNet"):]), width_multiplier=wm, max_batch=max_batch or max(n, 8),
-                 dropout_keep_prob=keep, window_size_samples=window, window_stride_samples=stride, label_smoothing=ls)
+                 dropout_keep_prob=keep, window_size_samples=window, window_stride_samples=stride, label_smoothing=ls,
+                 sample_rate=sample_rate, clip_samples=clip, num_mel_bins=mel, num_mfccs=mfcc, lower_edge_hertz=lower,
+                 upper_edge_hertz=upper, num_classes=num_classes, feature_kind=feature_kind)
     try:
-        assert eng.info.frames == t and eng.info.num_trainable == O.count_trainable(spec)
+        assert eng.info.frames == t and eng.info.features == f_in and eng.info.num_trainable == O.count_trainable(spec)
         assert eng.info.forward_flops_per_utt == O.forward_flops(spec)
         tab = eng.param_table()
         assert [d["name"] for d in tab if d["kind"] < 3] == spec.var_names
@@ -71,8 +133,8 @@ def run_case(backend, model="TCResNet8", wm=1.0, window=640, stride=320, n=4, ke
         params, moving = perturbed_variables(spec)
         rng = np.random.RandomState(7)
         slots = {k: 0.01 * rng.randn(*v.shape) for k, v in params.items()}
-        wav, onehot = O.synthetic_batch(n, adversarial=adversarial)
-        feat = O.mfcc(wav, window, stride)
+        wav, onehot = O.synthetic_batch(n, num_samples=clip, num_classes=num_classes, adversarial=adversarial)
+        feat = reference_features(wav, window, stride, sample_rate, mel, mfcc, lower, upper, feature_kind)
         mask = (rng.rand(n, spec.c_last) < keep).astype(np.float32) if keep < 1 else None
         lr, mom, wd = 0.1, 0.9, 1e-3
         report = {}
@@ -83,49 +145,17 @@ def run_case(backend, model="TCResNet8", wm=1.0, window=640, stride=320, n=4, ke
         assert report["features"] <= TOL_FEATURES, report
 
         inp = wav if use_wav else feat.astype(np.float32)
-        pf, mf, sf = O.flatten_vars(spec, params), O.flatten_moving(spec, moving), O.flatten_vars(spec, slots)
-
-        # evaluate_audio.py path: moving statistics, dropout identity
-        ev = eng.forward(inp, pf, mf, is_features=not use_wav, onehot_np=onehot, weight_decay=wd)
-        ref_logits, _ = O.forward(spec, params, moving, feat, False)
-        ref_total, ref_model = O.losses(spec, params, ref_logits, onehot, wd, ls)
-        report["eval_logits"] = rel_err(ev["logits"], ref_logits)
-        assert report["eval_logits"] <= TOL_LOGITS, report
-        check_argmax(ev["logits"], ref_logits, report["eval_logits"] * np.abs(ref_logits).max())
-        np.testing.assert_allclose(ev["probs"], O.softmax(ref_logits), rtol=0, atol=2e-5)
-        assert abs(ev["losses"][0] - ref_total) <= 1e-4 * abs(ref_total) + 1e-6
-        assert abs(ev["losses"][1] - ref_model) <= 1e-4 * abs(ref_model) + 1e-6
+        feat_f32 = reference_features(wav, window, stride, sample_rate, mel, mfcc, lower, upper, feature_kind, np.float32) \
+            if f32_front_end and use_wav else None
+        check_eval(eng, spec, inp, feat, onehot, params, moving, wd, ls, report, is_features=not use_wav)
 
         # training steps.  Each step is compared against the oracle started from the CUDA path's OWN previous state
         # (re-synchronised), so the check is per-step parity + correct carrying of state between calls, not the
         # divergence of two chaotic lr=0.1 trajectories (ReLU masks flip under 1e-6 perturbations).
-        pf_c, mf_c, sf_c = pf, mf, sf
+        state = O.flatten_vars(spec, params), O.flatten_moving(spec, moving), O.flatten_vars(spec, slots)
         for step in range(steps):
-            p = O.unflatten_vars(spec, pf_c)
-            mv = O.unflatten_moving(spec, mf_c)
-            sl = O.unflatten_vars(spec, sf_c)
-            ts = eng.train_step(inp, onehot, pf_c, sf_c, mf_c, lr, mom, wd, is_features=not use_wav, mask_np=mask, seed=step)
-            forced = cuda_relu_masks(eng, spec, n) if force_masks else None
-            p1, mv1, sl1, ref = O.train_step(spec, p, mv, sl, feat, onehot, lr, mom, wd, keep, mask, ls, forced_masks=forced)
-            pf_c, mf_c, sf_c = ts["params"], ts["moving"], ts["slots"]
-            report[f"train_logits{step}"] = rel_err(ts["logits"], ref["logits"])
-            report[f"grads{step}"] = rel_err(ts["grads"], O.flatten_vars(spec, ref["grads"], np.float64))
-            report[f"params{step}"] = rel_err(ts["params"], O.flatten_vars(spec, p1, np.float64))
-            report[f"slots{step}"] = rel_err(ts["slots"], O.flatten_vars(spec, sl1, np.float64))
-            report[f"moving{step}"] = rel_err(ts["moving"], O.flatten_moving(spec, mv1, np.float64))
-            floor = 0.0
-            if check_f32_floor:                      # every step: the fp32 NumPy oracle's own distance to fp64 on this input
-                p32, mv32, sl32 = (O.cast_vars(d, np.float32) for d in (p, mv, sl))
-                _, _, _, r32 = O.train_step(spec, p32, mv32, sl32, feat.astype(np.float32), onehot, lr, mom, wd, keep, mask, ls)
-                floor = 4 * rel_err(O.flatten_vars(spec, r32["grads"], np.float64), O.flatten_vars(spec, ref["grads"], np.float64))
-                report[f"grads_f32_oracle_floor{step}"] = floor / 4
-            assert report[f"train_logits{step}"] <= TOL_LOGITS, report
-            assert report[f"grads{step}"] <= max(TOL_STATE, floor), report
-            assert report[f"params{step}"] <= max(TOL_STATE, floor), report
-            assert report[f"slots{step}"] <= max(TOL_STATE, floor), report
-            assert report[f"moving{step}"] <= TOL_STATE, report
-            assert abs(ts["losses"][0] - ref["total_loss"]) <= 1e-4 * abs(ref["total_loss"]) + 1e-6
-            assert abs(ts["losses"][1] - ref["model_loss"]) <= 1e-4 * abs(ref["model_loss"]) + 1e-6
+            state = check_step(eng, spec, inp, feat, onehot, state, lr, mom, wd, keep, mask, ls, report, step, seed=step,
+                               is_features=not use_wav, check_f32_floor=check_f32_floor, force_masks=force_masks, feat_f32=feat_f32)
         return report
     finally:
         eng.close()

@@ -76,6 +76,63 @@ def test_stft_against_direct_dft():
         assert abs(spec[0, 3, k] - abs(x) ** 2) <= 1e-9 * max(1.0, abs(x) ** 2)
 
 
+@pytest.mark.parametrize("window,stride,clip", [(128, 64, 16000), (256, 128, 16000), (1600, 640, 16000), (240, 80, 8000)])
+def test_stft_against_direct_dft_at_every_fft_length(window, stride, clip):
+    """FFT 128, 256 and 2048 (and 256 from a 240-sample window): every bin of two frames, DC and Nyquist included."""
+    wav, _ = O.synthetic_batch(2, num_samples=clip, adversarial=True)
+    fft = O.next_pow2(window)
+    spec = O.power_spectrogram(wav, window, stride)
+    mag = O.power_spectrogram(wav, window, stride, magnitude_squared=False)
+    t = O.num_frames(clip, window, stride)
+    assert spec.shape == (2, t, fft // 2 + 1)
+    n, k = np.arange(window), np.arange(fft // 2 + 1)
+    basis = np.exp(-2j * np.pi * np.outer(n, k) / fft)
+    for c, f in ((0, 0), (1, t // 2), (1, t - 1)):
+        frame = wav[c, f * stride:f * stride + window].astype(np.float64) * O.hann_window_periodic(window)
+        x = frame @ basis
+        np.testing.assert_allclose(spec[c, f], np.abs(x) ** 2, rtol=1e-9, atol=1e-9)
+        np.testing.assert_allclose(mag[c, f], np.abs(x), rtol=1e-9, atol=1e-9)
+
+
+@pytest.mark.parametrize("bins,sample_rate,lower,upper,fft", [
+    (32, 16000, 80.0, 7600.0, 128), (64, 16000, 80.0, 7600.0, 128), (40, 16000, 20.0, 8000.0, 256), (41, 16000, 80.0, 7600.0, 1024),
+    (80, 16000, 80.0, 7600.0, 1024), (128, 16000, 20.0, 7600.0, 1024), (96, 16000, 80.0, 7600.0, 1024),
+    (64, 16000, 80.0, 7600.0, 2048), (40, 8000, 80.0, 7600.0, 256)])
+def test_mel_matrix_against_the_independent_port_at_every_geometry(bins, sample_rate, lower, upper, fft):
+    try:
+        from transformers.models.lasr.feature_extraction_lasr import linear_to_mel_weight_matrix as port
+    except Exception:
+        pytest.skip("transformers LASR feature extractor not importable")
+    w = O.linear_to_mel_weight_matrix(bins, fft // 2 + 1, sample_rate, lower, upper)
+    ref = port(num_mel_bins=bins, num_spectrogram_bins=fft // 2 + 1, sample_rate=sample_rate, lower_edge_hertz=lower,
+               upper_edge_hertz=upper, dtype=np.float64)
+    np.testing.assert_allclose(w, ref, rtol=1e-9, atol=1e-12)
+    assert np.all(w[0] == 0) and int((w > 0).sum(axis=1).max()) <= 2
+
+
+def test_bands_above_nyquist_and_between_bins_are_exactly_the_log_offset():
+    """8 kHz with the default 7600 Hz upper edge: the bands above 4 kHz cover no FFT bin, so they are log(1e-6) for any input.
+    FFT 128 at 64 bands: narrow low bands fall between two bins and are empty too."""
+    wav, _ = O.synthetic_batch(3, num_samples=8000, adversarial=True)
+    w = O.linear_to_mel_weight_matrix(40, 129, 8000, 80.0, 7600.0)
+    empty = np.flatnonzero(w.sum(axis=0) == 0)
+    assert list(empty) == list(range(32, 40))
+    lm = O.log_mel_spectrogram(wav, 240, 80, num_mel_bins=40, sample_rate=8000)
+    assert np.all(lm[..., empty] == math.log(1e-6)) and np.all(lm[1:, :, :32] > math.log(1e-6))
+    wav, _ = O.synthetic_batch(3, adversarial=True)
+    empty = np.flatnonzero(O.linear_to_mel_weight_matrix(64, 65, 16000, 80.0, 7600.0).sum(axis=0) == 0)
+    assert list(empty) == [2, 3, 6, 9, 12, 15]
+    lm = O.log_mel_spectrogram(wav, 128, 64)
+    assert np.all(lm[..., empty] == math.log(1e-6))
+
+
+@pytest.mark.parametrize("mel,mfccs", [(64, 12), (40, 20), (80, 32), (128, 64), (41, 40), (41, 12), (64, 64)])
+def test_dct_matches_scipy_at_every_coefficient_count(mel, mfccs):
+    x = np.random.RandomState(mel + mfccs).randn(5, mel)
+    ref = scipy.fft.dct(x, type=2, norm=None, axis=-1)[:, :mfccs] / math.sqrt(2 * mel)
+    np.testing.assert_allclose(x @ O.dct2_matrix(mel, mfccs), ref, rtol=1e-12, atol=1e-12)
+
+
 def test_silence_gives_log_offset():
     wav = np.zeros((1, 16000), np.float32)
     lm = O.log_mel_spectrogram(wav, 640, 320)
