@@ -23,6 +23,14 @@ static int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+// "outer: inner", where inner is the message a nested call left in g_err.  It is copied out first: vsnprintf must not read
+// the buffer it writes.
+static int fail_wrap(int code, const char* outer) {
+  char inner[sizeof(g_err)];
+  snprintf(inner, sizeof(inner), "%s", g_err);
+  return fail(code, "%s: %s", outer, inner);
+}
+
 #define TCR_CUDA(call)                                                                         \
   do {                                                                                         \
     cudaError_t e_ = (call);                                                                   \
@@ -438,7 +446,7 @@ extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
   rc = build_plan(h);
   if (rc) return bail(rc);
   rc = net_alloc_workspace(h);
-  if (rc) return bail(fail(rc, "workspace allocation failed: %s", g_err));
+  if (rc) return bail(fail_wrap(rc, "workspace allocation failed"));
   *out = h;
   return TCR_OK;
 }
@@ -623,7 +631,7 @@ extern "C" int tcr_forward(tcr_handle* h, const float* input, int32_t input_is_f
   }
   int rc = net_forward(h, feat, params, moving, n, is_training != 0, dropout_seed, dropout_mask, onehot, weight_decay,
                        logits, probs, losses, /*backward=*/false, s);
-  if (rc) return fail(rc, "forward launch failed: %s", g_err);
+  if (rc) return fail_wrap(rc, "forward launch failed");
   TCR_CUDA(cudaGetLastError());
   h->last_n = n;
   return TCR_OK;
@@ -762,12 +770,12 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
   int rc = resident != kResidentOff ? resident_forward(h, feat, a, s)
                                     : net_forward(h, feat, a->params, nullptr, a->n, true, a->dropout_seed, a->dropout_mask, a->onehot,
                                                   a->weight_decay, a->logits, a->probs, nullptr, /*backward=*/true, s);
-  if (rc) return fail(rc, "forward launch failed: %s", g_err);
+  if (rc) return fail_wrap(rc, "forward launch failed");
   rc = resident == kResidentFwdBwdData && h->bwd_phases > 0 ? resident_backward_data(h, feat, a, s)
                                                             : net_backward_data(h, a->params, a->n, s);
-  if (rc) return fail(rc, "backward launch failed: %s", g_err);
+  if (rc) return fail_wrap(rc, "backward launch failed");
   rc = net_weight_gradients(h, feat, a->n, s);
-  if (rc) return fail(rc, "weight-gradient launch failed: %s", g_err);
+  if (rc) return fail_wrap(rc, "weight-gradient launch failed");
 #ifndef TCR_EMU
   if (h->fe_gate) {                   // the gate of the NEXT step's front-end (see above)
     TCR_CUDA(cudaEventRecord((cudaEvent_t)h->fe_gate, s));
@@ -775,7 +783,7 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
   }
 #endif
   rc = net_update(h, a, s);
-  if (rc) return fail(rc, "update launch failed: %s", g_err);
+  if (rc) return fail_wrap(rc, "update launch failed");
   TCR_CUDA(cudaGetLastError());
 #ifndef TCR_EMU
   if (fe_buf >= 0) TCR_CUDA(cudaEventRecord((cudaEvent_t)h->fe_free[fe_buf], s));

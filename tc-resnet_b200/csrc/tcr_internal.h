@@ -20,6 +20,7 @@ namespace tcr {
 constexpr int kMaxConvs = 24;
 constexpr int kMaxBlocks = 8;
 constexpr int kThreads = 256;        // conv fwd / bwd-data CTAs
+constexpr int kOptThreads = 256;     // grad_finalize / update CTAs: one w^2 partial sum per grad_finalize CTA
 constexpr int kMaxClasses = 32;
 
 // Forward statistics of a layer as its producer kernel left them (tcr_bn.cuh): per-cluster records that the consumer

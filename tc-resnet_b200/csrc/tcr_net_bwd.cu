@@ -323,7 +323,8 @@ static size_t bwd_data_smem(const ConvPlan& cv, const ConvPlan* dn, int U, int K
 
 double tile_cost(int sms, int n, int U, int occ, bool wsm);     // tcr_net_fwd.cu
 
-static void pick_bwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n, int* U_out, int* KS_out, int* wsm_out) {
+// false: not even the smallest tile (one utterance, one slice, filters through L1/L2) fits in `limit` bytes (see pick_fwd_tile)
+static bool pick_bwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n, size_t limit, int* U_out, int* KS_out, int* wsm_out) {
   const size_t wbytes = ((size_t)cv.wnumel() + (dn ? (size_t)dn->wnumel() : 0)) * 4;
   const int S = cv.stride, NT0 = (cv.k + S - 1) / S;
   double best = 1e30;
@@ -353,6 +354,7 @@ static void pick_bwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n
       break;
     }
   }
+  return best < 1e30 || bwd_data_smem(cv, dn, 1, 1, false) <= limit;
 }
 
 static size_t bwd_weight_smem(const ConvPlan& cv, int cot, int RG, int UB) {
@@ -413,6 +415,58 @@ void plan_bwd_weight(tcr_handle* h) {
     cv.dw_R = R;
     cv.dw_UB = UB;
   }
+}
+
+// What the per-layer path can run, checked once when the handle is created (after plan_bwd_weight): a handle tcr_create accepts
+// can always evaluate (tcr_forward runs only these kernels) and always train with TCR_RESIDENT=0.  No layer has more than
+// kThreads / 2 channels, the head keeps its two-CTAs-per-SM budget; every convolution's smallest forward and backward-data tile (one
+// utterance per CTA) and its planned weight-gradient tile must fit in what one CTA may opt in to.  The resident kernels are not
+// part of it: where their layout does not fit, the step falls back to these.
+int net_check_envelope(tcr_handle* h) {
+  char msg[256];
+  auto refuse = [&](const std::string& what, size_t need, size_t limit) {
+    snprintf(msg, sizeof(msg), "%s needs %zu B of shared memory, limit %zu B: shorten the clip or the width", what.c_str(), need, limit);
+    set_error(msg);
+    return TCR_ERR_UNSUPPORTED;
+  };
+  // the one-pass BatchNorm statistics of the per-layer kernels (tile_stats, records_sum) give each of a layer's 2 x C columns
+  // one of the CTA's kThreads threads
+  int c_max = 0;
+  for (const ConvPlan& cv : h->convs) c_max = std::max(c_max, cv.cout);
+  if (2 * c_max > kThreads) {
+    snprintf(msg, sizeof(msg), "%s has a %d-channel layer, the per-layer kernels' BatchNorm statistics take at most %d channels: lower the width",
+             h->scope.c_str(), c_max, kThreads / 2);
+    set_error(msg);
+    return TCR_ERR_UNSUPPORTED;
+  }
+  const size_t limit = h->smem_optin;
+  int U, KS, wsm;
+  const ConvPlan& c0 = h->convs[0];
+  if (!pick_fwd_tile(h->sms, c0, nullptr, 1, limit, &U, &KS, &wsm))
+    return refuse("forward tile of " + h->scope + "/" + c0.name, fwd_smem_bytes(c0, nullptr, 1, 1, false), limit);
+  for (const BlockPlan& b : h->blocks) {
+    const ConvPlan& ca = h->convs[b.a];
+    const ConvPlan& cb = h->convs[b.b];
+    const ConvPlan* dn = b.down >= 0 ? &h->convs[b.down] : nullptr;
+    if (!pick_fwd_tile(h->sms, ca, dn, 1, limit, &U, &KS, &wsm))
+      return refuse("forward tile of " + h->scope + "/" + ca.name, fwd_smem_bytes(ca, dn, 1, 1, false), limit);
+    if (!pick_fwd_tile(h->sms, cb, nullptr, 1, limit, &U, &KS, &wsm))
+      return refuse("forward tile of " + h->scope + "/" + cb.name, fwd_smem_bytes(cb, nullptr, 1, 1, false), limit);
+    if (!pick_bwd_tile(h->sms, ca, dn, 1, limit, &U, &KS, &wsm))
+      return refuse("backward-data tile of " + h->scope + "/" + ca.name, bwd_data_smem(ca, dn, 1, 1, false), limit);
+    if (!pick_bwd_tile(h->sms, cb, nullptr, 1, limit, &U, &KS, &wsm))
+      return refuse("backward-data tile of " + h->scope + "/" + cb.name, bwd_data_smem(cb, nullptr, 1, 1, false), limit);
+  }
+  for (const ConvPlan& cv : h->convs) {
+    const size_t need = bwd_weight_smem(cv, cv.dw_cot, cv.dw_RG, cv.dw_UB);
+    if (need > limit) return refuse("weight-gradient tile of " + h->scope + "/" + cv.name, need, limit);
+  }
+  if (head_smem_bytes(h) > kSmemBudget) {
+    char what[128];
+    snprintf(what, sizeof(what), "head tile of %s (T_last %d, %d channels)", h->scope.c_str(), h->t_last, h->c_last);
+    return refuse(what, head_smem_bytes(h), kSmemBudget);
+  }
+  return 0;
 }
 
 // Device table of the grouped weight-gradient launch (pointers are workspace addresses: static per handle).  Only the layers
@@ -502,7 +556,10 @@ static DySrc make_dy(const tcr_handle* h, const ConvPlan& cv, const float* dz, i
 // *gc_out: per-cluster records of BatchNorm-backward sums this launch leaves for the layer(s) below (0 when recording)
 static int bwd_data(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, BwdDataArgs a, int n, cudaStream_t s, int* gc_out) {
   int U, KS, wsm;
-  pick_bwd_tile(h->sms, cv, dn, n, &U, &KS, &wsm);
+  if (!pick_bwd_tile(h->sms, cv, dn, n, h->smem_optin, &U, &KS, &wsm)) {   // tcr_create refuses such a handle (net_check_envelope)
+    set_error("backward-data tile does not fit in shared memory");
+    return TCR_ERR_UNSUPPORTED;
+  }
   a.n = n; a.U = U; a.w_smem = wsm;
   a.w = cv.wT; a.cin = cv.cin; a.cout = cv.cout; a.k = cv.k; a.stride = cv.stride;
   a.t_in = cv.t_in; a.t_out = cv.t_out; a.pad_left = cv.pad_left; a.KS = KS;
@@ -637,6 +694,7 @@ int net_backward_data(tcr_handle* h, const float* params, int n, cudaStream_t s)
 // weight gradients: every layer's inputs are final now -> one grouped launch over all layers
 int net_weight_gradients(tcr_handle* h, const float* feat, int n, cudaStream_t s) {
   if (h->dw_ctas == 0) return 0;     // no conv weight is trained
+  if (h->dw_smem > h->smem_optin) { set_error("weight-gradient tile does not fit in shared memory"); return TCR_ERR_UNSUPPORTED; }
   {
     auto kfn = dw_grouped_kernel;
 #ifndef TCR_EMU

@@ -331,7 +331,9 @@ double tile_cost(int sms, int n, int U, int occ, bool wsm) {
   return waves * (U * (occ == 2 ? 1.7 : 1.8) * (wsm ? 1.0 : 1.1) + 4.0);
 }
 
-static void pick_fwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n, int* U_out, int* KS_out, int* wsm_out) {
+// false: not even one utterance per CTA, one k-slice and the filters through L1/L2 fit in `limit` bytes.  Past the planner's
+// own budgets, that smallest tile is taken as long as the device can run it.
+static bool pick_fwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n, size_t limit, int* U_out, int* KS_out, int* wsm_out) {
   const size_t wbytes = fwd_weight_floats(cv, dn) * 4;
   double best = 1e30;
   *U_out = 1; *KS_out = 1; *wsm_out = 0;
@@ -360,6 +362,7 @@ static void pick_fwd_tile(int sms, const ConvPlan& cv, const ConvPlan* dn, int n
       break;                        // the largest U that fits is the candidate of this pass
     }
   }
+  return best < 1e30 || fwd_smem_bytes(cv, dn, 1, 1, false) <= limit;
 }
 
 template <class T>
@@ -383,12 +386,33 @@ static int ws_alloc(tcr_handle* h, T** p, size_t count) {
   } while (0)
 
 void plan_bwd_weight(tcr_handle* h);   // tcr_net_bwd.cu
+int net_check_envelope(tcr_handle* h);
+
+// The largest dynamic shared memory one CTA may opt in to: the device's limit (232,448 B on an H100).  The emulator takes the
+// H100's value, so both builds refuse the same configurations.
+static size_t smem_optin_limit(const tcr_handle* h) {
+#ifdef TCR_EMU
+  (void)h;
+  return 232448;
+#else
+  int v = 0;
+  if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->cfg.device) != cudaSuccess || v <= 0) return 48 * 1024;
+  return (size_t)v;
+#endif
+}
+
+// Head tile of the per-layer path (kHeadU utterances, the residual, pooled and gradient planes of the last block): bytes.
+static size_t head_smem_bytes(const tcr_handle* h) {
+  return (head_smem_floats(h->t_last, h->c_last, h->cfg.num_classes) + 8) * 4;
+}
 
 int net_alloc_workspace(tcr_handle* h) {
   const size_t N = (size_t)h->cfg.max_batch;
   h->g_max = h->cfg.max_batch;                       // U >= 1 -> at most max_batch CTA groups
   h->head_groups_max = head_groups(h->cfg.max_batch);
+  h->smem_optin = smem_optin_limit(h);
   plan_bwd_weight(h);
+  WS(net_check_envelope(h));
   WS(ws_alloc(h, &h->d_feat, N * h->frames * h->features));
   WS(ws_alloc(h, &h->d_logits, N * h->cfg.num_classes));
   WS(ws_alloc(h, &h->d_probs, N * h->cfg.num_classes));
@@ -417,7 +441,7 @@ int net_alloc_workspace(tcr_handle* h) {
   WS(ws_alloc(h, &h->d_loss, 4));
   WS(ws_alloc(h, &h->d_dwfc_part, rec_max * h->c_last * h->cfg.num_classes));
   WS(ws_alloc(h, &h->d_grads, (size_t)h->n_train));
-  WS(ws_alloc(h, &h->d_l2part, 4096));
+  WS(ws_alloc(h, &h->d_l2part, (size_t)((h->n_train + kOptThreads - 1) / kOptThreads)));   // one sum of w^2 per grad_finalize CTA
   WS(ws_alloc(h, &h->d_hyper, 1));
   WS(ws_alloc(h, &h->d_gridbar, 64));
   cudaMemset(h->d_gridbar, 0, 64 * sizeof(unsigned));
@@ -478,7 +502,10 @@ static int launch_conv_fwd(const char* name, const FwdArgs& a, int groups, size_
 static int conv_fwd(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, FwdArgs a, const float* params, int n, bool training,
                     cudaStream_t s) {
   int U, KS, wsm;
-  pick_fwd_tile(h->sms, cv, dn, n, &U, &KS, &wsm);
+  if (!pick_fwd_tile(h->sms, cv, dn, n, h->smem_optin, &U, &KS, &wsm)) {   // tcr_create refuses such a handle (net_check_envelope)
+    set_error("forward tile does not fit in shared memory");
+    return TCR_ERR_UNSUPPORTED;
+  }
   a.n = n; a.U = U; a.t_in = cv.t_in; a.cin = cv.cin; a.w_smem = wsm;
   a.w = params + cv.w_off; a.y = cv.y; a.fpart = cv.fpart;
   a.cout = cv.cout; a.stride = cv.stride; a.t_out = cv.t_out; a.pad_left = cv.pad_left; a.KS = KS;
@@ -521,7 +548,6 @@ int net_forward(tcr_handle* h, const float* feat, const float* params, const flo
                 uint64_t seed, const float* mask, const float* onehot, float weight_decay, float* logits,
                 float* probs, float* losses, bool backward, cudaStream_t s) {
   (void)weight_decay;
-  if (h->c_last > kHeadThreads) { set_error("last_channels > 256 unsupported by the head kernel"); return TCR_ERR_UNSUPPORTED; }
   if (!training) {
     EvalBnArgs e;
     e.nlayers = (int)h->convs.size();
@@ -599,7 +625,7 @@ int net_forward(tcr_handle* h, const float* feat, const float* params, const flo
       h->fc_records = groups;           // CE records the loss / update kernel adds
       cb.b_gc = backward ? grid / CL : 0;
       if (dn) dn->b_gc = cb.b_gc;
-      const size_t smem = (head_smem_floats(lb.t, lb.c, ha.classes) + 8) * 4;
+      const size_t smem = head_smem_bytes(h);
       if (smem > kSmemBudget || lb.c > kHeadThreads) { set_error("head tile does not fit in shared memory"); return TCR_ERR_UNSUPPORTED; }
       {
 #ifndef TCR_EMU

@@ -17,8 +17,6 @@
 
 namespace tcr {
 
-constexpr int kOptThreads = 256;
-
 __device__ __forceinline__ int find_segment(const OptSegment* segs, int nsegs, int64_t p) {
   int lo = 0, hi = nsegs - 1;
   while (lo < hi) {
@@ -315,8 +313,7 @@ static int launch_update(int var, const UpdateArgs& u, int grid, cudaStream_t s)
 }
 
 int net_update(tcr_handle* h, const tcr_step_args* a, cudaStream_t s) {
-  const int blocks = (int)((h->n_train + kOptThreads - 1) / kOptThreads);
-  if (blocks > 4096) { set_error("parameter count too large for the l2 partial buffer"); return TCR_ERR_UNSUPPORTED; }
+  const int blocks = (int)((h->n_train + kOptThreads - 1) / kOptThreads);   // d_l2part holds one partial per block
   const bool p2p = h->p2p.attached && h->world > 1;
   if (p2p) ++h->p2p.step;
   float* grads = p2p ? h->p2p.grads + (size_t)(h->p2p.step & 1u) * h->n_train : h->d_grads;

@@ -53,6 +53,7 @@ struct tcr_handle {
   int64_t n_train = 0, n_moving = 0, fc_off = 0, fc2_off = 0;
   std::vector<tcr_param_desc> table;
   int g_max = 0;                 // max CTA groups of any producer kernel (partials are sized for it)
+  size_t smem_optin = 0;         // dynamic shared memory one CTA may opt in to (net_alloc_workspace)
   int head_groups_max = 0;
   // front-end tables
   float* d_fe_consts = nullptr; int c_tw2 = 0, c_melw = 0, c_win = 0, c_smem = 0;   // front-end constant block (tcr_mfcc.h)
