@@ -43,6 +43,54 @@ __device__ __forceinline__ void fold_bn(const float* p, int64_t b, int64_t beta,
   scale[c] = rstd;
   shift[c] = (p[b + c] - p[mm + c]) * rstd + p[beta + c];
 }
+__device__ __forceinline__ float4 bn_relu4(float4 a, float4 s, float4 t) {
+  return make_float4(fmaxf(fmaf(a.x, s.x, t.x), 0.f), fmaxf(fmaf(a.y, s.y, t.y), 0.f), fmaxf(fmaf(a.z, s.z, t.z), 0.f),
+                     fmaxf(fmaf(a.w, s.w, t.w), 0.f));
+}
+
+// Input rows (with halo) and padded width of a tile of RH output rows.
+TCR_HD inline int ds_in_rows(const DsLayerDev& L, int RH) { return (RH - 1) * L.sh + L.kh; }
+TCR_HD inline int ds_in_cols(const DsLayerDev& L) { return (L.wout - 1) * L.sw + L.kw; }
+TCR_HD inline int ds_tiles_per_utt(const DsLayerDev& L, int RH) { return (L.hout + RH - 1) / RH; }
+
+// Shared-memory layout of one DS-CNN kernel, in floats.  The kernel carves its pointers from it; the host sizes the launch and
+// checks its limits with the same function.  Regions: x the input tile(s) (xs floats per channel chunk, channel half or buffer,
+// as the kernel describes), a the A operand ([buffers][hi, lo][K / 4][lba]) or the FMA block's depthwise output, b the B
+// operand ([hi, lo][K / 4][gmma_lbb]) or an FMA kernel's filter bank, tab the per-channel tables, floats the total.
+struct DsSmem { size_t x, a, b, tab, floats; int xs, lba; };
+// The separable blocks' table region: depthwise taps [kh * kw][C], folded BatchNorm of the depthwise stage (sc1, sf1 [C]) and
+// of the pointwise stage (sc2, sf2 [CO]).
+struct DsTables { float *taps, *sc1, *sf1, *sc2, *sf2; };
+TCR_HD inline size_t ds_tab_floats(int taps, int C, int CO) { return (size_t)taps * C + 2 * C + 2 * CO; }
+__device__ __forceinline__ DsTables ds_stage_tables(float* base, const DsLayerDev& L, int taps, int C, int CO, const float* params,
+                                                    float eps, int tid, int nthreads) {
+  const DsTables t = {base, base + taps * C, base + taps * C + C, base + taps * C + 2 * C, base + taps * C + 2 * C + CO};
+#pragma unroll 1  // at most one iteration per thread in the wgmma kernels; unrolled, the FMA block kernel spills
+  for (int i = tid; i < taps * C / 4; i += nthreads) st4(t.taps + 4 * i, ldg4(params + L.w + 4 * i));
+#pragma unroll 1
+  for (int c = tid; c < C; c += nthreads) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, t.sc1, t.sf1);
+#pragma unroll 1
+  for (int c = tid; c < CO; c += nthreads) fold_bn(params, L.pb, L.pbeta, L.pmm, L.pmv, c, eps, t.sc2, t.sf2);
+  return t;
+}
+
+// dscnn_conv_kernel, one utterance: x [hp][wp] (rounded to 4), b [kh * kw][cout], tab sc, sf [cout]
+TCR_HD inline DsSmem conv_smem(const DsLayerDev& L) {
+  DsSmem s = {};
+  s.b = (ds_in_rows(L, L.hout) * ds_in_cols(L) + 3) & ~3;
+  s.tab = s.b + (size_t)L.kh * L.kw * L.cout;
+  s.floats = s.tab + 2 * L.cout;
+  return s;
+}
+// dscnn_dsblock_kernel, RH output rows: x [hin_t][wp][C], a [RH * wout][C], b [C][COT] (a tile of COT output channels), tab
+TCR_HD inline DsSmem dsblock_smem(const DsLayerDev& L, int RH, int COT) {
+  DsSmem s = {};
+  s.a = (size_t)ds_in_rows(L, RH) * ds_in_cols(L) * L.cin;
+  s.b = s.a + (size_t)RH * L.wout * L.cin;
+  s.tab = s.b + (size_t)L.cin * COT;
+  s.floats = s.tab + ds_tab_floats(L.kh * L.kw, L.cin, L.cout);
+  return s;
+}
 
 // ---- first layer: cin == 1 ----
 __global__ void __launch_bounds__(256) dscnn_conv_kernel(DsLayerDev L, const float* __restrict__ params, const float* __restrict__ in,
@@ -50,11 +98,9 @@ __global__ void __launch_bounds__(256) dscnn_conv_kernel(DsLayerDev L, const flo
   pdl_wait();
   TCR_DYNAMIC_SMEM(smem_raw);
   float* smem = reinterpret_cast<float*>(smem_raw);
-  const int hp = (L.hout - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;      // padded input extent
-  float* xs = smem;                                   // [hp][wp]
-  float* ws = xs + ((hp * wp + 3) & ~3);              // [kh*kw][cout]
-  float* sc = ws + L.kh * L.kw * L.cout;              // [cout]
-  float* sf = sc + L.cout;
+  const DsSmem S = conv_smem(L);
+  const int hp = ds_in_rows(L, L.hout), wp = ds_in_cols(L);      // padded input extent
+  float *xs = smem, *ws = smem + S.b, *sc = smem + S.tab, *sf = sc + L.cout;
   const int n = blockIdx.x, tid = threadIdx.x;
   for (int i = tid; i < hp * wp; i += blockDim.x) {
     const int h = i / wp - L.pt, w = i % wp - L.pl;
@@ -75,10 +121,7 @@ __global__ void __launch_bounds__(256) dscnn_conv_kernel(DsLayerDev L, const flo
         const float4 w = ld4(ws + (i * L.kw + j) * L.cout + 4 * c4);
         acc.x = fmaf(x, w.x, acc.x); acc.y = fmaf(x, w.y, acc.y); acc.z = fmaf(x, w.z, acc.z); acc.w = fmaf(x, w.w, acc.w);
       }
-    const float4 s = ld4(sc + 4 * c4), t = ld4(sf + 4 * c4);
-    const float4 r = make_float4(fmaxf(fmaf(acc.x, s.x, t.x), 0.f), fmaxf(fmaf(acc.y, s.y, t.y), 0.f),
-                                 fmaxf(fmaf(acc.z, s.z, t.z), 0.f), fmaxf(fmaf(acc.w, s.w, t.w), 0.f));
-    st4(out + ((size_t)n * npos + pos) * L.cout + 4 * c4, r);
+    st4(out + ((size_t)n * npos + pos) * L.cout + 4 * c4, bn_relu4(acc, ld4(sc + 4 * c4), ld4(sf + 4 * c4)));
   }
 }
 
@@ -91,16 +134,9 @@ __global__ void __launch_bounds__(256) dscnn_dsblock_kernel(DsLayerDev L, int RH
   float* smem = reinterpret_cast<float*>(smem_raw);
   const int C = L.cin, CO = L.cout;
   const int n = blockIdx.y, h0 = blockIdx.x * RH, rh = imin(RH, L.hout - h0), tid = threadIdx.x;
-  const int hin_t = (RH - 1) * L.sh + L.kh;                      // staged input rows (with halo)
-  const int wp = (L.wout - 1) * L.sw + L.kw;                     // padded width
-  float* xs = smem;                                              // [hin_t][wp][C]
-  float* ds = xs + (size_t)hin_t * wp * C;                       // [RH*wout][C]  depthwise output
-  float* pws = ds + (size_t)RH * L.wout * C;                     // [C][COT]      pointwise weights, a tile of COT output channels
-  float* dws = pws + (size_t)C * COT;                            // [kh*kw][C]    depthwise weights   (COT = CO unless the bank exceeds shared memory: DS-CNN-L)
-  float* sc1 = dws + L.kh * L.kw * C;                            // folded BN of the depthwise stage
-  float* sf1 = sc1 + C;
-  float* sc2 = sf1 + C;                                          // folded BN of the pointwise stage
-  float* sf2 = sc2 + CO;
+  const int hin_t = ds_in_rows(L, RH), wp = ds_in_cols(L);      // staged input rows (with halo), padded width
+  const DsSmem S = dsblock_smem(L, RH, COT);                     // COT = CO unless the bank exceeds shared memory: DS-CNN-L
+  float *xs = smem, *ds = smem + S.a, *pws = smem + S.b;
   const int c4n = C >> 2;
   {
     const RowWalk w = row_walk(tid, blockDim.x, c4n);
@@ -125,16 +161,14 @@ __global__ void __launch_bounds__(256) dscnn_dsblock_kernel(DsLayerDev L, int RH
     }
   };
   load_slice(0, imin(COT, CO));
-  for (int i = tid; i < L.kh * L.kw * C / 4; i += blockDim.x) st4(dws + 4 * i, ldg4(params + L.w + 4 * i));
-  for (int c = tid; c < C; c += blockDim.x) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc1, sf1);
-  for (int c = tid; c < CO; c += blockDim.x) fold_bn(params, L.pb, L.pbeta, L.pmm, L.pmv, c, eps, sc2, sf2);
+  const DsTables T = ds_stage_tables(smem + S.tab, L, L.kh * L.kw, C, CO, params, eps, tid, blockDim.x);
   __syncthreads();
   // depthwise: thread owns 4 channels, walks output positions
   const int npos = rh * L.wout;
   {
     const RowWalk w = row_walk(tid, blockDim.x, c4n);
     if (w.row < npos) {
-      const float4 s = ld4(sc1 + 4 * w.c4), t = ld4(sf1 + 4 * w.c4);
+      const float4 s = ld4(T.sc1 + 4 * w.c4), t = ld4(T.sf1 + 4 * w.c4);
       int oh = w.row / L.wout, ow = w.row - oh * L.wout;
       for (int pos = w.row; pos < npos; pos += w.rstep) {
         const float* xb = xs + ((size_t)(oh * L.sh) * wp + ow * L.sw) * C + 4 * w.c4;
@@ -142,12 +176,10 @@ __global__ void __launch_bounds__(256) dscnn_dsblock_kernel(DsLayerDev L, int RH
         for (int i = 0; i < L.kh; ++i)
           for (int j = 0; j < L.kw; ++j) {
             const float4 x = ld4(xb + ((size_t)i * wp + j) * C);
-            const float4 k = ld4(dws + (i * L.kw + j) * C + 4 * w.c4);
+            const float4 k = ld4(T.taps + (i * L.kw + j) * C + 4 * w.c4);
             acc.x = fmaf(x.x, k.x, acc.x); acc.y = fmaf(x.y, k.y, acc.y); acc.z = fmaf(x.z, k.z, acc.z); acc.w = fmaf(x.w, k.w, acc.w);
           }
-        st4(ds + (size_t)pos * C + 4 * w.c4,
-            make_float4(fmaxf(fmaf(acc.x, s.x, t.x), 0.f), fmaxf(fmaf(acc.y, s.y, t.y), 0.f),
-                        fmaxf(fmaf(acc.z, s.z, t.z), 0.f), fmaxf(fmaf(acc.w, s.w, t.w), 0.f)));
+        st4(ds + (size_t)pos * C + 4 * w.c4, bn_relu4(acc, s, t));
         ow += w.rstep;
         while (ow >= L.wout) { ow -= L.wout; ++oh; }
       }
@@ -185,14 +217,11 @@ __global__ void __launch_bounds__(256) dscnn_dsblock_kernel(DsLayerDev L, int RH
           acc[i].x = fmaf(x.w, w3.x, acc[i].x); acc[i].y = fmaf(x.w, w3.y, acc[i].y); acc[i].z = fmaf(x.w, w3.z, acc[i].z); acc[i].w = fmaf(x.w, w3.w, acc[i].w);
         }
       }
-      const float4 s = ld4(sc2 + co0 + 4 * cg), t = ld4(sf2 + co0 + 4 * cg);
+      const float4 s = ld4(T.sc2 + co0 + 4 * cg), t = ld4(T.sf2 + co0 + 4 * cg);
 #pragma unroll
       for (int i = 0; i < kDsTM; ++i) {
         const int pos = rt + i * NRT;
-        if (pos < npos)
-          st4(out + (gbase + pos) * CO + co0 + 4 * cg,
-              make_float4(fmaxf(fmaf(acc[i].x, s.x, t.x), 0.f), fmaxf(fmaf(acc[i].y, s.y, t.y), 0.f),
-                          fmaxf(fmaf(acc[i].z, s.z, t.z), 0.f), fmaxf(fmaf(acc[i].w, s.w, t.w), 0.f)));
+        if (pos < npos) st4(out + (gbase + pos) * CO + co0 + 4 * cg, bn_relu4(acc[i], s, t));
       }
     }
   }
@@ -270,9 +299,9 @@ __device__ __forceinline__ void gmma_epilogue(const float (&acc)[NA][4 * NJ], in
     }
   }
 }
+__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xFFFFE000u); }
 __device__ __forceinline__ void tf32_split(float4 v, float4& hi, float4& lo) {
-  hi = make_float4(__uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u),
-                   __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u), __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u));
+  hi = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
   lo = make_float4(v.x - hi.x, v.y - hi.y, v.z - hi.z, v.w - hi.w);
 }
 
@@ -281,67 +310,240 @@ __device__ __forceinline__ void cp_async16_zfill(float* dst_smem, const float* s
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst_smem)), "l"(src), "r"(bytes) : "memory");
 }
 
-// Persistent: a CTA keeps the split filter bank and the per-channel tables for all its tiles (tile = RH output rows of one
-// utterance), and the next tile's input rows travel (cp.async) while the current tile is computed.
-// Specialised for the 3x3 / stride-1 depthwise stage (every separable block of DS-CNN-S, audio_nets/ds_cnn.py:20-26):
-//   * depthwise: a thread owns (4 channels, one output column) and slides down the rows, so every input float4 is read once
-//     per thread (3 loads per output instead of 9) and the 9 taps stay in registers;
-//   * the four warpgroups then each issue the 3 * C/8 wgmma (m64, n = CO/2, k8) of one quarter of the accumulator
-//     (rows 64 (g % 2) .., columns (g / 2) CO/2 ..) and drain it from their registers;
-//   * the descriptors are formed once; a k-step only adds its byte offset to the start-address field.
 constexpr int kTcThreads = 512;
-template <int C, int CO>
-__global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
-                                                                  const float* __restrict__ in, float* __restrict__ out, float eps) {
-  static_assert(CO == 64, "one m64n32k8 quarter per warpgroup");
-  TCR_DYNAMIC_SMEM(smem_raw);
-  float* smem = reinterpret_cast<float*>(smem_raw);
-  constexpr int C4 = C / 4, KS = C / 8;
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int hin_t = RH + 2;                                       // 3x3, stride 1
-  const int wp = L.wout + 2;
-  const int XP = hin_t * wp * 4 + 4;                              // floats per channel chunk of the input tile (+16 B against conflicts)
-  constexpr int LBA = 128 * 4 + 4, LBB = CO * 4 + 4;              // K-chunk strides of the A / B operand tiles (floats)
-  float* xs0 = smem;                                              // [2][C4][XP]
-  float* a_hi = xs0 + (size_t)2 * C4 * XP;                        // [C4][LBA]
-  float* a_lo = a_hi + (size_t)C4 * LBA;
-  float* b_hi = a_lo + (size_t)C4 * LBA;                          // [C4][LBB]
-  float* b_lo = b_hi + (size_t)C4 * LBB;
-  float* dws = b_lo + (size_t)C4 * LBB;                           // [9][C]
-  float* sc1 = dws + 9 * C;
-  float* sf1 = sc1 + C;
-  float* sc2 = sf1 + C;
-  float* sf2 = sc2 + CO;
-  const int tpu = (L.hout + RH - 1) / RH;                         // tiles per utterance
-  const int ntiles = tpu * n_utt;
-  // pointwise filters pw[ci][co] -> B operand [n = co][k = ci], hi / lo parts (params are caller-owned: independent of the producer)
-  for (int i0 = tid; i0 < C * CO; i0 += kTcThreads * 8) {
-    float v[8];
+constexpr int kWsProducerWarps = 10, kWsProducers = 32 * kWsProducerWarps, kWsConsumers = 128;
+constexpr int kWsConsumerWarp0 = kTcThreads / 32 - 4;
+constexpr int kLbaFull = 128 * 4 + 4;                             // K-chunk stride (floats) of a 128-row A operand, +16 B
+TCR_HD constexpr int gmma_lbb(int co) { return co * 4 + 4; }     // K-chunk stride of the B operand
+// Per-thread walks worked out once per kernel: dsblock_tc copies kDwCells input cells of its channel chunk per tile; the first
+// conv's im2col walk copies kConvCells 4-byte input cells and gathers kConvTasks (position, tap chunk) operands per thread.
+constexpr int kDwCells = 8, kConvCells = 4, kConvTasks = 4;
+
+// Filter bank w[k][co] (K x CO) -> B operand [n = co][k] in the K-major layout, hi / lo parts; NB loads in flight per thread.
+template <int NT, int CO, int NB>
+__device__ __forceinline__ void stage_b(const float* __restrict__ w, int K, float* b_hi, float* b_lo, int tid) {
+  constexpr int LBB = gmma_lbb(CO);
+  for (int i0 = tid; i0 < K * CO; i0 += NT * NB) {
+    float v[NB];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = i0 + kTcThreads * j < C * CO ? __ldg(params + L.pw + i0 + kTcThreads * j) : 0.f;
+    for (int j = 0; j < NB; ++j) v[j] = i0 + NT * j < K * CO ? __ldg(w + i0 + NT * j) : 0.f;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int i = i0 + kTcThreads * j;
-      if (i < C * CO) {
-        const int ci = i / CO, co = i - ci * CO;
-        const float hi = __uint_as_float(__float_as_uint(v[j]) & 0xFFFFE000u);
-        const int o = (ci >> 2) * LBB + co * 4 + (ci & 3);
+    for (int j = 0; j < NB; ++j) {
+      const int i = i0 + NT * j;
+      if (i < K * CO) {
+        const int k = i / CO, co = i - k * CO;
+        const float hi = tf32_hi(v[j]);
+        const int o = (k >> 2) * LBB + co * 4 + (k & 3);
         b_hi[o] = hi;
         b_lo[o] = v[j] - hi;
       }
     }
   }
-  for (int i = tid; i < 9 * C / 4; i += kTcThreads) st4(dws + 4 * i, ldg4(params + L.w + 4 * i));
-  for (int c = tid; c < C; c += kTcThreads) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc1, sf1);
-  for (int c = tid; c < CO; c += kTcThreads) fold_bn(params, L.pb, L.pbeta, L.pmm, L.pmv, c, eps, sc2, sf2);
+}
+
+// 3x3 / stride-1 depthwise + folded BN + ReLU of one (4-channel chunk, output column), sliding down the rows so that every input
+// float4 is read once (3 loads per output instead of 9) and the 9 taps stay in registers: outputs [rb, re) of the tile.
+// load(r, x) fetches the three taps of input row r; store(m, hi, lo) writes output row m's A operand.
+template <class Load, class Store>
+__device__ __forceinline__ void dw3_slide(int rb, int re, const float4 (&k)[9], float4 s, float4 t, Load load, Store store) {
+  auto tap_row = [&](float4& acc, const float4 (&x)[3], int kr) {
+    acc.x = fmaf(x[0].x, k[3 * kr].x, fmaf(x[1].x, k[3 * kr + 1].x, fmaf(x[2].x, k[3 * kr + 2].x, acc.x)));
+    acc.y = fmaf(x[0].y, k[3 * kr].y, fmaf(x[1].y, k[3 * kr + 1].y, fmaf(x[2].y, k[3 * kr + 2].y, acc.y)));
+    acc.z = fmaf(x[0].z, k[3 * kr].z, fmaf(x[1].z, k[3 * kr + 1].z, fmaf(x[2].z, k[3 * kr + 2].z, acc.z)));
+    acc.w = fmaf(x[0].w, k[3 * kr].w, fmaf(x[1].w, k[3 * kr + 1].w, fmaf(x[2].w, k[3 * kr + 2].w, acc.w)));
+  };
+  float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0, acc2 = acc0;        // outputs r-2, r-1, r while input row r arrives
+  for (int r = rb; r < re + 2; ++r) {
+    float4 x[3];
+    load(r, x);
+    tap_row(acc0, x, 2);                                          // input row r is the bottom tap row of output r-2, the middle
+    tap_row(acc1, x, 1);                                          // of r-1, the top of r
+    tap_row(acc2, x, 0);
+    if (r >= rb + 2) {
+      float4 hi, lo;
+      tf32_split(bn_relu4(acc0, s, t), hi, lo);
+      store(r - 2, hi, lo);
+    }
+    acc0 = acc1; acc1 = acc2; acc2 = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
+// The lock-step kernels' MMA: warpgroup tid / 128 owns one quarter of the 128 x CO accumulator (rows m0 .., columns col0 ..),
+// issues the 3 * KS wgmma m64n(CO/2)k8 of a tile on the A operand (stride kLbaFull) and drains it from its registers.  The
+// descriptors are formed once; a k-step only adds its byte offset to the start-address field.
+template <int CO>
+struct TcQuarter {
+  int m0, col0;
+  uint64_t da_hi, da_lo, db_hi, db_lo;
+  __device__ __forceinline__ TcQuarter(int tid, const float* a_hi, const float* a_lo, const float* b_hi, const float* b_lo) {
+    static_assert(CO == 64, "one m64n32k8 quarter per warpgroup");
+    const int g = tid >> 7;
+    m0 = 64 * (g & 1);
+    col0 = (g >> 1) * (CO / 2);
+    da_hi = gmma_desc(smem_u32(a_hi + 4 * m0), kLbaFull * 4u, 128u);
+    da_lo = gmma_desc(smem_u32(a_lo + 4 * m0), kLbaFull * 4u, 128u);
+    db_hi = gmma_desc(smem_u32(b_hi + 4 * col0), gmma_lbb(CO) * 4u, 128u);
+    db_lo = gmma_desc(smem_u32(b_lo + 4 * col0), gmma_lbb(CO) * 4u, 128u);
+  }
+  __device__ __forceinline__ void run(int KS, int npos, const float* sc, const float* sf, float* __restrict__ out, size_t gbase,
+                                      int wtid) const {
+    float acc[1][CO / 8 * 2];
+#pragma unroll
+    for (int i = 0; i < CO / 4; ++i) acc[0][i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int pass = 0; pass < 3; ++pass) {                       // lo*hi, hi*lo, hi*hi: the small terms first
+      const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
+#pragma unroll
+      for (int ks = 0; ks < KS; ++ks)                            // one MMA covers K = 8 = two 4-wide chunks
+        wgmma_m64n32k8_tf32(acc[0], da0 + (uint64_t)((2 * ks * kLbaFull * 4) >> 4), db0 + (uint64_t)((2 * ks * gmma_lbb(CO) * 4) >> 4));
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    gmma_epilogue<1, CO / 16>(acc, m0, col0, CO, npos, sc, sf, out, gbase, wtid);
+  }
+};
+
+// The first conv's im2col walk for a CTA of NT threads striding it: the input cells a thread copies (4-byte cp.async, zero-filled
+// halo) and the (position, 4-wide tap chunk) operands A[m][k] = x[oh*sh + k / kw][ow*sw + k % kw] it gathers are the same for
+// every tile, so the walk is worked out once (host side: im2col_walk_fits).
+TCR_HD inline bool im2col_walk_fits(const DsLayerDev& L, int RH, int NT) {
+  return ds_in_rows(L, RH) * ds_in_cols(L) <= kConvCells * NT && 128 * (L.kh * L.kw / 4) <= kConvTasks * NT && ds_in_rows(L, RH) < 512;
+}
+template <int NT>
+struct Im2colWalk {
+  int tid, cells, tasks;
+  int f_pk[kConvCells];                                           // position offset + pl | tile row | column valid
+  int g_x01[kConvTasks], g_x23[kConvTasks], g_a[kConvTasks];      // tile offsets of the four taps of a chunk (16 bits each), A offset | row
+  __device__ __forceinline__ Im2colWalk(const DsLayerDev& L, int RH, int tid_) : tid(tid_) {
+    const int wp = ds_in_cols(L);
+    cells = ds_in_rows(L, RH) * wp;
+    tasks = 128 * (L.kh * L.kw >> 2);
+#pragma unroll
+    for (int j = 0; j < kConvCells; ++j) {
+      const int i = tid + j * NT, r = i / wp, col = i - r * wp, x = col - L.pl;
+      f_pk[j] = ((r * L.win + x + L.pl) << 10) | (r << 1) | ((i < cells && x >= 0 && x < L.win) ? 1 : 0);
+    }
+#pragma unroll
+    for (int j = 0; j < kConvTasks; ++j) {
+      const int task = tid + j * NT, m = task & 127, kc = task >> 7;
+      const int oh = m / L.wout, ow = m - oh * L.wout;
+      int e[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int k = 4 * kc + q, ki = k / L.kw, kj = k - ki * L.kw;
+        e[q] = (oh * L.sh + ki) * wp + ow * L.sw + kj;
+      }
+      g_x01[j] = e[0] | (e[1] << 16);
+      g_x23[j] = e[2] | (e[3] << 16);
+      g_a[j] = ((kc * kLbaFull + 4 * m) << 7) | m;
+    }
+  }
+  // input rows of the tile starting at output row h0 of utterance n -> xs [hin_t][wp]
+  __device__ __forceinline__ void fetch(const DsLayerDev& L, const float* in, int n, int h0, float* xs) const {
+    const int hb = h0 * L.sh - L.pt;
+    const float* base = in + ((int64_t)n * L.hin + hb) * L.win - L.pl;
+#pragma unroll
+    for (int j = 0; j < kConvCells; ++j) {
+      if (tid + j * NT < cells) {
+        const int pk = f_pk[j], h = hb + ((pk >> 1) & 0x1FF);
+        const bool ok = (pk & 1) && h >= 0 && h < L.hin;
+        const uint32_t bytes = ok ? 4u : 0u;
+        const float* src = ok ? base + (pk >> 10) : in;
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(xs + tid + j * NT)), "l"(src), "r"(bytes) : "memory");
+      }
+    }
+  }
+  // A operand (hi / lo) of a tile of npos positions; rows past npos are zero
+  __device__ __forceinline__ void gather(const float* xs, int npos, float* a_hi, float* a_lo) const {
+#pragma unroll
+    for (int j = 0; j < kConvTasks; ++j) {
+      if (tid + j * NT < tasks) {
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if ((g_a[j] & 127) < npos) v = make_float4(xs[g_x01[j] & 0xFFFF], xs[g_x01[j] >> 16], xs[g_x23[j] & 0xFFFF], xs[g_x23[j] >> 16]);
+        float4 hi, lo;
+        tf32_split(v, hi, lo);
+        st4(a_hi + (g_a[j] >> 7), hi);
+        st4(a_lo + (g_a[j] >> 7), lo);
+      }
+    }
+  }
+};
+
+// dscnn_dsblock_tc: x [2][C4][xs] (channel-chunk-major input tiles, +16 B per chunk against conflicts), a [hi, lo][C4][kLbaFull],
+// b [hi, lo][C4][gmma_lbb], tab
+template <int C, int CO>
+TCR_HD inline DsSmem dsblock_tc_smem(const DsLayerDev& L, int RH) {
+  constexpr int C4 = C / 4;
+  DsSmem s = {};
+  s.xs = (RH + 2) * (L.wout + 2) * 4 + 4;
+  s.lba = kLbaFull;
+  s.a = 2 * (size_t)C4 * s.xs;
+  s.b = s.a + 2 * (size_t)C4 * s.lba;
+  s.tab = s.b + 2 * (size_t)C4 * gmma_lbb(CO);
+  s.floats = s.tab + ds_tab_floats(9, C, CO);
+  return s;
+}
+// dscnn_dsblock_ws: x [2 buffers][2 channel halves][xs] (TMA destination, xs a multiple of the 1024-byte swizzle atom), a [2][hi,
+// lo][C4][lba] (A rows packed to the tile's rows, rounded to 8, +16 B), b [hi, lo][C4][gmma_lbb] (b_hi also absorbs the last A
+// chunk's over-read), tab
+template <int C, int CO>
+TCR_HD inline DsSmem dsblock_ws_smem(const DsLayerDev& L, int RH) {
+  constexpr int C4 = C / 4;
+  DsSmem s = {};
+  s.xs = (((RH + 2) * (L.wout + 2) * (C / 2) * 4 + 1023) & ~1023) / 4;
+  s.lba = ((RH * L.wout + 7) & ~7) * 4 + 4;
+  s.a = 4 * (size_t)s.xs;
+  s.b = s.a + 4 * (size_t)C4 * s.lba;
+  s.tab = s.b + 2 * (size_t)C4 * gmma_lbb(CO);
+  s.floats = s.tab + ds_tab_floats(9, C, CO);
+  return s;
+}
+// dscnn_conv_tc (nbuf 1) and dscnn_conv_ws (nbuf 2): a [nbuf][hi, lo][K4][kLbaFull], b [hi, lo][K4][gmma_lbb], tab sc, sf [CO],
+// x [2][xs] (input rows [hin_t][wp], rounded to 4)
+template <int CO>
+TCR_HD inline DsSmem conv_tc_smem(const DsLayerDev& L, int RH, int nbuf) {
+  const int K4 = L.kh * L.kw / 4;
+  DsSmem s = {};
+  s.xs = (ds_in_rows(L, RH) * ds_in_cols(L) + 3) & ~3;
+  s.lba = kLbaFull;
+  s.b = 2 * (size_t)nbuf * K4 * s.lba;
+  s.tab = s.b + 2 * (size_t)K4 * gmma_lbb(CO);
+  s.x = s.tab + 2 * CO;
+  s.floats = s.x + 2 * (size_t)s.xs;
+  return s;
+}
+
+// Persistent: a CTA keeps the split filter bank and the per-channel tables for all its tiles (tile = RH output rows of one
+// utterance), and the next tile's input rows travel (cp.async) while the current tile is computed.
+// Specialised for the 3x3 / stride-1 depthwise stage (every separable block of DS-CNN-S, audio_nets/ds_cnn.py:20-26):
+//   * depthwise (dw3_slide): a thread owns (4 channels, one output column) and slides down the rows of the tile;
+//   * the four warpgroups then each issue the MMAs of one quarter of the accumulator and drain it (TcQuarter).
+template <int C, int CO>
+__global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
+                                                                  const float* __restrict__ in, float* __restrict__ out, float eps) {
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* smem = reinterpret_cast<float*>(smem_raw);
+  constexpr int C4 = C / 4;
+  const int tid = threadIdx.x;
+  const int hin_t = RH + 2, wp = L.wout + 2;                      // 3x3, stride 1
+  const DsSmem S = dsblock_tc_smem<C, CO>(L, RH);
+  const int XP = S.xs;                                            // floats per channel chunk of an input tile
+  float *xs0 = smem, *a_hi = smem + S.a, *a_lo = a_hi + (size_t)C4 * kLbaFull;
+  float *b_hi = smem + S.b, *b_lo = b_hi + (size_t)C4 * gmma_lbb(CO);
+  const int tpu = ds_tiles_per_utt(L, RH);
+  const int ntiles = tpu * n_utt;
+  // pointwise filters pw[ci][co] -> B operand (params are caller-owned: independent of the producer)
+  stage_b<kTcThreads, CO, 8>(params + L.pw, C, b_hi, b_lo, tid);
+  const DsTables T = ds_stage_tables(smem + S.tab, L, 9, C, CO, params, eps, tid, kTcThreads);
   pdl_wait();
   // input rows (+halo) of a tile, channel-chunk-major, asynchronously.  A thread copies the same (row, column) cells of every
   // tile (cell = tid / C4 + j * (threads / C4)), so the walk is worked out once: cell -> (tile row, column validity, element offset).
-  constexpr int kCells = 8, kRowStep = kTcThreads / C4;
+  constexpr int kRowStep = kTcThreads / C4;
   const int f_c4 = tid % C4, f_row0 = tid / C4, f_rows = hin_t * wp;
-  int f_pk[kCells];
+  int f_pk[kDwCells];
 #pragma unroll
-  for (int j = 0; j < kCells; ++j) {
+  for (int j = 0; j < kDwCells; ++j) {
     const int row = f_row0 + j * kRowStep;
     const int r = row / wp, col = row - r * wp, x = col - 1;
     const int okx = (row < f_rows && x >= 0 && x < L.win) ? 1 : 0;
@@ -352,7 +554,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
     const float* base = in + (((int64_t)n * L.hin + (h0 - 1)) * L.win - 1) * C + 4 * f_c4;      // never dereferenced out of range
     float* dst = xs + (size_t)f_c4 * XP + 4 * f_row0;
 #pragma unroll
-    for (int j = 0; j < kCells; ++j) {
+    for (int j = 0; j < kDwCells; ++j) {
       if (f_row0 + j * kRowStep < f_rows) {
         const int pk = f_pk[j], h = h0 - 1 + ((pk >> 1) & 0xFF);
         const bool ok = (pk & 1) && h >= 0 && h < L.hin;
@@ -360,10 +562,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
       }
     }
   };
-  // this warpgroup's quarter of the accumulator
-  const int g = warp >> 2, m0 = 64 * (g & 1), col0 = (g >> 1) * (CO / 2);
-  const uint64_t da_hi = gmma_desc(smem_u32(a_hi + 4 * m0), LBA * 4u, 128u), da_lo = gmma_desc(smem_u32(a_lo + 4 * m0), LBA * 4u, 128u);
-  const uint64_t db_hi = gmma_desc(smem_u32(b_hi + 4 * col0), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo + 4 * col0), LBB * 4u, 128u);
+  const TcQuarter<CO> q(tid, a_hi, a_lo, b_hi, b_lo);
   int tile = blockIdx.x, cur = 0;
   if (tile < ntiles) fetch_tile(tile, xs0);
   for (; tile < ntiles; tile += gridDim.x, cur ^= 1) {
@@ -384,49 +583,22 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
       if (rb >= re) continue;
       float4 k[9];
 #pragma unroll
-      for (int j = 0; j < 9; ++j) k[j] = ld4(dws + j * C + 4 * c4);
-      const float4 s = ld4(sc1 + 4 * c4), t = ld4(sf1 + 4 * c4);
+      for (int j = 0; j < 9; ++j) k[j] = ld4(T.taps + j * C + 4 * c4);
       const float* xb = xs + (size_t)c4 * XP + 4 * ow;
-      float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0, acc2 = acc0;      // outputs r-2, r-1, r while input row r arrives
-      for (int r = rb; r < re + 2; ++r) {
-        const float4 x0 = ld4(xb + 4 * (r * wp)), x1 = ld4(xb + 4 * (r * wp + 1)), x2 = ld4(xb + 4 * (r * wp + 2));
-#define TCR_DW3(acc, kr)                                                                                                                   \
-  acc.x = fmaf(x0.x, k[3 * (kr)].x, fmaf(x1.x, k[3 * (kr) + 1].x, fmaf(x2.x, k[3 * (kr) + 2].x, acc.x)));                                  \
-  acc.y = fmaf(x0.y, k[3 * (kr)].y, fmaf(x1.y, k[3 * (kr) + 1].y, fmaf(x2.y, k[3 * (kr) + 2].y, acc.y)));                                  \
-  acc.z = fmaf(x0.z, k[3 * (kr)].z, fmaf(x1.z, k[3 * (kr) + 1].z, fmaf(x2.z, k[3 * (kr) + 2].z, acc.z)));                                  \
-  acc.w = fmaf(x0.w, k[3 * (kr)].w, fmaf(x1.w, k[3 * (kr) + 1].w, fmaf(x2.w, k[3 * (kr) + 2].w, acc.w)));
-        TCR_DW3(acc0, 2)              // input row r is the bottom tap row of output r-2, the middle of r-1, the top of r
-        TCR_DW3(acc1, 1)
-        TCR_DW3(acc2, 0)
-#undef TCR_DW3
-        if (r >= rb + 2) {
-          float4 hi, lo;
-          tf32_split(make_float4(fmaxf(fmaf(acc0.x, s.x, t.x), 0.f), fmaxf(fmaf(acc0.y, s.y, t.y), 0.f), fmaxf(fmaf(acc0.z, s.z, t.z), 0.f),
-                                 fmaxf(fmaf(acc0.w, s.w, t.w), 0.f)), hi, lo);
-          const int m = (r - 2) * L.wout + ow;
-          st4(a_hi + (size_t)c4 * LBA + 4 * m, hi);
-          st4(a_lo + (size_t)c4 * LBA + 4 * m, lo);
-        }
-        acc0 = acc1; acc1 = acc2; acc2 = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
+      dw3_slide(
+          rb, re, k, ld4(T.sc1 + 4 * c4), ld4(T.sf1 + 4 * c4),
+          [&](int r, float4(&x)[3]) {
+            x[0] = ld4(xb + 4 * (r * wp)); x[1] = ld4(xb + 4 * (r * wp + 1)); x[2] = ld4(xb + 4 * (r * wp + 2));
+          },
+          [&](int m, float4 hi, float4 lo) {
+            st4(a_hi + (size_t)c4 * kLbaFull + 4 * (m * L.wout + ow), hi);
+            st4(a_lo + (size_t)c4 * kLbaFull + 4 * (m * L.wout + ow), lo);
+          });
     }
     // accumulator rows past rh * wout are never stored, whatever the A rows there hold (each output row depends on its own A row only)
     fence_proxy_async();                                         // generic-proxy stores of the operands -> visible to the async proxy
     __syncthreads();
-    float acc[1][CO / 8 * 2];
-#pragma unroll
-    for (int i = 0; i < CO / 4; ++i) acc[0][i] = 0.f;
-    wgmma_fence();
-#pragma unroll
-    for (int pass = 0; pass < 3; ++pass) {                       // lo*hi, hi*lo, hi*hi: the small terms first
-      const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
-#pragma unroll
-      for (int ks = 0; ks < KS; ++ks)                            // one MMA covers K = 8 = two 4-wide chunks
-        wgmma_m64n32k8_tf32(acc[0], da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db0 + (uint64_t)((2 * ks * LBB * 4) >> 4));
-    }
-    wgmma_commit();
-    wgmma_wait_all();
-    gmma_epilogue<1, CO / 16>(acc, m0, col0, CO, rh * L.wout, sc2, sf2, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
+    q.run(C / 8, rh * L.wout, T.sc2, T.sf2, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
   }
 }
 
@@ -439,8 +611,6 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_tc_kernel(DsLayer
 // Barriers (index = tile parity): in_full (TMA complete_tx), a_full (producers), mma_done (the consumer warpgroup, once its
 // MMAs have completed: the A buffer may be refilled).  A rows are packed to the tile's own row count (rounded to 8): the
 // 128-row MMA then reads a few rows of the next K chunk as rows >= npos, whose accumulator rows are never stored.
-constexpr int kWsProducerWarps = 10, kWsProducers = 32 * kWsProducerWarps, kWsConsumers = 128;
-constexpr int kWsConsumerWarp0 = kTcThreads / 32 - 4;
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -455,7 +625,7 @@ __device__ __forceinline__ void ws_consumer_role(const DsLayerDev& L, int RH, in
                                                  const float* b_hi, const float* b_lo, const float* sc, const float* sf,
                                                  float* __restrict__ out, uint64_t* a_full, uint64_t* mma_done, int wtid) {
   static_assert(CO == 64, "one m64n64k8 per 64 accumulator rows");
-  constexpr int LBB = CO * 4 + 4;
+  constexpr int LBB = gmma_lbb(CO);
   const uint64_t db_hi = gmma_desc(smem_u32(b_hi), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo), LBB * 4u, 128u);
   const int KS = K4 >> 1;
   int it = 0;
@@ -498,19 +668,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
   const int hin_t = RH + 2, wp = L.wout + 2;
   constexpr int CH = C / 2, CH4 = CH / 4;                         // channels per TMA box: 32 fp32 = one 128-byte swizzle row
   static_assert(CH * 4 == 128, "the input halves are 128-byte rows (SWIZZLE_128B)");
-  const int XH = ((hin_t * wp * CH * 4 + 1023) & ~1023) / 4;      // floats per half tile, a multiple of the 1024-byte swizzle atom
-  const int LBA = ((RH * L.wout + 7) & ~7) * 4 + 4;               // K-chunk stride of the A tiles (floats): the tile's rows, +16 B
-  constexpr int LBB = CO * 4 + 4;
-  float* xs0 = smem;                                              // [2 buffers][2 channel halves][XH], TMA destination (1024-aligned)
-  float* a0 = xs0 + (size_t)4 * XH;                               // [2][hi, lo][C4][LBA]
-  float* b_hi = a0 + (size_t)4 * C4 * LBA;                        // [C4][LBB]  (also absorbs the last A chunk's over-read)
-  float* b_lo = b_hi + (size_t)C4 * LBB;
-  float* dws = b_lo + (size_t)C4 * LBB;                           // [9][C]
-  float* sc1 = dws + 9 * C;
-  float* sf1 = sc1 + C;
-  float* sc2 = sf1 + C;
-  float* sf2 = sc2 + CO;
-  const int tpu = (L.hout + RH - 1) / RH;
+  const DsSmem S = dsblock_ws_smem<C, CO>(L, RH);
+  const int XH = S.xs, LBA = S.lba;                               // floats per half input tile; K-chunk stride of the A tiles
+  float *xs0 = smem, *a0 = smem + S.a, *b_hi = smem + S.b, *b_lo = b_hi + (size_t)C4 * gmma_lbb(CO);
+  const int tpu = ds_tiles_per_utt(L, RH);
   const int ntiles = tpu * n_utt;
   if (tid == 0) {
     for (int b = 0; b < 2; ++b) {
@@ -519,25 +680,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
       mbar_init(&mma_done[b], kWsConsumers);
     }
   }
-  for (int i0 = tid; i0 < C * CO; i0 += kTcThreads * 8) {
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = i0 + kTcThreads * j < C * CO ? __ldg(params + L.pw + i0 + kTcThreads * j) : 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int i = i0 + kTcThreads * j;
-      if (i < C * CO) {
-        const int ci = i / CO, co = i - ci * CO;
-        const float hi = __uint_as_float(__float_as_uint(v[j]) & 0xFFFFE000u);
-        const int o = (ci >> 2) * LBB + co * 4 + (ci & 3);
-        b_hi[o] = hi;
-        b_lo[o] = v[j] - hi;
-      }
-    }
-  }
-  for (int i = tid; i < 9 * C / 4; i += kTcThreads) st4(dws + 4 * i, ldg4(params + L.w + 4 * i));
-  for (int c = tid; c < C; c += kTcThreads) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc1, sf1);
-  for (int c = tid; c < CO; c += kTcThreads) fold_bn(params, L.pb, L.pbeta, L.pmm, L.pmv, c, eps, sc2, sf2);
+  stage_b<kTcThreads, CO, 8>(params + L.pw, C, b_hi, b_lo, tid);
+  const DsTables T = ds_stage_tables(smem + S.tab, L, 9, C, CO, params, eps, tid, kTcThreads);
   pdl_wait();
   fence_proxy_async();                                           // the B operand was written through the generic proxy
   __syncthreads();
@@ -571,8 +715,8 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
     const int half = c4 / CH4, cl = c4 - half * CH4;
     float4 kk[9];
 #pragma unroll
-    for (int j = 0; j < 9; ++j) kk[j] = ld4(dws + j * C + 4 * c4);
-    const float4 s = ld4(sc1 + 4 * c4), t = ld4(sf1 + 4 * c4);
+    for (int j = 0; j < 9; ++j) kk[j] = ld4(T.taps + j * C + 4 * c4);
+    const float4 s = ld4(T.sc1 + 4 * c4), t = ld4(T.sf1 + 4 * c4);
     int it = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
       const int b = it & 1, k = it >> 1;
@@ -586,29 +730,17 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
         const float* xh = xs + (size_t)half * XH;
         float* ah = a_hi + (size_t)c4 * LBA + 4 * ow;
         float* al = a_lo + (size_t)c4 * LBA + 4 * ow;
-        float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0, acc2 = acc0;    // outputs r-2, r-1, r while input row r arrives
-        int p = ow;                                               // position (tile row r, column ow) of the padded tile
-        for (int r = 0; r < rh + 2; ++r, p += wp) {
-          const float4 x0 = ld4(xh + p * CH + (((cl ^ p) & 7) << 2)), x1 = ld4(xh + (p + 1) * CH + (((cl ^ (p + 1)) & 7) << 2)),
-                       x2 = ld4(xh + (p + 2) * CH + (((cl ^ (p + 2)) & 7) << 2));
-#define TCR_DW3(acc, kr)                                                                                                                   \
-  acc.x = fmaf(x0.x, kk[3 * (kr)].x, fmaf(x1.x, kk[3 * (kr) + 1].x, fmaf(x2.x, kk[3 * (kr) + 2].x, acc.x)));                               \
-  acc.y = fmaf(x0.y, kk[3 * (kr)].y, fmaf(x1.y, kk[3 * (kr) + 1].y, fmaf(x2.y, kk[3 * (kr) + 2].y, acc.y)));                               \
-  acc.z = fmaf(x0.z, kk[3 * (kr)].z, fmaf(x1.z, kk[3 * (kr) + 1].z, fmaf(x2.z, kk[3 * (kr) + 2].z, acc.z)));                               \
-  acc.w = fmaf(x0.w, kk[3 * (kr)].w, fmaf(x1.w, kk[3 * (kr) + 1].w, fmaf(x2.w, kk[3 * (kr) + 2].w, acc.w)));
-          TCR_DW3(acc0, 2)            // input row r is the bottom tap row of output r-2, the middle of r-1, the top of r
-          TCR_DW3(acc1, 1)
-          TCR_DW3(acc2, 0)
-#undef TCR_DW3
-          if (r >= 2) {
-            float4 hi, lo;
-            tf32_split(make_float4(fmaxf(fmaf(acc0.x, s.x, t.x), 0.f), fmaxf(fmaf(acc0.y, s.y, t.y), 0.f),
-                                   fmaxf(fmaf(acc0.z, s.z, t.z), 0.f), fmaxf(fmaf(acc0.w, s.w, t.w), 0.f)), hi, lo);
-            st4(ah + 4 * (r - 2) * L.wout, hi);
-            st4(al + 4 * (r - 2) * L.wout, lo);
-          }
-          acc0 = acc1; acc1 = acc2; acc2 = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
+        dw3_slide(
+            0, rh, kk, s, t,
+            [&](int r, float4(&x)[3]) {
+              const int p = ow + r * wp;                          // position (tile row r, column ow) of the padded tile
+#pragma unroll
+              for (int j = 0; j < 3; ++j) x[j] = ld4(xh + (p + j) * CH + (((cl ^ (p + j)) & 7) << 2));
+            },
+            [&](int m, float4 hi, float4 lo) {
+              st4(ah + 4 * m * L.wout, hi);
+              st4(al + 4 * m * L.wout, lo);
+            });
       }
       fence_proxy_async();                                       // operand stores -> visible to the async proxy (wgmma)
       mbar_arrive(&a_full[b]);
@@ -619,13 +751,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
       }
     }
   } else if (warp >= kWsConsumerWarp0) {
-    ws_consumer_role<CO>(L, RH, tpu, ntiles, C4, LBA, a0, b_hi, b_lo, sc2, sf2, out, a_full, mma_done, tid - 32 * kWsConsumerWarp0);
+    ws_consumer_role<CO>(L, RH, tpu, ntiles, C4, LBA, a0, b_hi, b_lo, T.sc2, T.sf2, out, a_full, mma_done, tid - 32 * kWsConsumerWarp0);
   }
 }
 
-// First conv, warp-specialised (same roles and barriers as the block kernel): the producers copy the tile's input rows
-// (cp.async, 4-byte cells, zero-filled halo), gather the im2col operand A[m][k] = x[oh*sh + k / kw][ow*sw + k % kw] (hi / lo) into
-// the A buffer of the tile, and refill the input buffer for the tile two ahead; K = kh * kw (40).
+// First conv, warp-specialised (same roles and barriers as the block kernel): the producers copy the tile's input rows and
+// gather its im2col operand (Im2colWalk) into the A buffer of the tile, and refill the input buffer for the tile two ahead;
+// K = kh * kw (40).
 template <int CO>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
                                                                       const float* __restrict__ in, float* __restrict__ out, float eps) {
@@ -634,16 +766,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
   float* smem = reinterpret_cast<float*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5;
   const int K = L.kh * L.kw, K4 = K >> 2;
-  const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
-  const int XT = (hin_t * wp + 3) & ~3;
-  constexpr int LBA = 128 * 4 + 4, LBB = CO * 4 + 4;
-  float* a0 = smem;                                               // [2][hi, lo][K4][LBA]
-  float* b_hi = a0 + (size_t)4 * K4 * LBA;                        // [K4][LBB]
-  float* b_lo = b_hi + (size_t)K4 * LBB;
-  float* sc = b_lo + (size_t)K4 * LBB;
-  float* sf = sc + CO;
-  float* xs0 = sf + CO;                                           // [2][hin_t][wp]
-  const int tpu = (L.hout + RH - 1) / RH;
+  const DsSmem S = conv_tc_smem<CO>(L, RH, 2);
+  float *a0 = smem, *b_hi = smem + S.b, *b_lo = b_hi + (size_t)K4 * gmma_lbb(CO);
+  float *sc = smem + S.tab, *sf = sc + CO, *xs0 = smem + S.x;
+  const int tpu = ds_tiles_per_utt(L, RH);
   const int ntiles = tpu * n_utt;
   if (tid == 0) {
     for (int b = 0; b < 2; ++b) {
@@ -652,207 +778,84 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
       mbar_init(&mma_done[b], kWsConsumers);
     }
   }
-  for (int i = tid; i < K * CO; i += kTcThreads) {                // filters w[k][co] -> B operand [n = co][k]
-    const int k = i / CO, co = i - k * CO;
-    const float x = __ldg(params + L.w + i);
-    const float hi = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
-    const int o = (k >> 2) * LBB + co * 4 + (k & 3);
-    b_hi[o] = hi;
-    b_lo[o] = x - hi;
-  }
+  stage_b<kTcThreads, CO, 1>(params + L.w, K, b_hi, b_lo, tid);
   for (int c = tid; c < CO; c += kTcThreads) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc, sf);
   pdl_wait();
   fence_proxy_async();
   __syncthreads();
 
   if (warp < kWsProducerWarps) {
-    // the cells a thread copies and the (position, tap chunk) operands it gathers are the same for every tile: worked out once
-    constexpr int kCells = 4, kTasks = 4;                         // host side: hin_t * wp <= 4 * producers, 128 * K4 <= 4 * producers
-    int f_pk[kCells];
-#pragma unroll
-    for (int j = 0; j < kCells; ++j) {
-      const int i = tid + j * kWsProducers, r = i / wp, col = i - r * wp, x = col - L.pl;
-      f_pk[j] = ((r * L.win + x + L.pl) << 10) | (r << 1) | ((i < hin_t * wp && x >= 0 && x < L.win) ? 1 : 0);
-    }
-    auto fetch_tile = [&](int tile, float* xs) {
-      const int n = tile / tpu, h0 = (tile - n * tpu) * RH, hb = h0 * L.sh - L.pt;
-      const float* base = in + ((int64_t)n * L.hin + hb) * L.win - L.pl;
-#pragma unroll
-      for (int j = 0; j < kCells; ++j) {
-        if (tid + j * kWsProducers < hin_t * wp) {
-          const int pk = f_pk[j], h = hb + ((pk >> 1) & 0x1FF);
-          const bool ok = (pk & 1) && h >= 0 && h < L.hin;
-          const uint32_t bytes = ok ? 4u : 0u;
-          const float* src = ok ? base + (pk >> 10) : in;
-          asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(xs + tid + j * kWsProducers)), "l"(src), "r"(bytes) : "memory");
-        }
-      }
+    const Im2colWalk<kWsProducers> walk(L, RH, tid);
+    auto fetch_tile = [&](int tile, float* xs, uint64_t* bar) {
+      const int n = tile / tpu;
+      walk.fetch(L, in, n, (tile - n * tpu) * RH, xs);
+      cp_async_mbar_arrive(bar);
     };
-    int g_x01[kTasks], g_x23[kTasks], g_a[kTasks];                // tile offsets of the four taps of a chunk (16 bits each), A offset | row
-#pragma unroll
-    for (int j = 0; j < kTasks; ++j) {
-      const int task = tid + j * kWsProducers, m = task & 127, kc = task >> 7;
-      const int oh = m / L.wout, ow = m - oh * L.wout;
-      int e[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int kq = 4 * kc + q, ki = kq / L.kw, kj = kq - ki * L.kw;
-        e[q] = (oh * L.sh + ki) * wp + ow * L.sw + kj;
-      }
-      g_x01[j] = e[0] | (e[1] << 16);
-      g_x23[j] = e[2] | (e[3] << 16);
-      g_a[j] = ((kc * LBA + 4 * m) << 7) | m;
-    }
     {
       int t0 = blockIdx.x;
-      if (t0 < ntiles) { fetch_tile(t0, xs0); cp_async_mbar_arrive(&in_full[0]); }
+      if (t0 < ntiles) fetch_tile(t0, xs0, &in_full[0]);
       t0 += gridDim.x;
-      if (t0 < ntiles) { fetch_tile(t0, xs0 + XT); cp_async_mbar_arrive(&in_full[1]); }
+      if (t0 < ntiles) fetch_tile(t0, xs0 + S.xs, &in_full[1]);
     }
     int it = 0;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
       const int b = it & 1, k = it >> 1;
       const int h0 = (tile % tpu) * RH, npos = imin(RH, L.hout - h0) * L.wout;
-      float* xs = xs0 + b * XT;
-      float* a_hi = a0 + (size_t)b * 2 * K4 * LBA;
-      float* a_lo = a_hi + (size_t)K4 * LBA;
+      float* xs = xs0 + b * S.xs;
+      float* a_hi = a0 + (size_t)b * 2 * K4 * kLbaFull;
       mbar_wait(&in_full[b], (uint32_t)(k & 1));
       if (it >= 2) mbar_wait(&mma_done[b], (uint32_t)((k - 1) & 1));             // the MMAs of tile it-2 have read this A buffer
-#pragma unroll
-      for (int j = 0; j < kTasks; ++j) {
-        if (tid + j * kWsProducers < 128 * K4) {
-          float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-          if ((g_a[j] & 127) < npos) v = make_float4(xs[g_x01[j] & 0xFFFF], xs[g_x01[j] >> 16], xs[g_x23[j] & 0xFFFF], xs[g_x23[j] >> 16]);
-          float4 hi, lo;
-          tf32_split(v, hi, lo);
-          st4(a_hi + (g_a[j] >> 7), hi);
-          st4(a_lo + (g_a[j] >> 7), lo);
-        }
-      }
+      walk.gather(xs, npos, a_hi, a_hi + (size_t)K4 * kLbaFull);
       fence_proxy_async();
       mbar_arrive(&a_full[b]);
       const int nxt = tile + 2 * (int)gridDim.x;
       if (nxt < ntiles) {
         asm volatile("bar.sync 1, %0;" ::"n"(kWsProducers) : "memory");
-        fetch_tile(nxt, xs);
-        cp_async_mbar_arrive(&in_full[b]);
+        fetch_tile(nxt, xs, &in_full[b]);
       }
     }
   } else if (warp >= kWsConsumerWarp0) {
-    ws_consumer_role<CO>(L, RH, tpu, ntiles, K4, LBA, a0, b_hi, b_lo, sc, sf, out, a_full, mma_done, tid - 32 * kWsConsumerWarp0);
+    ws_consumer_role<CO>(L, RH, tpu, ntiles, K4, kLbaFull, a0, b_hi, b_lo, sc, sf, out, a_full, mma_done, tid - 32 * kWsConsumerWarp0);
   }
 }
 
 // First layer (kh x kw conv from the single-channel feature map, audio_nets/ds_cnn.py:21 `conv_1`) as an implicit GEMM on
-// wgmma: A[m][k] = x[oh*sh + k / kw, ow*sw + k % kw] is gathered from the staged input rows straight into the canonical
-// operand layout (hi / lo), B = the filter bank [co][k], K = kh * kw (40), same persistent / quarter-per-warpgroup structure as
-// the lock-step block kernel above.
+// wgmma: the im2col operand (Im2colWalk) is gathered from the staged input rows straight into the canonical operand layout
+// (hi / lo), B = the filter bank [co][k], K = kh * kw (40), same persistent / quarter-per-warpgroup structure as the lock-step
+// block kernel above.
 template <int CO>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
                                                                       const float* __restrict__ in, float* __restrict__ out, float eps) {
-  static_assert(CO == 64, "one m64n32k8 quarter per warpgroup");
   TCR_DYNAMIC_SMEM(smem_raw);
   float* smem = reinterpret_cast<float*>(smem_raw);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  const int K = L.kh * L.kw, K4 = K >> 2, KS = K >> 3;
-  const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
-  const int XT = (hin_t * wp + 3) & ~3;
-  constexpr int LBA = 128 * 4 + 4, LBB = CO * 4 + 4;
-  float* xs0 = smem;                                              // [2][hin_t][wp]
-  float* a_hi = xs0 + 2 * XT;                                     // [K4][LBA]
-  float* a_lo = a_hi + (size_t)K4 * LBA;
-  float* b_hi = a_lo + (size_t)K4 * LBA;                          // [K4][LBB]
-  float* b_lo = b_hi + (size_t)K4 * LBB;
-  float* sc = b_lo + (size_t)K4 * LBB;
-  float* sf = sc + CO;
-  const int tpu = (L.hout + RH - 1) / RH;
+  const int tid = threadIdx.x;
+  const int K = L.kh * L.kw, K4 = K >> 2;
+  const DsSmem S = conv_tc_smem<CO>(L, RH, 1);
+  float *a_hi = smem, *a_lo = a_hi + (size_t)K4 * kLbaFull, *b_hi = smem + S.b, *b_lo = b_hi + (size_t)K4 * gmma_lbb(CO);
+  float *sc = smem + S.tab, *sf = sc + CO, *xs0 = smem + S.x;
+  const int tpu = ds_tiles_per_utt(L, RH);
   const int ntiles = tpu * n_utt;
-  for (int i = tid; i < K * CO; i += kTcThreads) {                // filters w[k][co] -> B operand [n = co][k]
-    const int k = i / CO, co = i - k * CO;
-    const float x = __ldg(params + L.w + i);
-    const float hi = __uint_as_float(__float_as_uint(x) & 0xFFFFE000u);
-    const int o = (k >> 2) * LBB + co * 4 + (k & 3);
-    b_hi[o] = hi;
-    b_lo[o] = x - hi;
-  }
+  stage_b<kTcThreads, CO, 1>(params + L.w, K, b_hi, b_lo, tid);
   for (int c = tid; c < CO; c += kTcThreads) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc, sf);
   pdl_wait();
-  // The cells a thread copies and the (position, tap chunk) operands it gathers are the same for every tile: worked out once.
-  constexpr int kCells = 4, kTasks = 4;                           // host side: hin_t * wp <= 4 * threads, 128 * K4 <= 4 * threads
-  int f_pk[kCells];
-#pragma unroll
-  for (int j = 0; j < kCells; ++j) {
-    const int i = tid + j * kTcThreads, r = i / wp, col = i - r * wp, x = col - L.pl;
-    f_pk[j] = ((r * L.win + x + L.pl) << 10) | (r << 1) | ((i < hin_t * wp && x >= 0 && x < L.win) ? 1 : 0);
-  }
+  const Im2colWalk<kTcThreads> walk(L, RH, tid);
   auto fetch_tile = [&](int tile, float* xs) {
-    const int n = tile / tpu, h0 = (tile - n * tpu) * RH, hb = h0 * L.sh - L.pt;
-    const float* base = in + ((int64_t)n * L.hin + hb) * L.win - L.pl;
-#pragma unroll
-    for (int j = 0; j < kCells; ++j) {
-      if (tid + j * kTcThreads < hin_t * wp) {
-        const int pk = f_pk[j], h = hb + ((pk >> 1) & 0x1FF);
-        const bool ok = (pk & 1) && h >= 0 && h < L.hin;
-        const uint32_t bytes = ok ? 4u : 0u;
-        const float* src = ok ? base + (pk >> 10) : in;
-        asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(xs + tid + j * kTcThreads)), "l"(src), "r"(bytes) : "memory");
-      }
-    }
+    const int n = tile / tpu;
+    walk.fetch(L, in, n, (tile - n * tpu) * RH, xs);
   };
-  int g_x01[kTasks], g_x23[kTasks], g_a[kTasks];                  // tile offsets of the four taps of a chunk (16 bits each), A offset | row
-#pragma unroll
-  for (int j = 0; j < kTasks; ++j) {
-    const int task = tid + j * kTcThreads, m = task & 127, kc = task >> 7;
-    const int oh = m / L.wout, ow = m - oh * L.wout;
-    int e[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int k = 4 * kc + q, ki = k / L.kw, kj = k - ki * L.kw;
-      e[q] = (oh * L.sh + ki) * wp + ow * L.sw + kj;
-    }
-    g_x01[j] = e[0] | (e[1] << 16);
-    g_x23[j] = e[2] | (e[3] << 16);
-    g_a[j] = ((kc * LBA + 4 * m) << 7) | m;
-  }
-  // this warpgroup's quarter of the accumulator
-  const int g = warp >> 2, m0 = 64 * (g & 1), col0 = (g >> 1) * (CO / 2);
-  const uint64_t da_hi = gmma_desc(smem_u32(a_hi + 4 * m0), LBA * 4u, 128u), da_lo = gmma_desc(smem_u32(a_lo + 4 * m0), LBA * 4u, 128u);
-  const uint64_t db_hi = gmma_desc(smem_u32(b_hi + 4 * col0), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo + 4 * col0), LBB * 4u, 128u);
+  const TcQuarter<CO> q(tid, a_hi, a_lo, b_hi, b_lo);
   int tile = blockIdx.x, cur = 0;
   if (tile < ntiles) fetch_tile(tile, xs0);
   for (; tile < ntiles; tile += gridDim.x, cur ^= 1) {
-    const int n = tile / tpu, h0 = (tile - n * tpu) * RH, rh = imin(RH, L.hout - h0);
-    const float* xs = xs0 + cur * XT;
+    const int n = tile / tpu, h0 = (tile - n * tpu) * RH, npos = imin(RH, L.hout - h0) * L.wout;
+    const float* xs = xs0 + cur * S.xs;
     asm volatile("cp.async.wait_all;" ::: "memory");
     __syncthreads();                                             // rows landed; the previous tile's MMAs are done with A
-    if (tile + (int)gridDim.x < ntiles) fetch_tile(tile + gridDim.x, xs0 + (cur ^ 1) * XT);
-    // im2col gather: task = (position, 4-wide chunk of taps)
-    const int npos = rh * L.wout;
-#pragma unroll
-    for (int j = 0; j < kTasks; ++j) {
-      if (tid + j * kTcThreads < 128 * K4) {
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if ((g_a[j] & 127) < npos) v = make_float4(xs[g_x01[j] & 0xFFFF], xs[g_x01[j] >> 16], xs[g_x23[j] & 0xFFFF], xs[g_x23[j] >> 16]);
-        float4 hi, lo;
-        tf32_split(v, hi, lo);
-        st4(a_hi + (g_a[j] >> 7), hi);
-        st4(a_lo + (g_a[j] >> 7), lo);
-      }
-    }
+    if (tile + (int)gridDim.x < ntiles) fetch_tile(tile + gridDim.x, xs0 + (cur ^ 1) * S.xs);
+    walk.gather(xs, npos, a_hi, a_lo);
     fence_proxy_async();
     __syncthreads();
-    float acc[1][CO / 8 * 2];
-#pragma unroll
-    for (int i = 0; i < CO / 4; ++i) acc[0][i] = 0.f;
-    wgmma_fence();
-    for (int pass = 0; pass < 3; ++pass) {
-      const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
-      for (int ks = 0; ks < KS; ++ks)
-        wgmma_m64n32k8_tf32(acc[0], da0 + (uint64_t)((2 * ks * LBA * 4) >> 4), db0 + (uint64_t)((2 * ks * LBB * 4) >> 4));
-    }
-    wgmma_commit();
-    wgmma_wait_all();
-    gmma_epilogue<1, CO / 16>(acc, m0, col0, CO, npos, sc, sf, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
+    q.run(K >> 3, npos, sc, sf, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
   }
 }
 #endif
@@ -1080,6 +1083,13 @@ extern "C" int tcr_dscnn_param_table(const tcr_dscnn* d, const tcr_param_desc** 
   return TCR_OK;
 }
 
+// Tile rows of the wgmma kernels: at most 128 accumulator rows (RH * wout) per tile, balanced (25 rows -> 5 tiles of 5).
+static int ds_tile_rows(const DsLayerDev& L) {
+  const int cap = std::max(1, std::min(L.hout, 128 / std::max(1, std::min(L.wout, 128))));
+  const int tiles = (L.hout + cap - 1) / cap;
+  return (L.hout + tiles - 1) / tiles;
+}
+
 // Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC).  The kernel is chosen here, once for both entry
 // points: wgmma where the layer's shape fits the tensor-core kernels (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.
 // The warp-specialised block kernel reads its input through a TMA map over max_batch utterances, so only from an activation
@@ -1089,33 +1099,26 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
   const float eps = 1e-3f;
   if (L.type == 0) {
 #ifndef TCR_EMU
-    int RHt = std::min(L.hout, 128 / std::max(1, std::min(L.wout, 128)));
-    RHt = std::max(1, RHt);
-    RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);
-    const int K4 = L.kh * L.kw / 4, hin_t = (RHt - 1) * L.sh + L.kh, wpt = (L.wout - 1) * L.sw + L.kw;
-    // implicit GEMM on wgmma (3xTF32); the limits are the kernel's precomputed per-thread walks (4 cells, 4 gather tasks)
-    if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && hin_t * wpt <= 4 * kTcThreads &&
-        128 * K4 <= 4 * kTcThreads && hin_t < 512) {
-      const size_t smem_cws = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 4 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
-      if (d->tc_ws && smem_cws <= 220 * 1024 && hin_t * wpt <= 4 * kWsProducers && 128 * K4 <= 4 * kWsProducers && (K4 & 1) == 0) {
+    const int RHt = ds_tile_rows(L), grid = std::min(ds_tiles_per_utt(L, RHt) * n, d->sms);
+    // implicit GEMM on wgmma (3xTF32), where the kernel's per-thread im2col walk covers the tile
+    if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && im2col_walk_fits(L, RHt, kTcThreads)) {
+      const size_t smem_ws = conv_tc_smem<64>(L, RHt, 2).floats * 4;
+      if (d->tc_ws && smem_ws <= 220 * 1024 && im2col_walk_fits(L, RHt, kWsProducers) && (L.kh * L.kw / 4) % 2 == 0) {
         auto kws = dscnn_conv_ws_kernel<64>;
-        static SmemOptIn optin_cws;
-        if (optin_cws.ensure(kws, smem_cws) != cudaSuccess) return TCR_ERR_CUDA;
-        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-        TCR_LAUNCH("dscnn_conv_ws", kws, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_cws, s, L, RHt, n, params, in, out, eps);
+        static SmemOptIn optin_ws;
+        if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
+        TCR_LAUNCH("dscnn_conv_ws", kws, dim3(grid), dim3(kTcThreads), smem_ws, s, L, RHt, n, params, in, out, eps);
         return TCR_OK;
       }
-      const size_t smem_tc = (2 * (size_t)((hin_t * wpt + 3) & ~3) + 2 * (size_t)K4 * (128 * 4 + 4) + 2 * (size_t)K4 * (L.cout * 4 + 4) + 2 * L.cout) * 4;
+      const size_t smem_tc = conv_tc_smem<64>(L, RHt, 1).floats * 4;
       auto ktc = dscnn_conv_tc_kernel<64>;
       static SmemOptIn optin_tc;
       if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-      const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-      TCR_LAUNCH("dscnn_conv_tc", ktc, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
+      TCR_LAUNCH("dscnn_conv_tc", ktc, dim3(grid), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
       return TCR_OK;
     }
 #endif
-    const int hp = (L.hout - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
-    const size_t smem = (size_t)(((hp * wp + 3) & ~3) + L.kh * L.kw * L.cout + 2 * L.cout) * 4;
+    const size_t smem = conv_smem(L).floats * 4;
     auto kfn = dscnn_conv_kernel;
 #ifndef TCR_EMU
     static SmemOptIn optin;
@@ -1123,24 +1126,13 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
 #endif
     TCR_LAUNCH("dscnn_conv", kfn, dim3(n), dim3(256), smem, s, L, params, in, out, eps);
   } else {
-    auto smem_for = [&](int RH, int COT) {
-      const int hin_t = (RH - 1) * L.sh + L.kh, wp = (L.wout - 1) * L.sw + L.kw;
-      return (size_t)((size_t)hin_t * wp * L.cin + (size_t)RH * L.wout * L.cin + (size_t)L.cin * COT + L.kh * L.kw * L.cin +
-                      2 * L.cin + 2 * L.cout) * 4;
-    };
 #ifndef TCR_EMU
     // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
     if (d->use_tc && L.cin == 64 && L.cout == 64 && L.kh == 3 && L.kw == 3 && L.sh == 1 && L.sw == 1 && L.wout <= 64) {
-      int RHt = std::min(L.hout, 128 / L.wout);
-      RHt = (L.hout + ((L.hout + RHt - 1) / RHt) - 1) / ((L.hout + RHt - 1) / RHt);     // balanced: 25 rows -> 5 tiles of 5
-      const int C4 = L.cin / 4;
-      const bool walk_ok = (RHt + 2) * (L.wout + 2) <= 8 * (kTcThreads / C4);      // the kernel's precomputed fetch walk: 8 cells
-      const size_t smem_tc = (2 * (size_t)C4 * ((RHt + 2) * (L.wout + 2) * 4 + 4) + 2 * (size_t)C4 * (128 * 4 + 4) + 2 * (size_t)C4 * (L.cout * 4 + 4) +
-                              (size_t)9 * L.cin + 2 * L.cin + 2 * L.cout) * 4;
-      const int lba = ((RHt * L.wout + 7) & ~7) * 4 + 4;
-      const size_t xh = (((size_t)(RHt + 2) * (L.wout + 2) * 128 + 1023) & ~(size_t)1023) / 4;       // floats per half input tile
-      const size_t smem_ws = (4 * xh + 4 * (size_t)C4 * lba + 2 * (size_t)C4 * (L.cout * 4 + 4) + (size_t)9 * L.cin + 2 * L.cin + 2 * L.cout) * 4;
-      if (d->tc_ws && smem_ws <= 226 * 1024 && C4 * L.wout <= kWsProducers && L.wout + 2 <= 256 && RHt + 2 <= 256 && (in == d->act[0] || in == d->act[1])) {
+      const int RHt = ds_tile_rows(L), grid = std::min(ds_tiles_per_utt(L, RHt) * n, d->sms);
+      const size_t smem_ws = dsblock_ws_smem<64, 64>(L, RHt).floats * 4;
+      if (d->tc_ws && smem_ws <= 226 * 1024 && L.cin / 4 * L.wout <= kWsProducers && L.wout + 2 <= 256 && RHt + 2 <= 256 &&
+          (in == d->act[0] || in == d->act[1])) {
         auto kws = dscnn_dsblock_ws_kernel<64, 64>;
         static SmemOptIn optin_ws;
         if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
@@ -1152,16 +1144,15 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
           im.ptr = in;
           im.rh = RHt;
         }
-        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-        TCR_LAUNCH("dscnn_dsblock_ws", kws, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_ws, s, im.map, L, RHt, n, params, out, eps);
+        TCR_LAUNCH("dscnn_dsblock_ws", kws, dim3(grid), dim3(kTcThreads), smem_ws, s, im.map, L, RHt, n, params, out, eps);
         return TCR_OK;
       }
-      if (smem_tc <= 200 * 1024 && walk_ok) {
+      const size_t smem_tc = dsblock_tc_smem<64, 64>(L, RHt).floats * 4;
+      if (smem_tc <= 200 * 1024 && (RHt + 2) * (L.wout + 2) <= kDwCells * (kTcThreads / (L.cin / 4))) {   // the kernel's fetch walk
         auto ktc = dscnn_dsblock_tc_kernel<64, 64>;
         static SmemOptIn optin_tc;
         if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-        const int tiles = ((L.hout + RHt - 1) / RHt) * n;
-        TCR_LAUNCH("dscnn_dsblock_tc", ktc, dim3(std::min(tiles, d->sms)), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
+        TCR_LAUNCH("dscnn_dsblock_tc", ktc, dim3(grid), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
         return TCR_OK;
       }
     }
@@ -1169,17 +1160,17 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
     // the whole pointwise bank in shared memory when it fits next to a useful tile; else (DS-CNN-L: 276 x 276 fp32 = 305 KB) output-
     // channel tiles of COT, the depthwise output of the tile being reused for every slice
     int COT = L.cout;
-    while (COT > 32 && smem_for(1, COT) > 96 * 1024) COT = ((COT / 2) + 3) & ~3;
+    while (COT > 32 && dsblock_smem(L, 1, COT).floats * 4 > 96 * 1024) COT = ((COT / 2) + 3) & ~3;
     int RH = std::min(L.hout, 8);
-    while (RH > 1 && smem_for(RH, COT) > 100 * 1024) --RH;
-    const size_t smem = smem_for(RH, COT);
+    while (RH > 1 && dsblock_smem(L, RH, COT).floats * 4 > 100 * 1024) --RH;
+    const size_t smem = dsblock_smem(L, RH, COT).floats * 4;
     if (smem > 200 * 1024) { set_error("DS-CNN layer does not fit in shared memory"); return TCR_ERR_UNSUPPORTED; }
     auto kfn = dscnn_dsblock_kernel;
 #ifndef TCR_EMU
     static SmemOptIn optin;
     if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
 #endif
-    TCR_LAUNCH("dscnn_dsblock", kfn, dim3((L.hout + RH - 1) / RH, n), dim3(256), smem, s, L, RH, COT, params, in, out, eps);
+    TCR_LAUNCH("dscnn_dsblock", kfn, dim3(ds_tiles_per_utt(L, RH), n), dim3(256), smem, s, L, RH, COT, params, in, out, eps);
   }
   return TCR_OK;
 }
