@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 9
+#define TCR_ABI_VERSION 10
 
 enum {
   TCR_OK = 0,
@@ -287,6 +287,50 @@ int tcr_forward(tcr_handle* h, const float* input, int32_t input_is_features, co
                 const float* moving, int32_t n, int32_t is_training, uint64_t dropout_seed,
                 const float* dropout_mask, const float* onehot, float weight_decay,
                 float* logits, float* probs, float* losses, tcr_stream stream);
+
+/* Continuous-audio listener (ABI 10): scores S independent audio streams with a sliding window, the job the deploy graph of
+ * factory/audio_nets.py:87-125 is run for, without recomputing a frame of features per window it falls into.
+ *
+ * A listener belongs to one handle and shares its geometry: T frames, window W_s and stride s samples.  Each push hands it
+ * chunk_samples new samples per stream (a multiple of hop_frames * s) and emits exactly K = chunk_samples / (hop_frames * s)
+ * windows per stream.  The result equals an offline computation exactly:
+ *   1. after create or reset, a stream acts as if pre = (T - hop_frames) * s + (W_s - s) zero samples had already been pushed;
+ *   2. window k of a stream (counted from the reset) is made of frames [k * hop_frames, k * hop_frames + T) of that zero-prefixed
+ *      sample sequence, i.e. the clip of clip_samples samples that starts at sample k * hop_frames * s; it ends (k + 1) *
+ *      hop_frames * s samples after the reset;
+ *   3. its logits and softmax equal tcr_forward in evaluation mode (moving BatchNorm statistics, no dropout) on that clip, bit
+ *      for bit: a push computes each new frame once with the front-end kernel tcr_mfcc_forward selects for the handle, and conv0
+ *      reads every window in place from the stream's feature history; the rest is the evaluation forward at n = S * K.
+ * So a stream is just the concatenation of its pushes.
+ *
+ * The listener owns its persistent state (per stream: the last W_s - s samples and the last T - hop_frames feature frames); it
+ * borrows the handle's layer workspace for the forward pass, so a handle and its listeners follow the handle's rule: one stream,
+ * not thread-safe.  Training steps may run on the handle between pushes.  (`tcr_stream` is the cudaStream_t type above.)
+ *
+ * tcr_listener_create  TCR_ERR_INVALID: streams < 1, hop_frames outside [1, T], chunk_samples not a positive multiple of
+ *                      hop_frames * s, streams * K > max_batch.  Every stream starts reset; the call synchronises the device.
+ * tcr_listener_reset   stream: index of the stream to reset, or -1 for all of them (TCR_ERR_INVALID otherwise).
+ * tcr_listener_push    samples: device [S, chunk_samples], fp32 in [-1,1] (TCR_INPUT_WAV_F32) or int16 PCM (TCR_INPUT_WAV_PCM16,
+ *                      decode_wav's 1/32768 scaling, bit-identical to the decoded fp32 samples), 16-byte aligned;
+ *                      logits / probs: device [S, K, num_classes] or NULL.  TCR_ERR_INVALID: a NULL handle / samples / params /
+ *                      moving, another input kind, a misaligned samples pointer.  TCR_ERR_UNSUPPORTED: int16 input with window,
+ *                      stride or chunk lengths that are not multiples of 8 samples (as tcr_forward).
+ * tcr_listener_destroy frees the listener's buffers (NULL is a no-op); destroy listeners before their handle. */
+typedef struct tcr_listener tcr_listener;
+typedef struct tcr_listener_config {
+  int32_t streams;         /* S */
+  int32_t hop_frames;      /* frames between two windows of a stream, in [1, T] */
+  int32_t chunk_samples;   /* samples per stream and push, a multiple of hop_frames * window_stride_samples */
+} tcr_listener_config;
+int tcr_listener_create(tcr_handle* h, const tcr_listener_config* cfg, tcr_listener** out);
+int tcr_listener_reset(tcr_listener* L, int32_t stream, tcr_stream stream_);
+int tcr_listener_push(tcr_listener* L, const void* samples, int32_t input_kind, const float* params, const float* moving,
+                      float* logits, float* probs, tcr_stream stream_);
+int tcr_listener_destroy(tcr_listener* L);
+/* Inspection: device pointer of the feature history [S][*frames][F] (*frames = T - hop_frames + K * hop_frames).  Between calls,
+ * frames [0, T - hop_frames) of each stream are the last T - hop_frames frames of that stream, which the next push's first
+ * window starts with (after a reset: the features of silence). */
+int tcr_listener_history(const tcr_listener* L, float** history, int32_t* frames);
 
 /* The evaluation consumer behind the forward pass, on the device (SURVEY.md 8f row 3): reduces one batch of scores and
  * one-hot labels to the integers every count-based metric of the reference is a function of, instead of shipping

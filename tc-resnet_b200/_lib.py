@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtcr_b200.so")
 
 TCR_MODEL_TCRESNET8 = 8
 TCR_MODEL_TCRESNET14 = 14
-ABI_VERSION = 9        # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
+ABI_VERSION = 10       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
 TCR_INPUT_WAV_F32, TCR_INPUT_FEATURES, TCR_INPUT_WAV_PCM16 = 0, 1, 2
 TCR_OPT_MOMENTUM, TCR_OPT_ADAM, TCR_OPT_RMSPROP = 0, 1, 2
 TCR_FEATURE_MFCC = 0
@@ -77,6 +77,10 @@ class TcrStepArgs(C.Structure):
     ]
 
 
+class TcrListenerConfig(C.Structure):
+    _fields_ = [("streams", C.c_int32), ("hop_frames", C.c_int32), ("chunk_samples", C.c_int32)]
+
+
 class TcrDataset(C.Structure):
     _fields_ = [
         ("samples", C.c_void_p), ("num_samples", C.c_int64), ("clips", C.c_void_p), ("num_clips", C.c_int64),
@@ -105,6 +109,11 @@ SYMBOLS = {
     "tcr_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                               C.c_uint64, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                               C.c_void_p]),
+    "tcr_listener_create": (C.c_int, [C.c_void_p, C.POINTER(TcrListenerConfig), C.POINTER(C.c_void_p)]),
+    "tcr_listener_reset": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    "tcr_listener_push": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tcr_listener_destroy": (C.c_int, [C.c_void_p]),
+    "tcr_listener_history": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int32)]),
     "tcr_eval_accumulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "tcr_comm_set_sync_bn": (C.c_int, [C.c_void_p, C.c_int32]),
     "tcr_train_step": (C.c_int, [C.c_void_p, C.POINTER(TcrStepArgs), C.c_void_p]),

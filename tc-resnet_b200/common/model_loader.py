@@ -58,6 +58,20 @@ def restore_filter(include_scopes: str = "", exclude_scopes: str = "") -> Callab
     return keep
 
 
+def evaluation_restore(args, values: Dict[str, np.ndarray], trainable_names: Callable[[], Sequence[str]]):
+    """(values, restore predicate) for AudioNetModel.set_variables as evaluation restores a checkpoint (helper/evaluator.py, and
+    listen_audio.py): filtered by --checkpoint_{include,exclude}_scopes, or with --use_ema every trainable variable (the names
+    `trainable_names()` returns) taken from its shadow.  --use_ema together with a scope filter is rejected (the reference crashes
+    on it, SURVEY.md section 9)."""
+    include = getattr(args, "checkpoint_include_scopes", "")
+    exclude = getattr(args, "checkpoint_exclude_scopes", "")
+    if getattr(args, "use_ema", False):
+        if split_strip(include) or split_strip(exclude):
+            raise ValueError("--use_ema cannot be combined with --checkpoint_include_scopes / --checkpoint_exclude_scopes")
+        return ema_restore_values(values, trainable_names()), None
+    return values, restore_filter(include, exclude)
+
+
 def ema_restore_values(values: Dict[str, np.ndarray], trainable_names: Sequence[str]) -> Dict[str, np.ndarray]:
     """The checkpoint as the evaluator restores it with --use_ema: each trainable variable takes its shadow's value; one without
     a shadow in the checkpoint is absent (missing unless --ignore_missing_vars, which leaves its initial value)."""

@@ -237,7 +237,7 @@ static int build_frontend_tables(tcr_handle* h) {
   return TCR_OK;
 }
 
-static MfccArgs mfcc_args(const tcr_handle* h, const void* wav, int pcm16, float* feat) {
+MfccArgs tcr::mfcc_args(const tcr_handle* h, const void* wav, int pcm16, float* feat) {
   MfccArgs a;
   a.wav = wav;
   a.pcm16 = pcm16;
@@ -247,6 +247,7 @@ static MfccArgs mfcc_args(const tcr_handle* h, const void* wav, int pcm16, float
   a.stride = h->cfg.window_stride_samples;
   a.frames = h->frames;
   a.features = h->features;
+  a.feat_stride = (int64_t)h->frames * h->features;
   a.mel_bins = h->cfg.num_mel_bins;
   a.fpb = h->fpb;
   a.warps = h->fwarps;
@@ -531,18 +532,20 @@ static int mfcc_run(tcr_handle* h, const void* wav, int pcm16, float* features, 
   if (((uintptr_t)wav & 15) != 0) return fail(TCR_ERR_INVALID, "wav must be 16-byte aligned (TMA bulk copy)");
   if (pcm16 && (h->cfg.window_size_samples % 8 || h->cfg.window_stride_samples % 8 || h->cfg.clip_samples % 8))
     return fail(TCR_ERR_UNSUPPORTED, "int16 input needs window, stride and clip lengths that are multiples of 8 samples");
-  MfccArgs a = mfcc_args(h, wav, pcm16, features);
+  return mfcc_select_launch(h, mfcc_args(h, wav, pcm16, features), n, (cudaStream_t)stream);
+}
+int tcr::mfcc_select_launch(tcr_handle* h, const MfccArgs& a, int n, cudaStream_t stream) {
   bool launched = false;
   if (h->mfcc_pair) {                                             // two frames per warp (tcr_mfcc_pair.cu) where the shape allows
     MfccArgs b = a;
     b.fpb = h->pair_fpb;
     b.warps = h->pair_warps;
     if (mfcc_pair_supported(b, h->fft)) {
-      if (mfcc_pair_launch(b, n, 3 * h->sms, (cudaStream_t)stream) != 0) return fail(TCR_ERR_CUDA, "mfcc (frame pairs) launch configuration failed");
+      if (mfcc_pair_launch(b, n, 3 * h->sms, stream) != 0) return fail(TCR_ERR_CUDA, "mfcc (frame pairs) launch configuration failed");
       launched = true;
     }
   }
-  if (!launched && mfcc_launch(a, n, h->fft, (cudaStream_t)stream) != 0) return fail(TCR_ERR_CUDA, "mfcc launch configuration failed");
+  if (!launched && mfcc_launch(a, n, h->fft, stream) != 0) return fail(TCR_ERR_CUDA, "mfcc launch configuration failed");
   TCR_CUDA(cudaGetLastError());
   return TCR_OK;
 }

@@ -64,6 +64,10 @@ struct FwdArgs {
   // training statistics
   int train;
   float eps;
+  // windowed input (conv_fwd_kernel<K, WSMEM, true>, in_kind 0 only): utterance u is read at in.data + (u / win_k) * win_stream
+  // + (u % win_k) * win_step floats, its T rows of cin floats back to back (a listener's feature history, tcr_listener.cu)
+  int win_k;
+  int64_t win_stream, win_step;
 };
 
 // ---------------- head: residual + pool + dropout + fc + softmax + CE (+ head backward) ----------------

@@ -290,7 +290,7 @@ __global__ void __launch_bounds__(224, (NF2 <= 512) ? 4 : 2) mfcc_kernel(MfccArg
       }
     }
     __syncwarp();
-    float* out = a.feat + ((size_t)utt * a.frames + (f0 + f)) * a.features;
+    float* out = a.feat + (size_t)utt * a.feat_stride + (size_t)(f0 + f) * a.features;
     if (a.use_dct) {
       // DCT: lane (q, g) = (lane / 8, lane % 8) sums mel bins m = q, q + 4, ... for coefficients c = c0 + g, c0 + g + 8, ...;
       // the four quarter sums meet through two shuffles.  A pass covers 64 coefficients (eight per lane), so all 32 lanes

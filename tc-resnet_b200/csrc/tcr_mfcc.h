@@ -5,10 +5,11 @@
 namespace tcr {
 
 struct MfccArgs {
-  const void* wav;          // [N, clip] fp32 samples, or int16 PCM when pcm16 != 0
+  const void* wav;          // [N, clip] fp32 samples, or int16 PCM when pcm16 != 0 (clip: the row stride in samples)
   int pcm16;
-  float* feat;              // [N, frames, features]
+  float* feat;              // [N, frames, features], utterance u at feat + u * feat_stride
   int clip, window, stride, frames, features, mel_bins;
+  int64_t feat_stride;      // floats between two utterances' features: frames * features, or a listener's history row (tcr_listener.cu)
   int fpb;                  // frames per CTA
   int warps;                // warps per CTA (<= 7): a warp takes frames warp, warp + warps, ... of the CTA's chunk
   int magnitude;            // 0: power spectrogram (MFCC path), 1: magnitude (log-mel path)

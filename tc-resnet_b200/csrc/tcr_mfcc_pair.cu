@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(160, 3) mfcc_pair_kernel(MfccArgs a) {
       lm[lms + 63 - lane] = logf(hi_b + 1e-6f);
     }
     __syncwarp();
-    float* outa = a.feat + ((size_t)utt * a.frames + (f0 + fa)) * a.features;
+    float* outa = a.feat + (size_t)utt * a.feat_stride + (size_t)(f0 + fa) * a.features;
     float* outb = outa + a.features;
     if (a.use_dct) {
       // DCT-II (40 of 64) for both frames: lane (q, g) = (lane / 8, lane % 8) sums mel rows m = q + 4 i for coefficients

@@ -9,11 +9,23 @@ void set_error(const char* msg);
 
 int net_alloc_workspace(tcr_handle* h);
 
-// Forward pass on features [n, T, F].  training: batch-statistics BN (+ dropout); otherwise the BN tables are
-// built from `moving`.  backward: the head additionally emits dlogits-derived tensors for the backward pass.
+// Front-end (tcr_api.cu): the handle's arguments for `wav` -> `feat` (per-clip geometry), and the launch of the kernel the
+// handle selects for them (the frame-pair kernel where the shape allows and TCR_MFCC_PAIR does not turn it off).
+MfccArgs mfcc_args(const tcr_handle* h, const void* wav, int pcm16, float* feat);
+int mfcc_select_launch(tcr_handle* h, const MfccArgs& a, int n, cudaStream_t stream);
+
+// conv0 reading its utterances as windows of a listener's feature history (tcr_listener.cu) instead of a [n, T, F] tensor:
+// utterance u starts at feat + (u / k) * stream + (u % k) * step floats.
+struct WindowView {
+  int k;
+  int64_t stream, step;
+};
+
+// Forward pass on features [n, T, F] (or the windows `win` describes).  training: batch-statistics BN (+ dropout); otherwise
+// the BN tables are built from `moving`.  backward: the head additionally emits dlogits-derived tensors for the backward pass.
 int net_forward(tcr_handle* h, const float* feat, const float* params, const float* moving, int n, bool training,
                 uint64_t seed, const float* mask, const float* onehot, float weight_decay, float* logits,
-                float* probs, float* losses, bool backward, cudaStream_t s);
+                float* probs, float* losses, bool backward, cudaStream_t s, const WindowView* win = nullptr);
 
 int cluster_size(tcr_handle* h);
 StatSrc stat_src(const tcr_handle* h, const ConvPlan& cv, const float* params, int n);

@@ -21,7 +21,9 @@ constexpr int TM = 4;   // output rows per thread task
 // ------------------------------------------------------------------------------------------------
 // conv forward
 // ------------------------------------------------------------------------------------------------
-template <int K, bool WSMEM>
+// WIN: the input rows of utterance u come from a window view (FwdArgs::win_k ...) instead of row u of a [n, t_in, cin] tensor;
+// nothing else differs.
+template <int K, bool WSMEM, bool WIN = false>
 __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, unsigned char* smem_raw, MbarCtx& mb) {
   float* smem = reinterpret_cast<float*>(smem_raw);
   const int tid = threadIdx.x;
@@ -75,13 +77,22 @@ __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, un
     const size_t grow = (size_t)u0 * a.t_in;
     constexpr int PF = 4;             // rows per thread kept in flight (a thread owns at most ~4 rows at the tile sizes in use)
     const bool res = a.in_kind == 2;
+    auto src_ofs = [&](int row) -> size_t {
+      if constexpr (WIN) {
+        const int ur = row / a.t_in, u = u0 + ur;
+        return (size_t)(u / a.win_k) * a.win_stream + (size_t)(u % a.win_k) * a.win_step + (size_t)(row - ur * a.t_in) * a.cin +
+               4 * w.c4;
+      } else {
+        return (grow + row) * a.cin + 4 * w.c4;
+      }
+    };
     float4 pin[PF], psh[PF];
 #pragma unroll
     for (int i = 0; i < PF; ++i) {
       const int row = w.row + i * w.rstep;
       pin[i] = psh[i] = make_float4(0.f, 0.f, 0.f, 0.f);
       if (row < rows) {
-        const size_t gofs = (grow + row) * a.cin + 4 * w.c4;
+        const size_t gofs = src_ofs(row);
         pin[i] = ld4(a.in.data + gofs);
         if (res) psh[i] = ld4(a.shortcut.data + gofs);
       }
@@ -115,7 +126,7 @@ __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, un
         if (row < rows) place(row, pin[i], psh[i]);
       }
       for (int row = w.row + PF * w.rstep; row < rows; row += w.rstep) {
-        const size_t gofs = (grow + row) * a.cin + 4 * w.c4;
+        const size_t gofs = src_ofs(row);
         place(row, ld4(a.in.data + gofs), res ? ld4(a.shortcut.data + gofs) : make_float4(0.f, 0.f, 0.f, 0.f));
       }
     }
@@ -156,12 +167,12 @@ __device__ __forceinline__ void conv_fwd_body(const FwdArgs& a, const int vb, un
   tl_stamp(a.tl, vb, 6);
 }
 
-template <int K, bool WSMEM>
+template <int K, bool WSMEM, bool WIN = false>
 __global__ void __launch_bounds__(kThreads) conv_fwd_kernel(FwdArgs a) {
   TCR_DYNAMIC_SMEM(smem_raw);
   MbarCtx mb{reinterpret_cast<uint64_t*>(smem_raw), 0u, false};
   pdl_trigger();                    // grid <= resident CTA slots: the next kernel's CTAs may take slots as ours retire
-  conv_fwd_body<K, WSMEM>(a, blockIdx.x, smem_raw, mb);
+  conv_fwd_body<K, WSMEM, WIN>(a, blockIdx.x, smem_raw, mb);
 }
 
 // Eval mode: BN tables from the moving statistics (bn_forward with is_training=False).
@@ -488,9 +499,9 @@ static ActSrc act_of(const tcr_handle* h, const ConvPlan& cv, int kind, const fl
   return ActSrc{cv.y, cv.bnf, kind, stat_src(h, cv, params, n)};
 }
 
-template <int K, bool WSMEM>
+template <int K, bool WSMEM, bool WIN = false>
 static int launch_conv_fwd(const char* name, const FwdArgs& a, int groups, size_t smem, cudaStream_t s, int cluster) {
-  auto kfn = conv_fwd_kernel<K, WSMEM>;
+  auto kfn = conv_fwd_kernel<K, WSMEM, WIN>;
 #ifndef TCR_EMU
   static SmemOptIn optin;           // one per template instantiation
   if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
@@ -528,6 +539,11 @@ static int conv_fwd(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, FwdArgs a, const 
     if (dn) dn->f_gc = grid / CL;
   }
   int rc;
+  if (a.win_k > 0) {                // conv0 over a listener's windows (3-tap, raw features)
+    if (cv.k != 3 || a.in_kind != 0) { set_error("windowed input needs the raw-feature 3-tap conv0"); return TCR_ERR_UNSUPPORTED; }
+    return wsm ? launch_conv_fwd<3, true, true>(("fwd:" + cv.name).c_str(), a, grid, smem, s, CL)
+               : launch_conv_fwd<3, false, true>(("fwd:" + cv.name).c_str(), a, grid, smem, s, CL);
+  }
   switch (cv.k) {
     case 3: rc = wsm ? launch_conv_fwd<3, true>(("fwd:" + cv.name).c_str(), a, grid, smem, s, CL)
                      : launch_conv_fwd<3, false>(("fwd:" + cv.name).c_str(), a, grid, smem, s, CL);
@@ -546,8 +562,9 @@ static int conv_fwd(tcr_handle* h, ConvPlan& cv, ConvPlan* dn, FwdArgs a, const 
 
 int net_forward(tcr_handle* h, const float* feat, const float* params, const float* moving, int n, bool training,
                 uint64_t seed, const float* mask, const float* onehot, float weight_decay, float* logits,
-                float* probs, float* losses, bool backward, cudaStream_t s) {
+                float* probs, float* losses, bool backward, cudaStream_t s, const WindowView* win) {
   (void)weight_decay;
+  if (win && (training || backward)) { set_error("windowed input is an evaluation-only path"); return TCR_ERR_UNSUPPORTED; }
   if (!training) {
     EvalBnArgs e;
     e.nlayers = (int)h->convs.size();
@@ -565,6 +582,7 @@ int net_forward(tcr_handle* h, const float* feat, const float* params, const flo
     memset(&a, 0, sizeof(a));
     a.in_kind = 0;
     a.in = ActSrc{feat, nullptr, 0, StatSrc{}};
+    if (win) { a.win_k = win->k; a.win_stream = win->stream; a.win_step = win->step; }
     int rc = conv_fwd(h, h->convs[0], nullptr, a, params, n, training, s);
     if (rc) return rc;
   }

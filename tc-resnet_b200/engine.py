@@ -342,6 +342,12 @@ class Engine:
                                                        self._stream), "tcr_eval_accumulate")
         return counts
 
+    def listener(self, streams: int, hop_frames: int, chunk_samples: int, params: Optional[torch.Tensor] = None,
+                 moving: Optional[torch.Tensor] = None) -> "Listener":
+        """A continuous-audio listener on this handle (tcr_listener_*): `streams` streams, a window every `hop_frames` frames,
+        `chunk_samples` new samples per stream and push, scored with `params` / `moving` (the tensors, read at every push)."""
+        return Listener(self, streams, hop_frames, chunk_samples, params, moving)
+
     # ------------------------------------------------------------------ data parallel
     def set_sync_bn(self, enable: bool = True):
         """Parity-test flag (SURVEY.md 8(e)): BatchNorm statistics over the global batch of all ranks (= one device with batch
@@ -406,6 +412,57 @@ class Engine:
         v = C.c_double()
         L.check(self.lib, self.lib.tcr_measure_fp32_peak(self._h, C.byref(v), self._stream), "tcr_measure_fp32_peak")
         return float(v.value)
+
+
+class Listener:
+    """S audio streams scored with a sliding window (include/tcr_b200.h, tcr_listener_*).  Each push takes `chunk_samples` new
+    samples per stream and returns the softmax of K = chunk_samples / (hop_frames * window_stride_samples) windows per stream;
+    window k of a stream (counted from its reset) is the clip starting k * hop_frames strides into the stream after
+    (T - hop_frames) * stride + (window - stride) zeros, scored exactly as Engine.forward scores it in evaluation mode."""
+
+    def __init__(self, engine: Engine, streams: int, hop_frames: int, chunk_samples: int, params: Optional[torch.Tensor] = None,
+                 moving: Optional[torch.Tensor] = None):
+        self.eng, self.params, self.moving = engine, params, moving
+        self._p = C.c_void_p()
+        cfg = L.TcrListenerConfig(int(streams), int(hop_frames), int(chunk_samples))
+        with torch.cuda.device(engine.device):
+            L.check(engine.lib, engine.lib.tcr_listener_create(engine._h, C.byref(cfg), C.byref(self._p)), "tcr_listener_create")
+        self.streams, self.hop_frames, self.chunk_samples = int(streams), int(hop_frames), int(chunk_samples)
+        self.windows = self.chunk_samples // (self.hop_frames * int(engine.cfg.window_stride_samples))
+
+    def close(self):
+        if getattr(self, "_p", None):
+            self.eng.lib.tcr_listener_destroy(self._p)
+            self._p = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def reset(self, stream: Optional[int] = None):
+        """Back to the state after creation: one stream, or all of them (None)."""
+        L.check(self.eng.lib, self.eng.lib.tcr_listener_reset(self._p, -1 if stream is None else int(stream), self.eng._stream),
+                "tcr_listener_reset")
+
+    def push(self, samples: torch.Tensor, params: Optional[torch.Tensor] = None, moving: Optional[torch.Tensor] = None,
+             probs: Optional[torch.Tensor] = None, logits: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """samples: CUDA fp32 (in [-1, 1]) or int16 tensor [S, chunk_samples].  Returns device probs [S, K, classes] (`probs`, when
+        given, is written in place; `logits` likewise receives the logits).  params / moving: the variables of this push, by
+        default the ones the listener was created with."""
+        eng = self.eng
+        params = params if params is not None else self.params
+        moving = moving if moving is not None else self.moving
+        assert samples.is_cuda and samples.is_contiguous() and tuple(samples.shape) == (self.streams, self.chunk_samples), \
+            f"expected a contiguous CUDA tensor [{self.streams}, {self.chunk_samples}]"
+        kind = L.TCR_INPUT_WAV_PCM16 if samples.dtype == torch.int16 else L.TCR_INPUT_WAV_F32
+        if kind == L.TCR_INPUT_WAV_F32:
+            assert samples.dtype == torch.float32, "samples must be fp32 or int16"
+        probs = probs if probs is not None else eng._f32(self.streams, self.windows, eng.num_classes)
+        L.check(eng.lib, eng.lib.tcr_listener_push(self._p, samples.data_ptr(), kind, eng._ptr(params), eng._ptr(moving),
+                                                   eng._ptr(logits), eng._ptr(probs), eng._stream), "tcr_listener_push")
+        return probs
 
 
 class HostFeed:

@@ -83,14 +83,7 @@ class AudioNetModel(TFModel):
         if self.engine_model is None:
             raise NotImplementedError(f"{type(self).__name__} is a baseline outside the accelerated TC-ResNet path")
         a = self.args
-        self.engine = Engine(model=self.engine_model, width_multiplier=a.width_multiplier, num_classes=a.num_classes,
-                             sample_rate=a.sample_rate, clip_duration_ms=a.clip_duration_ms,
-                             window_size_ms=a.window_size_ms, window_stride_ms=a.window_stride_ms,
-                             num_mel_bins=a.num_mel_bins, num_mfccs=a.num_mfccs, lower_edge_hertz=a.lower_edge_hertz,
-                             upper_edge_hertz=a.upper_edge_hertz, preprocess_method=a.preprocess_method,
-                             max_batch=max(int(getattr(a, 'batch_size', 1) or 1), int(getattr(a, 'input_batch_size', 1) or 1)),
-                             dropout_keep_prob=a.dropout_keep_prob,
-                             label_smoothing=getattr(a, "label_smoothing", 0.0))
+        self.engine = self._new_engine(max(int(getattr(a, 'batch_size', 1) or 1), int(getattr(a, 'input_batch_size', 1) or 1)))
         self.params, self.slots, self.moving = self.engine.new_variables(seed=getattr(a, "seed", 0) or 0)
         if getattr(a, "data_parallel", False):
             self.engine.attach_process_group()
@@ -103,6 +96,16 @@ class AudioNetModel(TFModel):
         if getattr(a, "device_dataset", False) and self.dataset is not None and self.dataset.device_data is None:
             self.dataset.attach_device(self.engine)
         return Node("logits", [None, a.num_classes]), {"ranges": Node("ranges")}
+
+    def _new_engine(self, max_batch: int) -> Engine:
+        a = self.args
+        return Engine(model=self.engine_model, width_multiplier=a.width_multiplier, num_classes=a.num_classes,
+                      sample_rate=a.sample_rate, clip_duration_ms=a.clip_duration_ms,
+                      window_size_ms=a.window_size_ms, window_stride_ms=a.window_stride_ms,
+                      num_mel_bins=a.num_mel_bins, num_mfccs=a.num_mfccs, lower_edge_hertz=a.lower_edge_hertz,
+                      upper_edge_hertz=a.upper_edge_hertz, preprocess_method=a.preprocess_method,
+                      max_batch=max_batch, dropout_keep_prob=a.dropout_keep_prob,
+                      label_smoothing=getattr(a, "label_smoothing", 0.0))
 
     def build_loss(self, logits, scores, labels):
         return Node("total_loss", []), Node("model_loss", []), {}
@@ -125,6 +128,26 @@ class AudioNetModel(TFModel):
             assert a.height > 0 and a.width > 0 and a.channels > 0
             node = Node("input", [1, a.height, a.width, a.channels])
         return [node], DeployedModel(self, n, include_preprocess)
+
+    def build_streaming_model(self, streams: int = 1, hop_ms: float = 10, chunk_ms: float = 100) -> "StreamingModel":
+        """The deploy graph run over continuous audio (include/tcr_b200.h, tcr_listener_*): `streams` independent streams, a
+        window every hop_ms (a whole number of frame strides) and chunk_ms of new audio per stream and push (a whole number of
+        hops).  Scores with the variables this model holds, so a checkpoint restored with --use_ema scores with the shadows."""
+        a = self.args
+        stride = int(a.sample_rate * a.window_stride_ms / 1000)
+        hop_samples = int(round(a.sample_rate * hop_ms / 1000))
+        chunk = int(round(a.sample_rate * chunk_ms / 1000))
+        if hop_samples <= 0 or hop_samples % stride:
+            raise ValueError(f"hop_ms {hop_ms} is not a positive multiple of the {a.window_stride_ms} ms frame stride")
+        hop = hop_samples // stride
+        if chunk <= 0 or chunk % hop_samples:
+            raise ValueError(f"chunk_ms {chunk_ms} is not a positive multiple of hop_ms {hop_ms}")
+        windows = int(streams) * (chunk // hop_samples)
+        if self.engine is None:
+            self.build_inference(None, is_training=False)
+        # the listener's forward runs at streams * windows utterances: a handle sized for that, on the same variables
+        engine = self.engine if int(self.engine.cfg.max_batch) >= windows else self._new_engine(windows)
+        return StreamingModel(self, engine, int(streams), hop, chunk)
 
     # ------------------------------------------------------------------ attribute surface
     @property
@@ -458,6 +481,51 @@ class DeployedModel:
             self._graph.replay()
         self._calls += 1
         return self._out["probs"].cpu().numpy()
+
+
+class StreamingModel:
+    """Continuous-audio entry (AudioNetModel.build_streaming_model): __call__ takes [streams, chunk_samples] new samples (fp32 in
+    [-1, 1] or int16) and returns the softmax [streams, windows, classes] of the windows they complete; window k of a stream ends
+    (k + 1) * hop samples after its reset.  Like DeployedModel, two eager pushes, then each push is replayed from a CUDA graph."""
+
+    def __init__(self, model: "AudioNetModel", engine: Engine, streams: int, hop_frames: int, chunk_samples: int,
+                 use_graph: bool = True):
+        self.model, self.engine, self.use_graph = model, engine, use_graph
+        self.listener = engine.listener(streams, hop_frames, chunk_samples)
+        self.streams, self.hop_frames, self.chunk_samples = streams, hop_frames, chunk_samples
+        self.windows = self.listener.windows
+        self.hop_samples = hop_frames * int(engine.cfg.window_stride_samples)
+        self._in = {dt: torch.zeros(streams, chunk_samples, dtype=dt, device=engine.device) for dt in (torch.float32, torch.int16)}
+        self._probs = torch.zeros(streams, self.windows, engine.num_classes, dtype=torch.float32, device=engine.device)
+        self._graphs, self._calls = {}, 0
+
+    def _push(self, dt):
+        m = self.model
+        self.listener.push(self._in[dt], m.params, m.moving, probs=self._probs)
+
+    def reset(self, stream: Optional[int] = None):
+        self.listener.reset(stream)
+
+    def __call__(self, x) -> np.ndarray:
+        x = torch.as_tensor(x)
+        dt = torch.int16 if x.dtype == torch.int16 else torch.float32
+        self._in[dt].copy_(x.to(dt).reshape(self.streams, self.chunk_samples), non_blocking=True)
+        if not self.use_graph or self._calls < 2:                  # two eager calls first: lazy per-kernel attributes are set outside capture
+            self._push(dt)
+        else:
+            if dt not in self._graphs:
+                dev = self.engine.device
+                stream = torch.cuda.Stream(device=dev)
+                stream.wait_stream(torch.cuda.current_stream(dev))
+                with torch.cuda.stream(stream):
+                    g = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g, stream=stream):
+                        self._push(dt)
+                torch.cuda.current_stream(dev).wait_stream(stream)
+                self._graphs[dt] = g
+            self._graphs[dt].replay()
+        self._calls += 1
+        return self._probs.cpu().numpy()
 
 
 class TCResNet8Model(AudioNetModel):

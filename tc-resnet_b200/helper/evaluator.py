@@ -34,13 +34,7 @@ class Evaluator:
         (common/model_loader.py:42-83), or with --use_ema every trainable variable taken from its shadow
         (helper/evaluator.py:41-48).  The reference crashes on --use_ema together with a scope filter (model_loader.py:76-80
         calls .op.name on the dict's string keys); that combination is rejected here (SURVEY.md section 9)."""
-        include = getattr(self.args, "checkpoint_include_scopes", "")
-        exclude = getattr(self.args, "checkpoint_exclude_scopes", "")
-        if getattr(self.args, "use_ema", False):
-            if model_loader.split_strip(include) or model_loader.split_strip(exclude):
-                raise ValueError("--use_ema cannot be combined with --checkpoint_include_scopes / --checkpoint_exclude_scopes")
-            return model_loader.ema_restore_values(values, self.model.engine.trainable_names), None
-        return values, model_loader.restore_filter(include, exclude)
+        return model_loader.evaluation_restore(self.args, values, lambda: self.model.engine.trainable_names)
 
     def build_evaluation_step(self, checkpoint_path):
         return ckpt.checkpoint_step(checkpoint_path)
