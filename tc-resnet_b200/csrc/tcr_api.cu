@@ -565,7 +565,8 @@ extern "C" int tcr_augment_pcm16(tcr_handle* h, const int16_t* pcm, int64_t pcm_
   TCR_TRY(check_n(h, n));
   if (pcm_stride < 1) return fail(TCR_ERR_INVALID, "pcm_stride must be positive");
   if (((uintptr_t)wav_out & 15) != 0) return fail(TCR_ERR_INVALID, "wav_out must be 16-byte aligned");
-  augment_launch(pcm, pcm_stride, clips, background, h->background_samples, wav_out, h->cfg.clip_samples, n, (cudaStream_t)stream);
+  if (augment_launch(pcm, pcm_stride, clips, background, h->background_samples, wav_out, h->cfg.clip_samples, n, (cudaStream_t)stream))
+    return fail(TCR_ERR_CUDA, "augment launch failed");
   TCR_CUDA(cudaGetLastError());
   return TCR_OK;
 }
@@ -610,8 +611,9 @@ extern "C" int tcr_dataset_batch(tcr_handle* h, const tcr_dataset* desc, int64_t
   TCR_TRY(check_n(h, n));
   TCR_TRY(dataset_check(h, desc, position, n));
   if (((uintptr_t)wav_out & 15) != 0) return fail(TCR_ERR_INVALID, "wav_out must be 16-byte aligned");
-  dataset_batch_launch(*desc, position, epoch, seed, wav_out, onehot_out, h->cfg.clip_samples, h->cfg.num_classes, n,
-                       (cudaStream_t)stream);
+  if (dataset_batch_launch(*desc, position, epoch, seed, wav_out, onehot_out, h->cfg.clip_samples, h->cfg.num_classes, n,
+                           (cudaStream_t)stream))
+    return fail(TCR_ERR_CUDA, "dataset batch launch failed");
   TCR_CUDA(cudaGetLastError());
   return TCR_OK;
 }
@@ -741,8 +743,9 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
       float*& hot = fe_buf >= 0 ? h->fe_hot[fe_buf] : h->d_hot;
       TCR_TRY(lazy_buffer(h, aug, (size_t)h->cfg.max_batch * h->cfg.clip_samples));
       TCR_TRY(lazy_buffer(h, hot, (size_t)h->cfg.max_batch * h->cfg.num_classes));
-      dataset_batch_launch(*a->dataset, a->dataset_position, a->dataset_epoch, a->dataset_seed, aug, hot, h->cfg.clip_samples,
-                           h->cfg.num_classes, a->n, (cudaStream_t)fs);
+      if (dataset_batch_launch(*a->dataset, a->dataset_position, a->dataset_epoch, a->dataset_seed, aug, hot, h->cfg.clip_samples,
+                               h->cfg.num_classes, a->n, (cudaStream_t)fs))
+        return fail(TCR_ERR_CUDA, "dataset batch launch failed");
       TCR_TRY(mfcc_run(h, aug, 0, featbuf, a->n, fs));
       ds_args = *a;
       ds_args.onehot = hot;
@@ -752,8 +755,9 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
       const int64_t stride = a->pcm_stride > 0 ? a->pcm_stride : h->cfg.clip_samples;
       float*& aug = fe_buf >= 0 ? h->fe_aug : h->d_aug;       // the ahead path decodes into its own buffer
       TCR_TRY(lazy_buffer(h, aug, (size_t)h->cfg.max_batch * h->cfg.clip_samples));
-      augment_launch((const int16_t*)a->input, stride, a->clips, a->background, h->background_samples, aug, h->cfg.clip_samples, a->n,
-                     (cudaStream_t)fs);
+      if (augment_launch((const int16_t*)a->input, stride, a->clips, a->background, h->background_samples, aug, h->cfg.clip_samples, a->n,
+                         (cudaStream_t)fs))
+        return fail(TCR_ERR_CUDA, "augment launch failed");
       TCR_TRY(mfcc_run(h, aug, 0, featbuf, a->n, fs));
     } else {
       TCR_TRY(mfcc_run(h, a->input, a->input_is_features == TCR_INPUT_WAV_PCM16, featbuf, a->n, fs));

@@ -133,17 +133,26 @@ __global__ void __launch_bounds__(256) augment_kernel(Args a) {
 
 static int augment_blocks(int clip) { return std::max(1, std::min(8, (clip / 4 + 255) / 256)); }
 
+// One clip per blockIdx.y: batches past kMaxGridRows run as several launches over consecutive rows.  Nonzero: a launch failed.
 int augment_launch(const int16_t* pcm, int64_t pcm_stride, const tcr_augment_clip* clips, const float* background, int64_t background_samples,
                    float* out, int clip, int n, cudaStream_t s) {
-  AugArgs a{pcm, pcm_stride, clips, background, background_samples, out, clip};
-  TCR_LAUNCH("augment", augment_kernel<AugArgs>, dim3(augment_blocks(clip), n), dim3(256), 0, s, a);
+  for (int first = 0; first < n; first += kMaxGridRows) {
+    AugArgs a{pcm + (size_t)first * pcm_stride, pcm_stride, clips + first, background, background_samples, out + (size_t)first * clip, clip};
+    TCR_LAUNCH("augment", augment_kernel<AugArgs>, dim3(augment_blocks(clip), std::min(n - first, kMaxGridRows)), dim3(256), 0, s, a);
+    if (cudaGetLastError() != cudaSuccess) return 1;
+  }
   return 0;
 }
 
+// Row i of a slice is row first + i of the batch: its order entry and its draws are keyed by position + first + i.
 int dataset_batch_launch(const tcr_dataset& ds, int64_t position, int64_t epoch, uint64_t seed, float* out, float* onehot, int clip,
                          int classes, int n, cudaStream_t s) {
-  DatasetArgs a{ds, position, splitmix64(seed, (uint64_t)epoch), onehot, classes, out, clip};
-  TCR_LAUNCH("dataset_batch", augment_kernel<DatasetArgs>, dim3(augment_blocks(clip), n), dim3(256), 0, s, a);
+  for (int first = 0; first < n; first += kMaxGridRows) {
+    DatasetArgs a{ds, position + first, splitmix64(seed, (uint64_t)epoch), onehot + (size_t)first * classes, classes,
+                  out + (size_t)first * clip, clip};
+    TCR_LAUNCH("dataset_batch", augment_kernel<DatasetArgs>, dim3(augment_blocks(clip), std::min(n - first, kMaxGridRows)), dim3(256), 0, s, a);
+    if (cudaGetLastError() != cudaSuccess) return 1;
+  }
   return 0;
 }
 

@@ -82,6 +82,10 @@ struct SmemOptIn {
 
 namespace tcr {
 
+// CUDA's bound on gridDim.y and gridDim.z.  Kernels with one utterance (or stream) per blockIdx.y are launched in slices of at
+// most this many rows, with the row pointers offset on the host, so any batch a handle accepts runs.
+constexpr int kMaxGridRows = 65535;
+
 // programmatic dependent launch (see launch_pdl): no-ops in a kernel that was launched without the attribute
 __device__ __forceinline__ void pdl_wait() {
 #ifndef TCR_EMU

@@ -1170,7 +1170,13 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
     static SmemOptIn optin;
     if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
 #endif
-    TCR_LAUNCH("dscnn_dsblock", kfn, dim3(ds_tiles_per_utt(L, RH), n), dim3(256), smem, s, L, RH, COT, params, in, out, eps);
+    // one utterance per blockIdx.y: batches past kMaxGridRows run as several launches over consecutive utterances
+    const size_t in_utt = (size_t)L.hin * L.win * L.cin, out_utt = (size_t)L.hout * L.wout * L.cout;
+    for (int first = 0; first < n; first += kMaxGridRows) {
+      TCR_LAUNCH("dscnn_dsblock", kfn, dim3(ds_tiles_per_utt(L, RH), std::min(n - first, kMaxGridRows)), dim3(256), smem, s, L, RH, COT,
+                 params, in + first * in_utt, out + first * out_utt, eps);
+      if (cudaGetLastError() != cudaSuccess) { set_error("DS-CNN block launch failed"); return TCR_ERR_CUDA; }
+    }
   }
   return TCR_OK;
 }

@@ -118,10 +118,27 @@ int listener_reset_rows(tcr_listener* L, int first, int count, cudaStream_t st) 
   if (rc) return rc;
   if (L->carried > 1) {
     const int n = (L->carried - 1) * L->h->features;
-    TCR_LAUNCH("listener_reset", listener_reset_kernel, dim3((n + kListenThreads - 1) / kListenThreads, count), dim3(kListenThreads), 0, st,
-               L->hist, L->hist_stride, first, L->carried, L->h->features);
+    for (int f = first; f < first + count; f += kMaxGridRows) {      // one stream per blockIdx.y
+      const int rows = std::min(first + count - f, kMaxGridRows);
+      TCR_LAUNCH("listener_reset", listener_reset_kernel, dim3((n + kListenThreads - 1) / kListenThreads, rows), dim3(kListenThreads), 0, st,
+                 L->hist, L->hist_stride, f, L->carried, L->h->features);
+      if (cudaGetLastError() != cudaSuccess) return lfail(TCR_ERR_CUDA, "listener reset launch failed");
+    }
   }
-  if (cudaGetLastError() != cudaSuccess) return lfail(TCR_ERR_CUDA, "listener reset launch failed");
+  return TCR_OK;
+}
+
+// The new chunk of every stream into the sample rows behind the tail, in slices of at most kMaxGridRows streams (blockIdx.y).
+int listener_stage(tcr_listener* L, const void* samples, bool pcm, cudaStream_t st) {
+  const size_t in_bytes = pcm ? sizeof(int16_t) : sizeof(float);
+  for (int first = 0; first < L->S; first += kMaxGridRows) {
+    const dim3 sgrid((L->chunk / 4 + kListenThreads - 1) / kListenThreads, std::min(L->S - first, kMaxGridRows));
+    const void* in = static_cast<const char*>(samples) + (size_t)first * L->chunk * in_bytes;
+    float* rows = L->samples + (size_t)first * L->row;
+    if (pcm) TCR_LAUNCH("listener_stage", listener_stage_kernel<true>, sgrid, dim3(kListenThreads), 0, st, in, rows, L->chunk, L->tail, L->row);
+    else TCR_LAUNCH("listener_stage", listener_stage_kernel<false>, sgrid, dim3(kListenThreads), 0, st, in, rows, L->chunk, L->tail, L->row);
+    if (cudaGetLastError() != cudaSuccess) return lfail(TCR_ERR_CUDA, "listener stage launch failed");
+  }
   return TCR_OK;
 }
 
@@ -185,10 +202,9 @@ extern "C" int tcr_listener_push(tcr_listener* L, const void* samples, int32_t i
   if (pcm && (h->cfg.window_size_samples % 8 || h->cfg.window_stride_samples % 8 || L->chunk % 8))
     return lfail(TCR_ERR_UNSUPPORTED, "int16 input needs window, stride and chunk lengths that are multiples of 8 samples");
   cudaStream_t st = (cudaStream_t)stream_;
-  const dim3 sgrid((L->chunk / 4 + kListenThreads - 1) / kListenThreads, L->S);
-  if (pcm) TCR_LAUNCH("listener_stage", listener_stage_kernel<true>, sgrid, dim3(kListenThreads), 0, st, samples, L->samples, L->chunk, L->tail, L->row);
-  else TCR_LAUNCH("listener_stage", listener_stage_kernel<false>, sgrid, dim3(kListenThreads), 0, st, samples, L->samples, L->chunk, L->tail, L->row);
-  int rc = listener_frontend(L, 0, L->S, L->K * L->hop, L->carried, st);
+  int rc = listener_stage(L, samples, pcm, st);
+  if (rc) return rc;
+  rc = listener_frontend(L, 0, L->S, L->K * L->hop, L->carried, st);
   if (rc) return rc;
   const WindowView win{L->K, L->hist_stride, (int64_t)L->hop * h->features};
   rc = net_forward(h, L->hist, params, moving, L->S * L->K, false, 0, nullptr, nullptr, 0.f, logits, probs, nullptr, false, st, &win);

@@ -357,37 +357,44 @@ size_t mfcc_smem_bytes(const MfccArgs& a, int nf2, int warps) {
   return 16 + (size_t)span_max * 4 + (size_t)a.c_smem * 4 + per_warp * warps;
 }
 
+// One utterance per blockIdx.y: batches past kMaxGridRows run as several launches over consecutive rows.
 int mfcc_launch(const MfccArgs& a, int n, int fft_length, cudaStream_t stream) {
   const int nf2 = fft_length / 2;
   const int warps = a.warps;
-  dim3 grid((a.frames + a.fpb - 1) / a.fpb, n, 1);
   dim3 block(32 * warps, 1, 1);
   const size_t smem = mfcc_smem_bytes(a, nf2, warps);
+  for (int first = 0; first < n; first += kMaxGridRows) {
+    MfccArgs b = a;
+    b.wav = static_cast<const char*>(a.wav) + (size_t)first * a.clip * (a.pcm16 ? 2 : 4);
+    b.feat = a.feat + (size_t)first * a.feat_stride;
+    dim3 grid((a.frames + a.fpb - 1) / a.fpb, n - first < kMaxGridRows ? n - first : kMaxGridRows, 1);
 #ifndef TCR_EMU
 #define TCR_MFCC_CASE(NF2)                                                         \
   case NF2: {                                                                      \
     auto k = a.pcm16 ? mfcc_kernel<NF2, true> : mfcc_kernel<NF2, false>;           \
     static SmemOptIn optin[2];                                                     \
     if (optin[a.pcm16 ? 1 : 0].ensure(k, smem) != cudaSuccess) return 1;           \
-    TCR_LAUNCH("mfcc", k, grid, block, smem, stream, a);                           \
+    TCR_LAUNCH("mfcc", k, grid, block, smem, stream, b);                           \
   } break;
 #else
 #define TCR_MFCC_CASE(NF2)                         \
   case NF2: {                                      \
     auto k = a.pcm16 ? mfcc_kernel<NF2, true> : mfcc_kernel<NF2, false>; \
-    TCR_LAUNCH("mfcc", k, grid, block, smem, stream, a);   \
+    TCR_LAUNCH("mfcc", k, grid, block, smem, stream, b);   \
   } break;
 #endif
-  switch (nf2) {
-    TCR_MFCC_CASE(1024)
-    TCR_MFCC_CASE(512)
-    TCR_MFCC_CASE(256)
-    TCR_MFCC_CASE(128)
-    TCR_MFCC_CASE(64)
-    default:
-      return 2;
-  }
+    switch (nf2) {
+      TCR_MFCC_CASE(1024)
+      TCR_MFCC_CASE(512)
+      TCR_MFCC_CASE(256)
+      TCR_MFCC_CASE(128)
+      TCR_MFCC_CASE(64)
+      default:
+        return 2;
+    }
 #undef TCR_MFCC_CASE
+    if (cudaGetLastError() != cudaSuccess) return 1;
+  }
   return 0;
 }
 

@@ -180,7 +180,17 @@ unsigned ballot(int pred) {
   return m;
 }
 
-void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body) {
+// CUDA's launch bounds (compute capability 9.0): a launch outside them fails with cudaErrorInvalidConfiguration before any block runs
+static bool refused(dim3 grid, dim3 block) {
+  const unsigned long long threads = (unsigned long long)block.x * block.y * block.z;
+  const bool bad = grid.x < 1 || grid.x > 2147483647u || grid.y < 1 || grid.y > 65535u || grid.z < 1 || grid.z > 65535u ||
+                   threads < 1 || threads > 1024 || block.z > 64;
+  if (bad) g_state.last_error = cudaErrorInvalidConfiguration;
+  return bad;
+}
+
+int launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body) {
+  if (refused(grid, block)) return cudaErrorInvalidConfiguration;
   std::vector<uint3> one(1);
   for (unsigned bz = 0; bz < grid.z; ++bz)
     for (unsigned by = 0; by < grid.y; ++by)
@@ -188,6 +198,7 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()
         one[0] = uint3{bx, by, bz};
         run(grid, block, smem_bytes, body, one, 256 * 1024);
       }
+  return cudaSuccess;
 }
 
 unsigned cluster_rank() { return g_cluster > 1 ? (unsigned)me().block : 0u; }
@@ -203,8 +214,9 @@ const void* dsmem(const void* local, unsigned rank) {
   return theirs + ((const unsigned char*)local - mine);
 }
 
-void launch_cluster(dim3 grid, dim3 block, size_t smem_bytes, unsigned cluster, const std::function<void()>& body) {
-  if (cluster <= 1) { launch(grid, block, smem_bytes, body); return; }
+int launch_cluster(dim3 grid, dim3 block, size_t smem_bytes, unsigned cluster, const std::function<void()>& body) {
+  if (cluster <= 1) return launch(grid, block, smem_bytes, body);
+  if (refused(grid, block)) return cudaErrorInvalidConfiguration;
   if (grid.x % cluster != 0 || grid.y != 1 || grid.z != 1) { fprintf(stderr, "emu: grid %u not a multiple of cluster %u\n", grid.x, cluster); abort(); }
   std::vector<uint3> blocks(cluster);
   g_cluster = cluster;
@@ -213,14 +225,17 @@ void launch_cluster(dim3 grid, dim3 block, size_t smem_bytes, unsigned cluster, 
     run(grid, block, smem_bytes, body, blocks, 128 * 1024);
   }
   g_cluster = 1;
+  return cudaSuccess;
 }
 
-void launch_cooperative(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body) {
+int launch_cooperative(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body) {
+  if (refused(grid, block)) return cudaErrorInvalidConfiguration;
   std::vector<uint3> all;
   for (unsigned bz = 0; bz < grid.z; ++bz)
     for (unsigned by = 0; by < grid.y; ++by)
       for (unsigned bx = 0; bx < grid.x; ++bx) all.push_back(uint3{bx, by, bz});
   run(grid, block, smem_bytes, body, all, 128 * 1024);
+  return cudaSuccess;
 }
 
 }  // namespace emu

@@ -49,11 +49,14 @@ struct ThreadCtx { uint3 tid; uint3 bid; unsigned char* smem; };
 struct State {
   ThreadCtx* cur = nullptr;
   dim3 bdim, gdim;
+  int last_error = 0;   // what cudaGetLastError returns (and clears): a launch the device would refuse
 };
 State& st();
-void launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body);
-void launch_cooperative(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body);   // all blocks co-resident
-void launch_cluster(dim3 grid, dim3 block, size_t smem_bytes, unsigned cluster, const std::function<void()>& body);   // one cluster at a time
+// A launch whose grid or block CUDA would refuse (grid.x outside [1, 2^31 - 1], grid.y or grid.z outside [1, 65535], more than
+// 1,024 threads or block.z > 64) runs nothing and returns cudaErrorInvalidConfiguration, which cudaGetLastError then reports.
+int launch(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body);
+int launch_cooperative(dim3 grid, dim3 block, size_t smem_bytes, const std::function<void()>& body);   // all blocks co-resident
+int launch_cluster(dim3 grid, dim3 block, size_t smem_bytes, unsigned cluster, const std::function<void()>& body);   // one cluster at a time
 void gridsync();
 unsigned cluster_rank();
 unsigned cluster_size();
@@ -139,11 +142,15 @@ static inline size_t max(size_t a, size_t b) { return a > b ? a : b; }
 typedef int cudaError_t;
 typedef void* cudaStream_t;
 typedef void* cudaEvent_t;
-enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2 };
+enum { cudaSuccess = 0, cudaErrorMemoryAllocation = 2, cudaErrorInvalidConfiguration = 9 };
 enum cudaMemcpyKind { cudaMemcpyHostToHost, cudaMemcpyHostToDevice, cudaMemcpyDeviceToHost, cudaMemcpyDeviceToDevice, cudaMemcpyDefault };
-static inline const char* cudaGetErrorString(cudaError_t) { return "emu"; }
-static inline cudaError_t cudaGetLastError() { return cudaSuccess; }
-static inline cudaError_t cudaPeekAtLastError() { return cudaSuccess; }
+static inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaErrorInvalidConfiguration ? "invalid configuration argument" : "emu"; }
+static inline cudaError_t cudaGetLastError() {
+  const cudaError_t e = emu::st().last_error;
+  emu::st().last_error = cudaSuccess;
+  return e;
+}
+static inline cudaError_t cudaPeekAtLastError() { return emu::st().last_error; }
 static inline cudaError_t cudaMalloc(void** p, size_t n) {
   if (posix_memalign(p, 256, n ? n : 256) != 0) return cudaErrorMemoryAllocation;
   std::memset(*p, 0xFF, n);  // poison

@@ -63,17 +63,20 @@ class Offline:
         self.seq[s], self.k[s] = np.zeros(self.pre, np.float32), 0
 
     def push(self, samples):
-        """The clips of the windows this push emits, [S, K, clip] fp32 (int16 decoded as decode_wav does)."""
+        """The clips of the windows this push emits, [S, K, clip] fp32 (int16 decoded as decode_wav does).  A clip longer than
+        (T - 1) * stride + window (400 / 160 at 16 kHz: 80 samples) ends in samples no frame reads; where the stream has not
+        reached them yet they are zeros."""
         x = np.asarray(samples)
         x = x.astype(np.float32) / np.float32(32768.0) if x.dtype == np.int16 else x.astype(np.float32)
         step = self.hop * self.stride
         K = x.shape[1] // step
-        out = np.empty((len(self.seq), K, self.clip), np.float32)
+        out = np.zeros((len(self.seq), K, self.clip), np.float32)
         for s in range(len(self.seq)):
             self.seq[s] = np.concatenate([self.seq[s], x[s]])
             for j in range(K):
                 k = self.k[s] + j
-                out[s, j] = self.seq[s][k * step:k * step + self.clip]
+                seg = self.seq[s][k * step:k * step + self.clip]
+                out[s, j, :seg.size] = seg
             self.k[s] += K
         return out
 
