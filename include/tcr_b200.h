@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 10
+#define TCR_ABI_VERSION 11
 
 enum {
   TCR_OK = 0,
@@ -312,9 +312,10 @@ int tcr_forward(tcr_handle* h, const float* input, int32_t input_is_features, co
  * tcr_listener_reset   stream: index of the stream to reset, or -1 for all of them (TCR_ERR_INVALID otherwise).
  * tcr_listener_push    samples: device [S, chunk_samples], fp32 in [-1,1] (TCR_INPUT_WAV_F32) or int16 PCM (TCR_INPUT_WAV_PCM16,
  *                      decode_wav's 1/32768 scaling, bit-identical to the decoded fp32 samples), 16-byte aligned;
- *                      logits / probs: device [S, K, num_classes] or NULL.  TCR_ERR_INVALID: a NULL handle / samples / params /
- *                      moving, another input kind, a misaligned samples pointer.  TCR_ERR_UNSUPPORTED: int16 input with window,
- *                      stride or chunk lengths that are not multiples of 8 samples (as tcr_forward).
+ *                      logits / probs: device [S, K, num_classes] or NULL.  TCR_ERR_INVALID: a NULL handle / samples / params,
+ *                      a NULL `moving` on a TC-ResNet listener or a non-NULL one on a DS-CNN listener (tcr_dscnn_listener_create),
+ *                      another input kind, a misaligned samples pointer.  TCR_ERR_UNSUPPORTED: int16 input with window, stride
+ *                      or chunk lengths that are not multiples of 8 samples (as tcr_forward).
  * tcr_listener_destroy frees the listener's buffers (NULL is a no-op); destroy listeners before their handle. */
 typedef struct tcr_listener tcr_listener;
 typedef struct tcr_listener_config {
@@ -407,8 +408,8 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
 /* DS-CNN (Hello-Edge) forward pass, inference mode: the reference's 2-D-conv comparison model
  * (audio_nets/ds_cnn.py:20-118; factory/audio_nets.py DSCNN{S,M,L}Model.build_inference; BASELINE.json config 5).
  * features [n, height, width] (== [N,H,W,1]); params = one flat fp32 buffer laid out by tcr_dscnn_param_table
- * (TF variable names "DSCNN/conv_1/weights", ".../batch_norm/moving_mean", "DSCNN/fc1/biases", ...).
- * size: 'S' or 'M' ('L' builds its table but its 276-channel head is not supported yet). */
+ * (TF variable names "DSCNN/conv_1/weights", ".../batch_norm/moving_mean", "DSCNN/fc1/biases", ...), the BatchNorm moving
+ * statistics included.  size: 'S', 'M' or 'L' (64, 172 and 276 channels; the head takes up to 320). */
 typedef struct tcr_dscnn tcr_dscnn;
 typedef struct tcr_dscnn_config {
   int32_t size;          /* 'S' | 'M' | 'L' */
@@ -428,6 +429,30 @@ int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const float* params, 
  * num_layers - 1 is written to act_out and nothing else is (for checking one layer at a time against a reference). */
 int tcr_dscnn_forward_partial(tcr_dscnn* d, const float* features, const float* params, int32_t n, int32_t num_layers,
                               float* act_out, tcr_stream stream);
+/* Evaluation from audio on a DS-CNN handle (ABI 11), the evaluation graph of evaluate_audio.py with a DSCNN{S,M,L}Model
+ * (helper/base.py:52-125):
+ * tcr_dscnn_set_frontend   gives the handle the front-end of a tcr_config (datasets/preprocessors.py:64-96, 183-194): only the
+ *                          front-end fields are read (sample_rate, clip_samples, window / stride, num_mel_bins, num_mfccs, edges,
+ *                          feature_kind), with tcr_create's refusals; TCR_ERR_INVALID, naming both shapes, when its (T, F) is not
+ *                          the handle's (height, width).  Sizes a feature buffer for max_batch.  The tables are the ones tcr_create
+ *                          builds, and the same kernel runs, so the features equal tcr_mfcc_forward's bit for bit.  Calling it
+ *                          again replaces the front-end (the call synchronises the device).
+ * tcr_dscnn_mfcc_forward   front-end only: wav [n, clip_samples] (TCR_INPUT_WAV_F32 or TCR_INPUT_WAV_PCM16, 16-byte aligned)
+ *                          -> features [n, height, width].
+ * tcr_dscnn_forward_input  the forward from TCR_INPUT_FEATURES (== tcr_dscnn_forward), TCR_INPUT_WAV_F32 or TCR_INPUT_WAV_PCM16: the
+ *                          front-end into the handle's feature buffer, then the same forward, so the result equals
+ *                          tcr_dscnn_forward on tcr_dscnn_mfcc_forward's features bit for bit.
+ * tcr_dscnn_eval_accumulate  tcr_eval_accumulate's counts (same kernel, same layout) for num_classes of the DS-CNN handle.
+ * tcr_dscnn_listener_create  a tcr_listener (see above) on the DS-CNN handle and its front-end; tcr_listener_reset / _push / _history
+ *                          / _destroy are shared, with the same four promises (tcr_dscnn_forward in place of tcr_forward).  Its
+ *                          pushes pass moving = NULL.  TCR_ERR_INVALID without a front-end. */
+int tcr_dscnn_set_frontend(tcr_dscnn* d, const tcr_config* frontend);
+int tcr_dscnn_mfcc_forward(tcr_dscnn* d, const void* wav, int32_t input_kind, float* features, int32_t n, tcr_stream stream);
+int tcr_dscnn_forward_input(tcr_dscnn* d, const void* input, int32_t input_kind, const float* params, int32_t n, float* logits,
+                            float* probs, tcr_stream stream);
+int tcr_dscnn_eval_accumulate(tcr_dscnn* d, const float* scores, const float* onehot, int32_t n, int32_t topk, int64_t* counts,
+                              tcr_stream stream);
+int tcr_dscnn_listener_create(tcr_dscnn* d, const tcr_listener_config* cfg, tcr_listener** out);
 
 /* Process-wide launch accounting (no reference counterpart; the reference only logs wall-clock per
  * session.run, helper/trainer.py:312-321).  tcr_launch_count: kernels launched by this library so far.

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtcr_b200.so")
 
 TCR_MODEL_TCRESNET8 = 8
 TCR_MODEL_TCRESNET14 = 14
-ABI_VERSION = 10       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
+ABI_VERSION = 11       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
 TCR_INPUT_WAV_F32, TCR_INPUT_FEATURES, TCR_INPUT_WAV_PCM16 = 0, 1, 2
 TCR_OPT_MOMENTUM, TCR_OPT_ADAM, TCR_OPT_RMSPROP = 0, 1, 2
 TCR_FEATURE_MFCC = 0
@@ -135,6 +135,11 @@ SYMBOLS = {
                                         C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "tcr_dscnn_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tcr_dscnn_forward_partial": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "tcr_dscnn_set_frontend": (C.c_int, [C.c_void_p, C.POINTER(TcrConfig)]),
+    "tcr_dscnn_mfcc_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "tcr_dscnn_forward_input": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tcr_dscnn_eval_accumulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "tcr_dscnn_listener_create": (C.c_int, [C.c_void_p, C.POINTER(TcrListenerConfig), C.POINTER(C.c_void_p)]),
     "tcr_profile_enable": (C.c_int, [C.c_int]),
     "tcr_profile_read": (C.c_int, [C.POINTER(C.POINTER(TcrKernelStat)), C.POINTER(C.c_int32)]),
     "tcr_launch_count": (C.c_int, [C.POINTER(C.c_uint64)]),

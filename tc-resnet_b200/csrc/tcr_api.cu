@@ -68,19 +68,23 @@ extern "C" int tcr_config_default(tcr_config* cfg) {
 // device allocation helpers
 // ------------------------------------------------------------------------------------------------
 template <class T>
-static int dev_alloc(tcr_handle* h, T** p, size_t count) {
+static int dev_alloc(std::vector<void*>& allocs, int64_t& total, T** p, size_t count) {
   void* q = nullptr;
   size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
   bytes = (bytes + 255) & ~(size_t)255;
   if (cudaMalloc(&q, bytes) != cudaSuccess) return fail(TCR_ERR_CUDA, "cudaMalloc(%zu bytes) failed", bytes);
-  h->allocs.push_back(q);
-  h->workspace_bytes += (int64_t)bytes;
+  allocs.push_back(q);
+  total += (int64_t)bytes;
   *p = (T*)q;
   return TCR_OK;
 }
 template <class T>
-static int dev_upload(tcr_handle* h, T** p, const std::vector<T>& v) {
-  int rc = dev_alloc(h, p, v.size());
+static int dev_alloc(tcr_handle* h, T** p, size_t count) {
+  return dev_alloc(h->allocs, h->workspace_bytes, p, count);
+}
+template <class T>
+static int dev_upload(Frontend& fe, T** p, const std::vector<T>& v) {
+  int rc = dev_alloc(fe.allocs, fe.bytes, p, v.size());
   if (rc) return rc;
   if (!v.empty()) TCR_CUDA(cudaMemcpy(*p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
   return TCR_OK;
@@ -100,9 +104,9 @@ static int next_pow2(int n) {
   return p;
 }
 
-static int build_frontend_tables(tcr_handle* h) {
-  const tcr_config& c = h->cfg;
-  const int W = c.window_size_samples, fft = h->fft, nf2 = fft / 2, bins = nf2 + 1;
+static int build_frontend_tables(Frontend& fe) {
+  const tcr_config& c = fe.cfg;
+  const int W = c.window_size_samples, fft = fe.fft, nf2 = fft / 2, bins = nf2 + 1;
   // tf.contrib.signal.hann_window(periodic=True): n = W + even - 1, w = 0.5 - 0.5 cos(2 pi i / n)
   std::vector<float> win(W);
   const int even = 1 - W % 2;
@@ -154,7 +158,7 @@ static int build_frontend_tables(tcr_handle* h) {
     }
   }
   // mfccs_from_log_mel_spectrograms: DCT-II (unnormalised, x2) * rsqrt(2 M), first F coefficients.
-  const int F = h->features;
+  const int F = fe.features;
   std::vector<float> dct((size_t)M * F);
   for (int m = 0; m < M; ++m)
     for (int k = 0; k < F; ++k)
@@ -165,20 +169,20 @@ static int build_frontend_tables(tcr_handle* h) {
     auto pad4 = [&]() { while (blk.size() % 4) blk.push_back(0.f); };
     for (auto& v : tw) { blk.push_back(v.x); blk.push_back(v.y); }
     pad4();
-    h->c_melw = (int)blk.size();
+    fe.c_melw = (int)blk.size();
     blk.insert(blk.end(), wts.begin(), wts.end());
     pad4();
-    h->c_smem = (int)blk.size();                   // everything above is staged in shared memory
-    h->c_tw2 = (int)blk.size();
+    fe.c_smem = (int)blk.size();                   // everything above is staged in shared memory
+    fe.c_tw2 = (int)blk.size();
     for (auto& v : tw2) { blk.push_back(v.x); blk.push_back(v.y); }
     pad4();
-    h->c_win = (int)blk.size();
+    fe.c_win = (int)blk.size();
     blk.insert(blk.end(), win.begin(), win.end());
     pad4();
     if (fft == 1024 && M == 64) {
       // frame-pair kernel (tcr_mfcc_pair.cu), one contiguous section staged by a single TMA copy:
       //   W_512^(n2 k1), k1 < 16 rows of n2 < 32 | segment weights | DCT entries in lane order
-      h->c_twa = (int)blk.size();
+      fe.c_twa = (int)blk.size();
       for (int k1 = 0; k1 < 16; ++k1)
         for (int n2 = 0; n2 < 32; ++n2) {
           const double a = -2.0 * M_PI * (double)(n2 * k1) / 512.0;
@@ -217,51 +221,51 @@ static int build_frontend_tables(tcr_handle* h) {
         const int slot = j < 32 ? j : (j > 32 ? 32 + (64 - j) : 64);
         seg_meta[slot] = (first4 >> 2) | (groups << 8) | (off4 << 16);
       }
-      h->pair_segw_len = (int)blk.size() - segw0;
+      fe.pair_segw_len = (int)blk.size() - segw0;
       // DCT entries in the order the kernel's lanes use them: lane (q, g) = (lane / 8, lane % 8), rows q + 4 i, columns g + 8 j
       if (F == 40) {
         for (int i = 0; i < 8; ++i)
           for (int j = 0; j < 5; ++j)
             for (int lane = 0; lane < 32; ++lane) blk.push_back(dct[(size_t)((lane >> 3) + 4 * i) * F + (lane & 7) + 8 * j]);
-        h->pair_dct_len = 8 * 5 * 32;
+        fe.pair_dct_len = 8 * 5 * 32;
       }
       pad4();
-      TCR_TRY(dev_upload(h, &h->d_seg_meta, seg_meta));
+      TCR_TRY(dev_upload(fe, &fe.d_seg_meta, seg_meta));
     }
-    TCR_TRY(dev_upload(h, &h->d_fe_consts, blk));
+    TCR_TRY(dev_upload(fe, &fe.d_fe_consts, blk));
   }
-  TCR_TRY(dev_upload(h, &h->d_mel_start, start));
-  TCR_TRY(dev_upload(h, &h->d_mel_len, len));
-  TCR_TRY(dev_upload(h, &h->d_mel_off, off));
-  TCR_TRY(dev_upload(h, &h->d_dct, dct));
+  TCR_TRY(dev_upload(fe, &fe.d_mel_start, start));
+  TCR_TRY(dev_upload(fe, &fe.d_mel_len, len));
+  TCR_TRY(dev_upload(fe, &fe.d_mel_off, off));
+  TCR_TRY(dev_upload(fe, &fe.d_dct, dct));
   return TCR_OK;
 }
 
-MfccArgs tcr::mfcc_args(const tcr_handle* h, const void* wav, int pcm16, float* feat) {
+MfccArgs tcr::mfcc_args(const Frontend& fe, const void* wav, int pcm16, float* feat) {
   MfccArgs a;
   a.wav = wav;
   a.pcm16 = pcm16;
   a.feat = feat;
-  a.clip = h->cfg.clip_samples;
-  a.window = h->cfg.window_size_samples;
-  a.stride = h->cfg.window_stride_samples;
-  a.frames = h->frames;
-  a.features = h->features;
-  a.feat_stride = (int64_t)h->frames * h->features;
-  a.mel_bins = h->cfg.num_mel_bins;
-  a.fpb = h->fpb;
-  a.warps = h->fwarps;
-  a.magnitude = h->cfg.feature_kind == TCR_FEATURE_LOG_MEL;
-  a.use_dct = h->cfg.feature_kind == TCR_FEATURE_MFCC;
-  a.consts = h->d_fe_consts;
-  a.c_tw2 = h->c_tw2; a.c_melw = h->c_melw; a.c_win = h->c_win; a.c_smem = h->c_smem;
-  a.c_twa = h->c_twa;
-  a.seg_meta = h->d_seg_meta; a.segw_len = h->pair_segw_len; a.dct_len = h->pair_dct_len;
+  a.clip = fe.cfg.clip_samples;
+  a.window = fe.cfg.window_size_samples;
+  a.stride = fe.cfg.window_stride_samples;
+  a.frames = fe.frames;
+  a.features = fe.features;
+  a.feat_stride = (int64_t)fe.frames * fe.features;
+  a.mel_bins = fe.cfg.num_mel_bins;
+  a.fpb = fe.fpb;
+  a.warps = fe.fwarps;
+  a.magnitude = fe.cfg.feature_kind == TCR_FEATURE_LOG_MEL;
+  a.use_dct = fe.cfg.feature_kind == TCR_FEATURE_MFCC;
+  a.consts = fe.d_fe_consts;
+  a.c_tw2 = fe.c_tw2; a.c_melw = fe.c_melw; a.c_win = fe.c_win; a.c_smem = fe.c_smem;
+  a.c_twa = fe.c_twa;
+  a.seg_meta = fe.d_seg_meta; a.segw_len = fe.pair_segw_len; a.dct_len = fe.pair_dct_len;
   a.n_utts = 0;
-  a.mel_start = h->d_mel_start;
-  a.mel_len = h->d_mel_len;
-  a.mel_off = h->d_mel_off;
-  a.dct = h->d_dct;
+  a.mel_start = fe.d_mel_start;
+  a.mel_len = fe.d_mel_len;
+  a.mel_off = fe.d_mel_off;
+  a.dct = fe.d_dct;
   return a;
 }
 
@@ -304,7 +308,7 @@ static int build_plan(tcr_handle* h) {
       return fail(TCR_ERR_UNSUPPORTED, "channel count %d (width_multiplier %g) is not a positive multiple of 4", x,
                   c.width_multiplier);
   }
-  if (h->features % 4 != 0) return fail(TCR_ERR_UNSUPPORTED, "feature count %d is not a multiple of 4", h->features);
+  if (h->fe.features % 4 != 0) return fail(TCR_ERR_UNSUPPORTED, "feature count %d is not a multiple of 4", h->fe.features);
   auto mk = [&](const std::string& name, int cin, int cout, int k, int s, int t, int relu) {
     ConvPlan cv;
     cv.name = name;
@@ -318,7 +322,7 @@ static int build_plan(tcr_handle* h) {
     h->convs.push_back(cv);
     return (int)h->convs.size() - 1;
   };
-  mk("conv0", h->features, plan[0], 3, 1, h->frames, 1);
+  mk("conv0", h->fe.features, plan[0], 3, 1, h->fe.frames, 1);
   int ch = plan[0], t = h->convs[0].t_out;
   for (size_t i = 1; i < plan.size(); ++i) {
     const int n = plan[i];
@@ -381,10 +385,8 @@ static int build_plan(tcr_handle* h) {
   return TCR_OK;
 }
 
-extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
-  if (!cfg || !out) return fail(TCR_ERR_INVALID, "cfg/out is NULL");
-  *out = nullptr;
-  if (cfg->max_batch <= 0) return fail(TCR_ERR_INVALID, "max_batch must be positive");
+// The refusals of a front-end configuration, shared by tcr_create and tcr_dscnn_set_frontend.
+int tcr::frontend_check(const tcr_config* cfg) {
   if (cfg->window_size_samples <= 0 || cfg->window_stride_samples <= 0 || cfg->clip_samples < cfg->window_size_samples)
     return fail(TCR_ERR_INVALID, "bad window/stride/clip (%d/%d/%d)", cfg->window_size_samples,
                 cfg->window_stride_samples, cfg->clip_samples);
@@ -396,6 +398,62 @@ extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
     return fail(TCR_ERR_INVALID, "bad num_mel_bins/num_mfccs (%d/%d)", cfg->num_mel_bins, cfg->num_mfccs);
   if (cfg->feature_kind != TCR_FEATURE_MFCC && cfg->feature_kind != TCR_FEATURE_LOG_MEL)
     return fail(TCR_ERR_INVALID, "bad feature_kind %d", cfg->feature_kind);
+  return TCR_OK;
+}
+
+void tcr::frontend_geometry(const tcr_config& cfg, int* frames, int* features) {
+  *frames = 1 + (cfg.clip_samples - cfg.window_size_samples) / cfg.window_stride_samples;
+  *features = cfg.feature_kind == TCR_FEATURE_MFCC ? cfg.num_mfccs : cfg.num_mel_bins;
+}
+
+// Geometry, kernel choice and tables of a checked configuration, on the current device; the tables are fe->allocs.
+int tcr::frontend_init(Frontend* fe, const tcr_config* cfg, int sms) {
+  fe->cfg = *cfg;
+  fe->sms = sms;
+  frontend_geometry(*cfg, &fe->frames, &fe->features);
+  fe->fft = next_pow2(cfg->window_size_samples);
+  if (fe->fft < 128 || fe->fft > 2048) return fail(TCR_ERR_UNSUPPORTED, "fft length %d outside [128, 2048]", fe->fft);
+  // frames per CTA: a divisor-ish of T in [4, 8] so that chunks are balanced (49 -> 7, 98 -> 7)
+  fe->fpb = 8;
+  {
+    int best = 8, best_waste = 1 << 30;
+    for (int f = 8; f >= 4; --f) {
+      const int chunks = (fe->frames + f - 1) / f;
+      const int waste = chunks * f - fe->frames;
+      if (waste < best_waste) {
+        best_waste = waste;
+        best = f;
+      }
+    }
+    fe->fpb = std::min(best, fe->frames);
+  }
+  fe->fwarps = std::min(fe->fpb, 7);
+  if (const char* e = getenv("TCR_MFCC_FPB")) {                  // tuning knob: frames per CTA[,warps per CTA]
+    int f = 0, w = 0;
+    const int got = sscanf(e, "%d,%d", &f, &w);
+    if (got >= 1 && f >= 1) { fe->fpb = std::min(f, fe->frames); fe->fwarps = std::min(fe->fpb, 7); }
+    if (got >= 2 && w >= 1) fe->fwarps = std::min(std::min(w, 7), fe->fpb);
+  }
+  if (const char* e = getenv("TCR_MFCC_PAIR")) {                 // frame-pair kernel: 0 | 1 | frames per work item (even, <= 10)
+    int f = 0, w = 0;
+    const int got = sscanf(e, "%d,%d", &f, &w);
+    fe->mfcc_pair = got >= 1 && f >= 1;
+    if (got >= 1 && f >= 2) { fe->pair_fpb = std::min(f & ~1, 10); fe->pair_warps = fe->pair_fpb / 2; }   // one warp per frame pair
+    (void)w;
+  }
+  return build_frontend_tables(*fe);
+}
+
+void tcr::frontend_free(Frontend* fe) {
+  for (void* p : fe->allocs) cudaFree(p);
+  *fe = Frontend();
+}
+
+extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
+  if (!cfg || !out) return fail(TCR_ERR_INVALID, "cfg/out is NULL");
+  *out = nullptr;
+  if (cfg->max_batch <= 0) return fail(TCR_ERR_INVALID, "max_batch must be positive");
+  TCR_TRY(frontend_check(cfg));
   if (!(cfg->dropout_keep_prob > 0.f && cfg->dropout_keep_prob <= 1.f))
     return fail(TCR_ERR_INVALID, "dropout_keep_prob must be in (0,1]");
   if (cfg->num_classes <= 0 || cfg->num_classes > kMaxClasses)
@@ -410,39 +468,8 @@ extern "C" int tcr_create(const tcr_config* cfg, tcr_handle** out) {
 #ifndef TCR_EMU
   if (cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, cfg->device) != cudaSuccess || h->sms < 1) h->sms = 1;
 #endif
-  h->frames = 1 + (cfg->clip_samples - cfg->window_size_samples) / cfg->window_stride_samples;
-  h->features = cfg->feature_kind == TCR_FEATURE_MFCC ? cfg->num_mfccs : cfg->num_mel_bins;
-  h->fft = next_pow2(cfg->window_size_samples);
-  if (h->fft < 128 || h->fft > 2048) return bail(fail(TCR_ERR_UNSUPPORTED, "fft length %d outside [128, 2048]", h->fft));
-  // frames per CTA: a divisor-ish of T in [4, 8] so that chunks are balanced (49 -> 7, 98 -> 7)
-  h->fpb = 8;
-  {
-    int best = 8, best_waste = 1 << 30;
-    for (int f = 8; f >= 4; --f) {
-      const int chunks = (h->frames + f - 1) / f;
-      const int waste = chunks * f - h->frames;
-      if (waste < best_waste) {
-        best_waste = waste;
-        best = f;
-      }
-    }
-    h->fpb = std::min(best, h->frames);
-  }
-  h->fwarps = std::min(h->fpb, 7);
-  if (const char* e = getenv("TCR_MFCC_FPB")) {                  // tuning knob: frames per CTA[,warps per CTA]
-    int f = 0, w = 0;
-    const int got = sscanf(e, "%d,%d", &f, &w);
-    if (got >= 1 && f >= 1) { h->fpb = std::min(f, h->frames); h->fwarps = std::min(h->fpb, 7); }
-    if (got >= 2 && w >= 1) h->fwarps = std::min(std::min(w, 7), h->fpb);
-  }
-  if (const char* e = getenv("TCR_MFCC_PAIR")) {                 // frame-pair kernel: 0 | 1 | frames per work item (even, <= 10)
-    int f = 0, w = 0;
-    const int got = sscanf(e, "%d,%d", &f, &w);
-    h->mfcc_pair = got >= 1 && f >= 1;
-    if (got >= 1 && f >= 2) { h->pair_fpb = std::min(f & ~1, 10); h->pair_warps = h->pair_fpb / 2; }   // one warp per frame pair
-    (void)w;
-  }
-  int rc = build_frontend_tables(h);
+  int rc = frontend_init(&h->fe, cfg, h->sms);
+  h->workspace_bytes += h->fe.bytes;
   if (rc) return bail(rc);
   rc = build_plan(h);
   if (rc) return bail(rc);
@@ -462,6 +489,7 @@ extern "C" int tcr_destroy(tcr_handle* h) {
   frontend_ahead_destroy(h);
   resident_destroy(h);
   comm_destroy(h);
+  frontend_free(&h->fe);
   for (void* p : h->allocs) cudaFree(p);
   if (h->h_hyper) cudaFreeHost(h->h_hyper);
   delete h;
@@ -472,9 +500,9 @@ extern "C" int tcr_get_info(const tcr_handle* h, tcr_info* out) {
   if (!h || !out) return fail(TCR_ERR_INVALID, "NULL argument");
   memset(out, 0, sizeof(*out));
   out->abi_version = TCR_ABI_VERSION;
-  out->frames = h->frames;
-  out->features = h->features;
-  out->fft_length = h->fft;
+  out->frames = h->fe.frames;
+  out->features = h->fe.features;
+  out->fft_length = h->fe.fft;
   out->num_conv_layers = (int)h->convs.size();
   out->num_blocks = (int)h->blocks.size();
   out->last_channels = h->c_last;
@@ -526,26 +554,29 @@ static int check_n(const tcr_handle* h, int n) {
   return TCR_OK;
 }
 
+int tcr::frontend_run(const Frontend& fe, const void* wav, int pcm16, float* features, int n, cudaStream_t stream) {
+  if (((uintptr_t)wav & 15) != 0) return fail(TCR_ERR_INVALID, "wav must be 16-byte aligned (TMA bulk copy)");
+  if (pcm16 && (fe.cfg.window_size_samples % 8 || fe.cfg.window_stride_samples % 8 || fe.cfg.clip_samples % 8))
+    return fail(TCR_ERR_UNSUPPORTED, "int16 input needs window, stride and clip lengths that are multiples of 8 samples");
+  return mfcc_select_launch(fe, mfcc_args(fe, wav, pcm16, features), n, stream);
+}
 static int mfcc_run(tcr_handle* h, const void* wav, int pcm16, float* features, int32_t n, tcr_stream stream) {
   if (!h || !wav || !features) return fail(TCR_ERR_INVALID, "NULL argument");
   TCR_TRY(check_n(h, n));
-  if (((uintptr_t)wav & 15) != 0) return fail(TCR_ERR_INVALID, "wav must be 16-byte aligned (TMA bulk copy)");
-  if (pcm16 && (h->cfg.window_size_samples % 8 || h->cfg.window_stride_samples % 8 || h->cfg.clip_samples % 8))
-    return fail(TCR_ERR_UNSUPPORTED, "int16 input needs window, stride and clip lengths that are multiples of 8 samples");
-  return mfcc_select_launch(h, mfcc_args(h, wav, pcm16, features), n, (cudaStream_t)stream);
+  return frontend_run(h->fe, wav, pcm16, features, n, (cudaStream_t)stream);
 }
-int tcr::mfcc_select_launch(tcr_handle* h, const MfccArgs& a, int n, cudaStream_t stream) {
+int tcr::mfcc_select_launch(const Frontend& fe, const MfccArgs& a, int n, cudaStream_t stream) {
   bool launched = false;
-  if (h->mfcc_pair) {                                             // two frames per warp (tcr_mfcc_pair.cu) where the shape allows
+  if (fe.mfcc_pair) {                                             // two frames per warp (tcr_mfcc_pair.cu) where the shape allows
     MfccArgs b = a;
-    b.fpb = h->pair_fpb;
-    b.warps = h->pair_warps;
-    if (mfcc_pair_supported(b, h->fft)) {
-      if (mfcc_pair_launch(b, n, 3 * h->sms, stream) != 0) return fail(TCR_ERR_CUDA, "mfcc (frame pairs) launch configuration failed");
+    b.fpb = fe.pair_fpb;
+    b.warps = fe.pair_warps;
+    if (mfcc_pair_supported(b, fe.fft)) {
+      if (mfcc_pair_launch(b, n, 3 * fe.sms, stream) != 0) return fail(TCR_ERR_CUDA, "mfcc (frame pairs) launch configuration failed");
       launched = true;
     }
   }
-  if (!launched && mfcc_launch(a, n, h->fft, stream) != 0) return fail(TCR_ERR_CUDA, "mfcc launch configuration failed");
+  if (!launched && mfcc_launch(a, n, fe.fft, stream) != 0) return fail(TCR_ERR_CUDA, "mfcc launch configuration failed");
   TCR_CUDA(cudaGetLastError());
   return TCR_OK;
 }
@@ -662,9 +693,9 @@ static int frontend_ahead_get(tcr_handle* h) {
   TCR_CUDA(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, lo));
   for (int b = 0; b < 2; ++b) {      // its own two feature buffers: h->d_feat stays with the calls that are ordered on their stream
     void* p = nullptr;
-    TCR_CUDA(cudaMalloc(&p, (size_t)h->cfg.max_batch * h->frames * h->features * sizeof(float)));
+    TCR_CUDA(cudaMalloc(&p, (size_t)h->cfg.max_batch * h->fe.frames * h->fe.features * sizeof(float)));
     h->allocs.push_back(p);
-    h->workspace_bytes += (int64_t)h->cfg.max_batch * h->frames * h->features * (int64_t)sizeof(float);
+    h->workspace_bytes += (int64_t)h->cfg.max_batch * h->fe.frames * h->fe.features * (int64_t)sizeof(float);
     h->fe_feat[b] = (float*)p;
   }
   for (int b = 0; b < 2; ++b) {
@@ -883,7 +914,7 @@ static int hostfeed_get(tcr_handle* h, HostFeedState** out) {
     HostFeedState* f = new HostFeedState();
     h->hostfeed = f;
     TCR_CUDA(cudaStreamCreateWithFlags(&f->copy, cudaStreamNonBlocking));
-    const size_t in_bytes = (size_t)h->cfg.max_batch * std::max((size_t)h->cfg.clip_samples, (size_t)h->frames * h->features) * 4;
+    const size_t in_bytes = (size_t)h->cfg.max_batch * std::max((size_t)h->cfg.clip_samples, (size_t)h->fe.frames * h->fe.features) * 4;
     for (auto& s : f->slot) {
       TCR_CUDA(cudaMalloc(&s.d_in, in_bytes));
       TCR_CUDA(cudaMalloc((void**)&s.d_hot, (size_t)h->cfg.max_batch * h->cfg.num_classes * 4));
@@ -927,7 +958,7 @@ extern "C" int tcr_train_step_host(tcr_handle* h, const tcr_step_args* a, int32_
       if (stride > 2 * (int64_t)h->cfg.clip_samples) return fail(TCR_ERR_INVALID, "pcm_stride %lld exceeds 2 x clip_samples", (long long)stride);
       in_bytes = (size_t)a->n * stride * 2;
     } break;
-    case TCR_INPUT_FEATURES: in_bytes = (size_t)a->n * h->frames * h->features * 4; break;
+    case TCR_INPUT_FEATURES: in_bytes = (size_t)a->n * h->fe.frames * h->fe.features * 4; break;
     default: return fail(TCR_ERR_INVALID, "unknown input kind %d", a->input_is_features);
   }
   if (f->submitted >= kFeedDepth) TCR_CUDA(cudaStreamWaitEvent(f->copy, sl.consumed, 0));   // the slot's previous step has read it
@@ -969,7 +1000,7 @@ extern "C" int tcr_workspace_tensor(tcr_handle* h, const char* name, float** ptr
     return TCR_OK;
   };
   if (s == "timeline" && h->d_timeline) return ret((float*)h->d_timeline, 2 * 16 * 8192);   // int64 viewed as float pairs
-  if (s == "features") return ret(h->feat_last ? h->feat_last : h->d_feat, n * h->frames * h->features);
+  if (s == "features") return ret(h->feat_last ? h->feat_last : h->d_feat, n * h->fe.frames * h->fe.features);
   if (s == "grads") return ret(h->p2p.attached && h->world > 1 ? h->p2p.grads + (size_t)(h->p2p.step & 1u) * h->n_train : h->d_grads, h->n_train);
   if (s == "logits") return ret(h->d_logits, n * h->cfg.num_classes);
   if (s == "probs") return ret(h->d_probs, n * h->cfg.num_classes);

@@ -1,7 +1,9 @@
 // tcr_dscnn.cu — DS-CNN (Hello-Edge) forward pass for sm_90a: the reference's 2-D-conv comparison model
 // (audio_nets/ds_cnn.py:20-118, BASELINE.json config 5), inference mode.
 //
-//   dscnn_conv_kernel      first layer: kh x kw conv from the single-channel feature map (+bias, BN, ReLU)
+//   dscnn_conv_kernel      first layer: kh x kw conv from the single-channel feature map (+bias, BN, ReLU); like the wgmma
+//                          first-layer kernels it has a windowed instantiation (WIN = true) that reads utterance u in place from a
+//                          listener's feature history (WindowView, tcr_listener.cu) instead of from a [n, height, width] tensor
 //   dscnn_dsblock_kernel   depthwise 3x3 (+bias, BN, ReLU) -> pointwise 1x1 (+bias, BN, ReLU) fused per tile of output rows:
 //                          the input rows (+halo) and both filter banks are staged in shared memory, the depthwise result
 //                          never leaves the SM, the pointwise conv is a register-tiled 4 positions x 4 channels contraction
@@ -11,6 +13,7 @@
 #ifndef TCR_EMU
 #include <cuda.h>   // CUtensorMap (types only: the encoder is looked up through the runtime)
 #endif
+#include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -92,9 +95,16 @@ TCR_HD inline DsSmem dsblock_smem(const DsLayerDev& L, int RH, int COT) {
   return s;
 }
 
+// Utterance n of the first layer's windowed input: at in + (n / k) * stream + (n % k) * step floats, its height x width features
+// back to back.
+__device__ __forceinline__ const float* ds_window(const float* in, int n, const WindowView& win) {
+  return in + (int64_t)(n / win.k) * win.stream + (int64_t)(n % win.k) * win.step;
+}
+
 // ---- first layer: cin == 1 ----
+template <bool WIN>
 __global__ void __launch_bounds__(256) dscnn_conv_kernel(DsLayerDev L, const float* __restrict__ params, const float* __restrict__ in,
-                                                         float* __restrict__ out, float eps) {
+                                                         float* __restrict__ out, float eps, WindowView win) {
   pdl_wait();
   TCR_DYNAMIC_SMEM(smem_raw);
   float* smem = reinterpret_cast<float*>(smem_raw);
@@ -104,7 +114,8 @@ __global__ void __launch_bounds__(256) dscnn_conv_kernel(DsLayerDev L, const flo
   const int n = blockIdx.x, tid = threadIdx.x;
   for (int i = tid; i < hp * wp; i += blockDim.x) {
     const int h = i / wp - L.pt, w = i % wp - L.pl;
-    xs[i] = (h >= 0 && h < L.hin && w >= 0 && w < L.win) ? in[((size_t)n * L.hin + h) * L.win + w] : 0.f;
+    if constexpr (WIN) xs[i] = (h >= 0 && h < L.hin && w >= 0 && w < L.win) ? ds_window(in, n, win)[h * L.win + w] : 0.f;
+    else xs[i] = (h >= 0 && h < L.hin && w >= 0 && w < L.win) ? in[((size_t)n * L.hin + h) * L.win + w] : 0.f;
   }
   for (int i = tid; i < L.kh * L.kw * L.cout; i += blockDim.x) ws[i] = params[L.w + i];
   for (int c = tid; c < L.cout; c += blockDim.x) fold_bn(params, L.b, L.beta, L.mm, L.mv, c, eps, sc, sf);
@@ -439,10 +450,13 @@ struct Im2colWalk {
       g_a[j] = ((kc * kLbaFull + 4 * m) << 7) | m;
     }
   }
-  // input rows of the tile starting at output row h0 of utterance n -> xs [hin_t][wp]
-  __device__ __forceinline__ void fetch(const DsLayerDev& L, const float* in, int n, int h0, float* xs) const {
+  // input rows of the tile starting at output row h0 of utterance n -> xs [hin_t][wp]; WIN: utterance n is a window (ds_window)
+  template <bool WIN>
+  __device__ __forceinline__ void fetch(const DsLayerDev& L, const float* in, int n, int h0, float* xs, const WindowView& win) const {
     const int hb = h0 * L.sh - L.pt;
-    const float* base = in + ((int64_t)n * L.hin + hb) * L.win - L.pl;
+    const float* base;
+    if constexpr (WIN) base = ds_window(in, n, win) + (int64_t)hb * L.win - L.pl;
+    else base = in + ((int64_t)n * L.hin + hb) * L.win - L.pl;
 #pragma unroll
     for (int j = 0; j < kConvCells; ++j) {
       if (tid + j * NT < cells) {
@@ -758,9 +772,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_dsblock_ws_kernel(const _
 // First conv, warp-specialised (same roles and barriers as the block kernel): the producers copy the tile's input rows and
 // gather its im2col operand (Im2colWalk) into the A buffer of the tile, and refill the input buffer for the tile two ahead;
 // K = kh * kw (40).
-template <int CO>
+template <int CO, bool WIN>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
-                                                                      const float* __restrict__ in, float* __restrict__ out, float eps) {
+                                                                      const float* __restrict__ in, float* __restrict__ out, float eps,
+                                                                      WindowView win) {
   TCR_DYNAMIC_SMEM(smem_raw);
   __shared__ uint64_t in_full[2], a_full[2], mma_done[2];
   float* smem = reinterpret_cast<float*>(smem_raw);
@@ -788,7 +803,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
     const Im2colWalk<kWsProducers> walk(L, RH, tid);
     auto fetch_tile = [&](int tile, float* xs, uint64_t* bar) {
       const int n = tile / tpu;
-      walk.fetch(L, in, n, (tile - n * tpu) * RH, xs);
+      walk.fetch<WIN>(L, in, n, (tile - n * tpu) * RH, xs, win);
       cp_async_mbar_arrive(bar);
     };
     {
@@ -823,9 +838,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_ws_kernel(DsLayerDev
 // wgmma: the im2col operand (Im2colWalk) is gathered from the staged input rows straight into the canonical operand layout
 // (hi / lo), B = the filter bank [co][k], K = kh * kw (40), same persistent / quarter-per-warpgroup structure as the lock-step
 // block kernel above.
-template <int CO>
+template <int CO, bool WIN>
 __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev L, int RH, int n_utt, const float* __restrict__ params,
-                                                                      const float* __restrict__ in, float* __restrict__ out, float eps) {
+                                                                      const float* __restrict__ in, float* __restrict__ out, float eps,
+                                                                      WindowView win) {
   TCR_DYNAMIC_SMEM(smem_raw);
   float* smem = reinterpret_cast<float*>(smem_raw);
   const int tid = threadIdx.x;
@@ -841,7 +857,7 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev
   const Im2colWalk<kTcThreads> walk(L, RH, tid);
   auto fetch_tile = [&](int tile, float* xs) {
     const int n = tile / tpu;
-    walk.fetch(L, in, n, (tile - n * tpu) * RH, xs);
+    walk.fetch<WIN>(L, in, n, (tile - n * tpu) * RH, xs, win);
   };
   const TcQuarter<CO> q(tid, a_hi, a_lo, b_hi, b_lo);
   int tile = blockIdx.x, cur = 0;
@@ -937,6 +953,8 @@ struct tcr_dscnn {
   struct InMap { CUtensorMap map; const void* ptr = nullptr; int rh = 0; };
   std::vector<InMap> in_maps;   // per layer: TMA descriptor of the block's input activations (re-encoded if the buffer changes)
 #endif
+  Frontend fe;               // tcr_dscnn_set_frontend: the wav front-end in front of conv_1 (fe.frames == 0: none yet)
+  float* feat = nullptr;     // [max_batch, height, width]: the features of a wav-input forward
 };
 
 #ifndef TCR_EMU
@@ -1069,6 +1087,8 @@ extern "C" int tcr_dscnn_destroy(tcr_dscnn* d) {
   if (!d) return TCR_OK;
   for (int i = 0; i < 2; ++i)
     if (d->act[i]) cudaFree(d->act[i]);
+  frontend_free(&d->fe);
+  if (d->feat) cudaFree(d->feat);
   delete d;
   return TCR_OK;
 }
@@ -1090,41 +1110,54 @@ static int ds_tile_rows(const DsLayerDev& L) {
   return (L.hout + tiles - 1) / tiles;
 }
 
-// Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC).  The kernel is chosen here, once for both entry
-// points: wgmma where the layer's shape fits the tensor-core kernels (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.
-// The warp-specialised block kernel reads its input through a TMA map over max_batch utterances, so only from an activation
-// buffer of the handle.
-static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s) {
+// The first layer (cin == 1).  WIN: utterance u is the window `win` describes (tcr_listener.cu); the kernel choice is the same.
+template <bool WIN>
+static int ds_launch_conv(tcr_dscnn* d, const DsLayerDev& L, const float* params, const float* in, float* out, int32_t n, cudaStream_t s,
+                          WindowView win) {
+  const float eps = 1e-3f;
+#ifndef TCR_EMU
+  const int RHt = ds_tile_rows(L), grid = std::min(ds_tiles_per_utt(L, RHt) * n, d->sms);
+  // implicit GEMM on wgmma (3xTF32), where the kernel's per-thread im2col walk covers the tile
+  if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && im2col_walk_fits(L, RHt, kTcThreads)) {
+    const size_t smem_ws = conv_tc_smem<64>(L, RHt, 2).floats * 4;
+    if (d->tc_ws && smem_ws <= 220 * 1024 && im2col_walk_fits(L, RHt, kWsProducers) && (L.kh * L.kw / 4) % 2 == 0) {
+      auto kws = dscnn_conv_ws_kernel<64, WIN>;
+      static SmemOptIn optin_ws;
+      if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
+      TCR_LAUNCH(WIN ? "dscnn_conv_ws:win" : "dscnn_conv_ws", kws, dim3(grid), dim3(kTcThreads), smem_ws, s, L, RHt, n, params, in, out, eps,
+                 win);
+      return TCR_OK;
+    }
+    const size_t smem_tc = conv_tc_smem<64>(L, RHt, 1).floats * 4;
+    auto ktc = dscnn_conv_tc_kernel<64, WIN>;
+    static SmemOptIn optin_tc;
+    if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
+    TCR_LAUNCH(WIN ? "dscnn_conv_tc:win" : "dscnn_conv_tc", ktc, dim3(grid), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps,
+               win);
+    return TCR_OK;
+  }
+#endif
+  const size_t smem = conv_smem(L).floats * 4;
+  auto kfn = dscnn_conv_kernel<WIN>;
+#ifndef TCR_EMU
+  static SmemOptIn optin;
+  if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
+#endif
+  TCR_LAUNCH(WIN ? "dscnn_conv:win" : "dscnn_conv", kfn, dim3(n), dim3(256), smem, s, L, params, in, out, eps, win);
+  return TCR_OK;
+}
+
+// Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC), or for l == 0 with `win` the windows it describes.
+// The kernel is chosen here, once for every entry point: wgmma where the layer's shape fits the tensor-core kernels
+// (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.  The warp-specialised block kernel reads its input through a TMA map
+// over max_batch utterances, so only from an activation buffer of the handle.
+static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s,
+                           const WindowView* win = nullptr) {
   const DsLayerDev& L = d->net.layer[l];
   const float eps = 1e-3f;
   if (L.type == 0) {
-#ifndef TCR_EMU
-    const int RHt = ds_tile_rows(L), grid = std::min(ds_tiles_per_utt(L, RHt) * n, d->sms);
-    // implicit GEMM on wgmma (3xTF32), where the kernel's per-thread im2col walk covers the tile
-    if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && im2col_walk_fits(L, RHt, kTcThreads)) {
-      const size_t smem_ws = conv_tc_smem<64>(L, RHt, 2).floats * 4;
-      if (d->tc_ws && smem_ws <= 220 * 1024 && im2col_walk_fits(L, RHt, kWsProducers) && (L.kh * L.kw / 4) % 2 == 0) {
-        auto kws = dscnn_conv_ws_kernel<64>;
-        static SmemOptIn optin_ws;
-        if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
-        TCR_LAUNCH("dscnn_conv_ws", kws, dim3(grid), dim3(kTcThreads), smem_ws, s, L, RHt, n, params, in, out, eps);
-        return TCR_OK;
-      }
-      const size_t smem_tc = conv_tc_smem<64>(L, RHt, 1).floats * 4;
-      auto ktc = dscnn_conv_tc_kernel<64>;
-      static SmemOptIn optin_tc;
-      if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-      TCR_LAUNCH("dscnn_conv_tc", ktc, dim3(grid), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
-      return TCR_OK;
-    }
-#endif
-    const size_t smem = conv_smem(L).floats * 4;
-    auto kfn = dscnn_conv_kernel;
-#ifndef TCR_EMU
-    static SmemOptIn optin;
-    if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
-#endif
-    TCR_LAUNCH("dscnn_conv", kfn, dim3(n), dim3(256), smem, s, L, params, in, out, eps);
+    if (win) return ds_launch_conv<true>(d, L, params, in, out, n, s, *win);
+    return ds_launch_conv<false>(d, L, params, in, out, n, s, WindowView{0, 0, 0});
   } else {
 #ifndef TCR_EMU
     // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
@@ -1181,16 +1214,12 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
   return TCR_OK;
 }
 
-extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const float* params, int32_t n, float* logits, float* probs,
-                                 tcr_stream stream) {
-  pdl_chain_reset();
-  if (!d || !features || !params) { set_error("NULL argument"); return TCR_ERR_INVALID; }
-  if (n <= 0 || n > d->cfg.max_batch) { set_error("n outside [1, max_batch]"); return TCR_ERR_INVALID; }
-  cudaStream_t s = (cudaStream_t)stream;
-  const float* in = features;
+int tcr::dscnn_forward(tcr_dscnn* d, const float* feat, const float* params, int n, float* logits, float* probs, cudaStream_t s,
+                       const WindowView* win) {
+  const float* in = feat;
   for (int l = 0; l < d->net.nlayers; ++l) {
     float* out = d->act[l & 1];
-    const int rc = ds_launch_layer(d, l, params, in, out, n, s);
+    const int rc = ds_launch_layer(d, l, params, in, out, n, s, l == 0 ? win : nullptr);
     if (rc != TCR_OK) return rc;
     in = out;
   }
@@ -1199,6 +1228,88 @@ extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const floa
   TCR_LAUNCH("dscnn_head", dscnn_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes, d->net.fcw,
              d->net.fcb, params, in, logits, probs);
   if (cudaGetLastError() != cudaSuccess) { set_error("DS-CNN launch failed"); return TCR_ERR_CUDA; }
+  return TCR_OK;
+}
+const Frontend* tcr::dscnn_frontend(const tcr_dscnn* d) { return d->fe.frames ? &d->fe : nullptr; }
+int tcr::dscnn_max_batch(const tcr_dscnn* d) { return d->cfg.max_batch; }
+
+extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const float* params, int32_t n, float* logits, float* probs,
+                                 tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !features || !params) { set_error("NULL argument"); return TCR_ERR_INVALID; }
+  if (n <= 0 || n > d->cfg.max_batch) { set_error("n outside [1, max_batch]"); return TCR_ERR_INVALID; }
+  return dscnn_forward(d, features, params, n, logits, probs, (cudaStream_t)stream, nullptr);
+}
+
+static int ds_fail(int code, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  set_error(buf);
+  return code;
+}
+
+extern "C" int tcr_dscnn_set_frontend(tcr_dscnn* d, const tcr_config* cfg) {
+  pdl_chain_reset();
+  if (!d || !cfg) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  int rc = frontend_check(cfg);
+  if (rc) return rc;
+  int T = 0, F = 0;
+  frontend_geometry(*cfg, &T, &F);
+  if (T != d->cfg.height || F != d->cfg.width)
+    return ds_fail(TCR_ERR_INVALID, "the front-end gives (T, F) = (%d, %d) features, the DS-CNN handle takes (height, width) = (%d, %d)",
+                   T, F, d->cfg.height, d->cfg.width);
+  if (cudaSetDevice(d->cfg.device) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "cudaSetDevice(%d) failed", d->cfg.device);
+  if (d->feat || d->fe.frames) {
+    cudaDeviceSynchronize();                                      // no queued forward may still read the old tables
+    frontend_free(&d->fe);
+    cudaFree(d->feat);
+    d->feat = nullptr;
+  }
+  tcr_config c = *cfg;
+  c.device = d->cfg.device;
+  c.max_batch = d->cfg.max_batch;
+  rc = frontend_init(&d->fe, &c, d->sms);
+  if (!rc && cudaMalloc((void**)&d->feat, (size_t)d->cfg.max_batch * T * F * sizeof(float)) != cudaSuccess)
+    rc = ds_fail(TCR_ERR_CUDA, "cudaMalloc failed for the DS-CNN feature buffer");
+  if (rc) frontend_free(&d->fe);
+  return rc;
+}
+
+extern "C" int tcr_dscnn_mfcc_forward(tcr_dscnn* d, const void* wav, int32_t input_kind, float* features, int32_t n, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !wav || !features) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  if (n <= 0 || n > d->cfg.max_batch) return ds_fail(TCR_ERR_INVALID, "n outside [1, max_batch]");
+  if (input_kind != TCR_INPUT_WAV_F32 && input_kind != TCR_INPUT_WAV_PCM16)
+    return ds_fail(TCR_ERR_INVALID, "input_kind %d: the front-end takes TCR_INPUT_WAV_F32 or TCR_INPUT_WAV_PCM16", input_kind);
+  if (!d->fe.frames) return ds_fail(TCR_ERR_INVALID, "the DS-CNN handle has no front-end (call tcr_dscnn_set_frontend first)");
+  return frontend_run(d->fe, wav, input_kind == TCR_INPUT_WAV_PCM16, features, n, (cudaStream_t)stream);
+}
+
+extern "C" int tcr_dscnn_forward_input(tcr_dscnn* d, const void* input, int32_t input_kind, const float* params, int32_t n, float* logits,
+                                       float* probs, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !input || !params) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  if (n <= 0 || n > d->cfg.max_batch) return ds_fail(TCR_ERR_INVALID, "n outside [1, max_batch]");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (input_kind == TCR_INPUT_FEATURES) return dscnn_forward(d, static_cast<const float*>(input), params, n, logits, probs, s, nullptr);
+  if (input_kind != TCR_INPUT_WAV_F32 && input_kind != TCR_INPUT_WAV_PCM16) return ds_fail(TCR_ERR_INVALID, "unknown input kind %d", input_kind);
+  if (!d->fe.frames) return ds_fail(TCR_ERR_INVALID, "the DS-CNN handle has no front-end (call tcr_dscnn_set_frontend first)");
+  const int rc = frontend_run(d->fe, input, input_kind == TCR_INPUT_WAV_PCM16, d->feat, n, s);
+  if (rc) return rc;
+  return dscnn_forward(d, d->feat, params, n, logits, probs, s, nullptr);
+}
+
+extern "C" int tcr_dscnn_eval_accumulate(tcr_dscnn* d, const float* scores, const float* onehot, int32_t n, int32_t topk, int64_t* counts,
+                                         tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !scores || !onehot || !counts) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  if (n <= 0) return ds_fail(TCR_ERR_INVALID, "n must be positive (got %d)", n);
+  if (topk < 1) return ds_fail(TCR_ERR_INVALID, "topk must be at least 1");
+  eval_accumulate_launch(scores, onehot, n, d->cfg.num_classes, topk, counts, (cudaStream_t)stream);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "eval_accumulate launch failed");
   return TCR_OK;
 }
 

@@ -8,8 +8,9 @@
 //   mfcc            the K * hop new frames of every stream, written straight into the history behind the carried frames,
 //                   by the kernel tcr_mfcc_forward selects for the handle (frame pairs or one frame per warp), so the features
 //                   are bit-identical to the per-clip front-end's;
-//   fwd:* / head    the evaluation forward at n = S * K, conv0 reading window u of the batch in place from the history at
-//                   (u / K) * stream + (u % K) * hop * F (conv_fwd_kernel<3, WSMEM, true>);
+//   forward         the evaluation forward of the listener's model at n = S * K, its first layer reading window u of the batch in
+//                   place from the history at (u / K) * stream + (u % K) * hop * F: TC-ResNet's conv0 (conv_fwd_kernel<3, WSMEM,
+//                   true>) or DS-CNN's conv_1 (the windowed dscnn_conv* instantiations, tcr_dscnn.cu);
 //   listener_roll   the last tail samples and the last carried frames of each stream to the front of their buffers.
 // A reset zeroes the sample rows and fills the carried frames with the features of a silent frame (one front-end launch over
 // one frame, and listener_reset to copy it): the stream then holds exactly what pushing pre = carried * s + tail zeros would
@@ -23,8 +24,12 @@
 
 using namespace tcr;
 
+// A listener serves one model: a TC-ResNet handle (h) or a DS-CNN handle (d).  Everything but the forward call goes through the
+// model's front-end (fe).
 struct tcr_listener {
   tcr_handle* h = nullptr;
+  tcr_dscnn* d = nullptr;
+  const tcr::Frontend* fe = nullptr;
   int S = 0, hop = 0, chunk = 0, K = 0;
   int tail = 0;                // W_s - s samples carried to the next push
   int row = 0;                 // samples per stream row: tail + chunk
@@ -70,10 +75,11 @@ __global__ void __launch_bounds__(kListenThreads) listener_stage_kernel(const vo
 
 // base[i] = base[i + shift] for i < n (float4 units, shift > 0), in place: the CTA walks blocks of blockDim.x in ascending order
 // and reads a whole block before writing it, so every read happens before the write of its address.
-__device__ __forceinline__ void move_down(float4* base, int64_t shift, int64_t n) {
+template <class V>
+__device__ __forceinline__ void move_down(V* base, int64_t shift, int64_t n) {
   for (int64_t b = 0; b < n; b += blockDim.x) {
     const int64_t i = b + threadIdx.x;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    V v = {};
     if (i < n) v = base[i + shift];
     __syncthreads();
     if (i < n) base[i] = v;
@@ -81,13 +87,17 @@ __device__ __forceinline__ void move_down(float4* base, int64_t shift, int64_t n
   }
 }
 
-// blockIdx.x = stream; y = 0: the sample tail, y = 1: the carried feature frames
+// blockIdx.x = stream; y = 0: the sample tail, y = 1: the carried feature frames.  The history moves in float4 units when every
+// stream row, shift and carried length is a multiple of four floats (F % 4 == 0, every TC-ResNet front-end); in floats otherwise
+// (e.g. DS-CNN's 10 MFCCs).
+template <class V>
 __global__ void __launch_bounds__(kListenThreads) listener_roll_kernel(float* samples, float* hist, int row, int chunk, int tail,
                                                                        int64_t hist_stride, int64_t hist_shift, int64_t carry) {
   pdl_wait();
   const int s = blockIdx.x;
+  constexpr int kV = sizeof(V) / sizeof(float);
   if (blockIdx.y == 0) move_down(reinterpret_cast<float4*>(samples + (size_t)s * row), chunk / 4, tail / 4);
-  else move_down(reinterpret_cast<float4*>(hist + (size_t)s * hist_stride), hist_shift / 4, carry / 4);
+  else move_down(reinterpret_cast<V*>(hist + (size_t)s * hist_stride), hist_shift / kV, carry / kV);
 }
 
 // frames 1 .. carried - 1 of streams first + blockIdx.y = frame 0 (the features of a silent frame)
@@ -101,13 +111,12 @@ __global__ void __launch_bounds__(kListenThreads) listener_reset_kernel(float* h
 
 // Front-end over `frames` frames of rows [first, first + count): samples rows -> history frame `frame0` onwards.
 int listener_frontend(tcr_listener* L, int first, int count, int frames, int frame0, cudaStream_t st) {
-  tcr_handle* h = L->h;
-  MfccArgs a = mfcc_args(h, L->samples + (size_t)first * L->row, 0,
-                         L->hist + (size_t)first * L->hist_stride + (size_t)frame0 * h->features);
+  MfccArgs a = mfcc_args(*L->fe, L->samples + (size_t)first * L->row, 0,
+                         L->hist + (size_t)first * L->hist_stride + (size_t)frame0 * L->fe->features);
   a.clip = L->row;
   a.frames = frames;
   a.feat_stride = L->hist_stride;
-  return mfcc_select_launch(h, a, count, st);
+  return mfcc_select_launch(*L->fe, a, count, st);
 }
 
 int listener_reset_rows(tcr_listener* L, int first, int count, cudaStream_t st) {
@@ -117,11 +126,11 @@ int listener_reset_rows(tcr_listener* L, int first, int count, cudaStream_t st) 
   int rc = listener_frontend(L, first, count, 1, 0, st);
   if (rc) return rc;
   if (L->carried > 1) {
-    const int n = (L->carried - 1) * L->h->features;
+    const int n = (L->carried - 1) * L->fe->features;
     for (int f = first; f < first + count; f += kMaxGridRows) {      // one stream per blockIdx.y
       const int rows = std::min(first + count - f, kMaxGridRows);
       TCR_LAUNCH("listener_reset", listener_reset_kernel, dim3((n + kListenThreads - 1) / kListenThreads, rows), dim3(kListenThreads), 0, st,
-                 L->hist, L->hist_stride, f, L->carried, L->h->features);
+                 L->hist, L->hist_stride, f, L->carried, L->fe->features);
       if (cudaGetLastError() != cudaSuccess) return lfail(TCR_ERR_CUDA, "listener reset launch failed");
     }
   }
@@ -145,29 +154,29 @@ int listener_stage(tcr_listener* L, const void* samples, bool pcm, cudaStream_t 
 }  // namespace
 }  // namespace tcr
 
-extern "C" int tcr_listener_create(tcr_handle* h, const tcr_listener_config* cfg, tcr_listener** out) {
-  pdl_chain_reset();
-  if (!h || !cfg || !out) return lfail(TCR_ERR_INVALID, "NULL argument");
-  *out = nullptr;
-  const int T = h->frames, W = h->cfg.window_size_samples, s = h->cfg.window_stride_samples;
-  if (cfg->streams < 1) return lfail(TCR_ERR_INVALID, "streams must be at least 1 (got %d)", cfg->streams);
+// Shared by both handle types: L->h or L->d and L->fe are set; max_batch and device are the model handle's.
+static int listener_create(tcr_listener* L, const tcr_listener_config* cfg, int max_batch, int device, tcr_listener** out) {
+  const int T = L->fe->frames, W = L->fe->cfg.window_size_samples, s = L->fe->cfg.window_stride_samples;
+  auto refuse = [&](int rc) {
+    delete L;
+    return rc;
+  };
+  if (cfg->streams < 1) return refuse(lfail(TCR_ERR_INVALID, "streams must be at least 1 (got %d)", cfg->streams));
   if (cfg->hop_frames < 1 || cfg->hop_frames > T)
-    return lfail(TCR_ERR_INVALID, "hop_frames %d outside [1, T = %d]", cfg->hop_frames, T);
+    return refuse(lfail(TCR_ERR_INVALID, "hop_frames %d outside [1, T = %d]", cfg->hop_frames, T));
   const int64_t step = (int64_t)cfg->hop_frames * s;
   if (cfg->chunk_samples <= 0 || cfg->chunk_samples % step)
-    return lfail(TCR_ERR_INVALID, "chunk_samples %d is not a positive multiple of hop_frames * window_stride_samples = %lld",
-                 cfg->chunk_samples, (long long)step);
+    return refuse(lfail(TCR_ERR_INVALID, "chunk_samples %d is not a positive multiple of hop_frames * window_stride_samples = %lld",
+                        cfg->chunk_samples, (long long)step));
   const int K = (int)(cfg->chunk_samples / step);
-  if ((int64_t)cfg->streams * K > h->cfg.max_batch)
-    return lfail(TCR_ERR_INVALID, "streams * windows per push = %d * %d exceeds max_batch = %d", cfg->streams, K, h->cfg.max_batch);
-  tcr_listener* L = new tcr_listener();
-  L->h = h;
+  if ((int64_t)cfg->streams * K > max_batch)
+    return refuse(lfail(TCR_ERR_INVALID, "streams * windows per push = %d * %d exceeds max_batch = %d", cfg->streams, K, max_batch));
   L->S = cfg->streams; L->hop = cfg->hop_frames; L->chunk = cfg->chunk_samples; L->K = K;
   L->tail = W - s;
   L->row = L->tail + L->chunk;
   L->carried = T - L->hop;
-  L->hist_stride = (int64_t)(L->carried + K * L->hop) * h->features;
-  if (cudaSetDevice(h->cfg.device) != cudaSuccess ||
+  L->hist_stride = (int64_t)(L->carried + K * L->hop) * L->fe->features;
+  if (cudaSetDevice(device) != cudaSuccess ||
       cudaMalloc((void**)&L->samples, (size_t)L->S * L->row * sizeof(float)) != cudaSuccess ||
       cudaMalloc((void**)&L->hist, (size_t)L->S * L->hist_stride * sizeof(float)) != cudaSuccess) {
     tcr_listener_destroy(L);
@@ -183,6 +192,27 @@ extern "C" int tcr_listener_create(tcr_handle* h, const tcr_listener_config* cfg
   return TCR_OK;
 }
 
+extern "C" int tcr_listener_create(tcr_handle* h, const tcr_listener_config* cfg, tcr_listener** out) {
+  pdl_chain_reset();
+  if (!h || !cfg || !out) return lfail(TCR_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  tcr_listener* L = new tcr_listener();
+  L->h = h;
+  L->fe = &h->fe;
+  return listener_create(L, cfg, h->cfg.max_batch, h->cfg.device, out);
+}
+
+extern "C" int tcr_dscnn_listener_create(tcr_dscnn* d, const tcr_listener_config* cfg, tcr_listener** out) {
+  pdl_chain_reset();
+  if (!d || !cfg || !out) return lfail(TCR_ERR_INVALID, "NULL argument");
+  *out = nullptr;
+  if (!dscnn_frontend(d)) return lfail(TCR_ERR_INVALID, "the DS-CNN handle has no front-end (call tcr_dscnn_set_frontend first)");
+  tcr_listener* L = new tcr_listener();
+  L->d = d;
+  L->fe = dscnn_frontend(d);
+  return listener_create(L, cfg, dscnn_max_batch(d), dscnn_frontend(d)->cfg.device, out);
+}
+
 extern "C" int tcr_listener_reset(tcr_listener* L, int32_t stream, tcr_stream stream_) {
   pdl_chain_reset();
   if (!L) return lfail(TCR_ERR_INVALID, "NULL listener");
@@ -193,28 +223,33 @@ extern "C" int tcr_listener_reset(tcr_listener* L, int32_t stream, tcr_stream st
 extern "C" int tcr_listener_push(tcr_listener* L, const void* samples, int32_t input_kind, const float* params, const float* moving,
                                  float* logits, float* probs, tcr_stream stream_) {
   pdl_chain_reset();
-  if (!L || !samples || !params || !moving) return lfail(TCR_ERR_INVALID, "NULL argument (listener, samples, params and moving are required)");
+  if (!L || !samples || !params || (L->h && !moving))
+    return lfail(TCR_ERR_INVALID, "NULL argument (listener, samples, params and, for TC-ResNet, moving are required)");
+  if (L->d && moving) return lfail(TCR_ERR_INVALID, "a DS-CNN listener takes moving = NULL: its moving statistics are in params");
   if (input_kind != TCR_INPUT_WAV_F32 && input_kind != TCR_INPUT_WAV_PCM16)
     return lfail(TCR_ERR_INVALID, "input_kind %d: a listener takes TCR_INPUT_WAV_F32 or TCR_INPUT_WAV_PCM16", input_kind);
   if (((uintptr_t)samples & 15) != 0) return lfail(TCR_ERR_INVALID, "samples must be 16-byte aligned");
-  tcr_handle* h = L->h;
+  const Frontend& fe = *L->fe;
   const bool pcm = input_kind == TCR_INPUT_WAV_PCM16;
-  if (pcm && (h->cfg.window_size_samples % 8 || h->cfg.window_stride_samples % 8 || L->chunk % 8))
+  if (pcm && (fe.cfg.window_size_samples % 8 || fe.cfg.window_stride_samples % 8 || L->chunk % 8))
     return lfail(TCR_ERR_UNSUPPORTED, "int16 input needs window, stride and chunk lengths that are multiples of 8 samples");
   cudaStream_t st = (cudaStream_t)stream_;
   int rc = listener_stage(L, samples, pcm, st);
   if (rc) return rc;
   rc = listener_frontend(L, 0, L->S, L->K * L->hop, L->carried, st);
   if (rc) return rc;
-  const WindowView win{L->K, L->hist_stride, (int64_t)L->hop * h->features};
-  rc = net_forward(h, L->hist, params, moving, L->S * L->K, false, 0, nullptr, nullptr, 0.f, logits, probs, nullptr, false, st, &win);
+  const WindowView win{L->K, L->hist_stride, (int64_t)L->hop * fe.features};
+  rc = L->h ? net_forward(L->h, L->hist, params, moving, L->S * L->K, false, 0, nullptr, nullptr, 0.f, logits, probs, nullptr, false, st, &win)
+            : dscnn_forward(L->d, L->hist, params, L->S * L->K, logits, probs, st, &win);
   if (rc) {
     char inner[512];
     snprintf(inner, sizeof(inner), "%s", tcr_last_error());
     return lfail(rc, "listener forward launch failed: %s", inner);
   }
-  TCR_LAUNCH("listener_roll", listener_roll_kernel, dim3(L->S, 2), dim3(kListenThreads), 0, st, L->samples, L->hist, L->row, L->chunk,
-             L->tail, L->hist_stride, (int64_t)L->K * L->hop * h->features, (int64_t)L->carried * h->features);
+  const int64_t shift = (int64_t)L->K * L->hop * fe.features, carry = (int64_t)L->carried * fe.features;
+  auto roll = (L->hist_stride % 4 || shift % 4 || carry % 4) ? listener_roll_kernel<float> : listener_roll_kernel<float4>;
+  TCR_LAUNCH("listener_roll", roll, dim3(L->S, 2), dim3(kListenThreads), 0, st, L->samples, L->hist, L->row, L->chunk, L->tail,
+             L->hist_stride, shift, carry);
   if (cudaGetLastError() != cudaSuccess) return lfail(TCR_ERR_CUDA, "listener launch failed");
   return TCR_OK;
 }

@@ -1,8 +1,27 @@
-// tcr_mfcc.h — argument block and launcher of the fused front-end kernel (tcr_mfcc.cu).
+// tcr_mfcc.h — argument block and launcher of the fused front-end kernel (tcr_mfcc.cu), and the front-end a handle owns.
 #pragma once
+#include <vector>
+
 #include "tcr_device.cuh"
+#include "../../include/tcr_b200.h"
 
 namespace tcr {
+
+// One front-end geometry and its constant tables (Hann window, twiddles, packed mel weights, DCT) and kernel choice, built by
+// frontend_init (tcr_api.cu) from the front-end fields of a tcr_config.  A TC-ResNet handle owns one; a DS-CNN handle owns one
+// once tcr_dscnn_set_frontend has been called.  mfcc_args / mfcc_select_launch (tcr_net.h) run it.
+struct Frontend {
+  tcr_config cfg = {};             // only the front-end fields are read: sample rate, clip, window, stride, mel bins, MFCCs, edges, kind
+  int frames = 0, features = 0, fft = 0, fpb = 1, fwarps = 1;
+  int mfcc_pair = 1, pair_fpb = 10, pair_warps = 5, c_twa = -1, pair_segw_len = 0, pair_dct_len = 0;
+  int sms = 1;                     // multiprocessors of the device: the frame-pair kernel's persistent grid
+  int* d_seg_meta = nullptr;       // frame-pair front-end kernel (tcr_mfcc_pair.cu)
+  float* d_fe_consts = nullptr; int c_tw2 = 0, c_melw = 0, c_win = 0, c_smem = 0;   // front-end constant block (MfccArgs)
+  int* d_mel_start = nullptr; int* d_mel_len = nullptr; int* d_mel_off = nullptr;
+  float* d_dct = nullptr;
+  std::vector<void*> allocs;       // the device tables above
+  int64_t bytes = 0;
+};
 
 struct MfccArgs {
   const void* wav;          // [N, clip] fp32 samples, or int16 PCM when pcm16 != 0 (clip: the row stride in samples)

@@ -9,17 +9,31 @@ void set_error(const char* msg);
 
 int net_alloc_workspace(tcr_handle* h);
 
-// Front-end (tcr_api.cu): the handle's arguments for `wav` -> `feat` (per-clip geometry), and the launch of the kernel the
-// handle selects for them (the frame-pair kernel where the shape allows and TCR_MFCC_PAIR does not turn it off).
-MfccArgs mfcc_args(const tcr_handle* h, const void* wav, int pcm16, float* feat);
-int mfcc_select_launch(tcr_handle* h, const MfccArgs& a, int n, cudaStream_t stream);
+// Front-end (tcr_api.cu), the same for every handle type that owns a Frontend: the refusals of a configuration's front-end
+// fields, its (T, F), building and freeing the tables, the arguments for `wav` -> `feat` (per-clip geometry), and the launch of
+// the kernel the front-end selects for them (the frame-pair kernel where the shape allows and TCR_MFCC_PAIR does not turn it off).
+int frontend_check(const tcr_config* cfg);
+void frontend_geometry(const tcr_config& cfg, int* frames, int* features);
+int frontend_init(Frontend* fe, const tcr_config* cfg, int sms);
+void frontend_free(Frontend* fe);
+MfccArgs mfcc_args(const Frontend& fe, const void* wav, int pcm16, float* feat);
+int mfcc_select_launch(const Frontend& fe, const MfccArgs& a, int n, cudaStream_t stream);
+// wav (16-byte aligned; int16 needs window, stride and clip lengths that are multiples of 8) -> features [n, T, F]
+int frontend_run(const Frontend& fe, const void* wav, int pcm16, float* features, int n, cudaStream_t stream);
 
-// conv0 reading its utterances as windows of a listener's feature history (tcr_listener.cu) instead of a [n, T, F] tensor:
-// utterance u starts at feat + (u / k) * stream + (u % k) * step floats.
+// The first layer reading its utterances as windows of a listener's feature history (tcr_listener.cu) instead of a [n, T, F]
+// tensor: utterance u starts at feat + (u / k) * stream + (u % k) * step floats (TC-ResNet conv0, DS-CNN conv_1).
 struct WindowView {
   int k;
   int64_t stream, step;
 };
+
+// DS-CNN (tcr_dscnn.cu) as the listener sees it: its front-end (nullptr before tcr_dscnn_set_frontend), max_batch, and the
+// evaluation forward on features [n, height, width] or on the windows `win` describes.
+const Frontend* dscnn_frontend(const tcr_dscnn* d);
+int dscnn_max_batch(const tcr_dscnn* d);
+int dscnn_forward(tcr_dscnn* d, const float* feat, const float* params, int n, float* logits, float* probs, cudaStream_t s,
+                  const WindowView* win);
 
 // Forward pass on features [n, T, F] (or the windows `win` describes).  training: batch-statistics BN (+ dropout); otherwise
 // the BN tables are built from `moving`.  backward: the head additionally emits dlogits-derived tensors for the backward pass.

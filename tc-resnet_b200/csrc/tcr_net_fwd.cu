@@ -424,7 +424,7 @@ int net_alloc_workspace(tcr_handle* h) {
   h->smem_optin = smem_optin_limit(h);
   plan_bwd_weight(h);
   WS(net_check_envelope(h));
-  WS(ws_alloc(h, &h->d_feat, N * h->frames * h->features));
+  WS(ws_alloc(h, &h->d_feat, N * h->fe.frames * h->fe.features));
   WS(ws_alloc(h, &h->d_logits, N * h->cfg.num_classes));
   WS(ws_alloc(h, &h->d_probs, N * h->cfg.num_classes));
   for (auto& cv : h->convs) {

@@ -43,9 +43,8 @@ struct BlockPlan {
 
 struct tcr_handle {
   tcr_config cfg;
-  int frames = 0, features = 0, fft = 0, fpb = 1, fwarps = 1;
-  int mfcc_pair = 1, pair_fpb = 10, pair_warps = 5, c_twa = -1, sms = 1, pair_segw_len = 0, pair_dct_len = 0;
-  int* d_seg_meta = nullptr;   // frame-pair front-end kernel (tcr_mfcc_pair.cu)
+  tcr::Frontend fe;            // the front-end: geometry (frames T, features F), tables and kernel choice
+  int sms = 1;
   std::string scope;
   std::vector<tcr::ConvPlan> convs;
   std::vector<tcr::BlockPlan> blocks;
@@ -55,10 +54,6 @@ struct tcr_handle {
   int g_max = 0;                 // max CTA groups of any producer kernel (partials are sized for it)
   size_t smem_optin = 0;         // dynamic shared memory one CTA may opt in to (net_alloc_workspace)
   int head_groups_max = 0;
-  // front-end tables
-  float* d_fe_consts = nullptr; int c_tw2 = 0, c_melw = 0, c_win = 0, c_smem = 0;   // front-end constant block (tcr_mfcc.h)
-  int* d_mel_start = nullptr; int* d_mel_len = nullptr; int* d_mel_off = nullptr;
-  float* d_dct = nullptr;
   // workspace
   float* d_feat = nullptr;
   // front-end running ahead on its own stream (tcr_step_args::input_resident, tcr_train_step_host): two feature buffers, the

@@ -1,18 +1,24 @@
 """DS-CNN forward (inference) on the CUDA path: the reference's 2-D-conv comparison model
-(audio_nets/ds_cnn.py; DSCNN{S,M}Model.build_inference in factory/audio_nets.py:298-358).  Training DS-CNN is out of scope
-(SURVEY.md 2 #13): weights come from a checkpoint keyed by the TF variable names in `self.table`."""
+(audio_nets/ds_cnn.py; DSCNN{S,M,L}Model.build_inference in factory/audio_nets.py:298-358).  Training DS-CNN is out of scope
+(SURVEY.md 2 #13): weights come from a checkpoint keyed by the TF variable names in `self.table`.
+
+With a front-end (set_frontend) the handle also takes audio: `mfcc`, `forward_input`, `eval_accumulate` and `listener` mirror
+Engine.mfcc / Engine.forward / Engine.eval_accumulate / Engine.listener (include/tcr_b200.h, tcr_dscnn_set_frontend ff.)."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict
+from typing import Dict, Optional
 
 import numpy as np
 import torch
 
 from . import _lib as L
+from .engine import Listener, frontend_config, frontend_shape
 
 
 class DsCnn:
+    _LISTENER_CREATE = "tcr_dscnn_listener_create"
+
     def __init__(self, size: str = "S", height: int = 49, width: int = 40, num_classes: int = 12, max_batch: int = 512,
                  device: int | None = None):
         if not torch.cuda.is_available():
@@ -26,10 +32,19 @@ class DsCnn:
         descs, count, nparams, flops = C.POINTER(L.TcrParamDesc)(), C.c_int32(), C.c_int64(), C.c_int64()
         L.check(self.lib, self.lib.tcr_dscnn_param_table(self._h, C.byref(descs), C.byref(count), C.byref(nparams),
                                                          C.byref(flops)), "tcr_dscnn_param_table")
-        self.table = [dict(name=descs[i].name.decode(), shape=tuple(descs[i].shape[:descs[i].rank]), offset=int(descs[i].offset),
+        self.table = [dict(name=descs[i].name.decode(), kind=L.KIND_NAMES[descs[i].kind], trainable=descs[i].kind < 3,
+                           shape=tuple(descs[i].shape[:descs[i].rank]), offset=int(descs[i].offset),
                            numel=int(descs[i].numel)) for i in range(count.value)]
         self.num_params, self.forward_flops = int(nparams.value), int(flops.value)
         self.num_classes, self.height, self.width = num_classes, height, width
+        self.size, self.max_batch = size, int(max_batch)
+        self.cfg: Optional[L.TcrConfig] = None          # the front-end's configuration (set_frontend)
+        # the counts AudioNetModel reports, in tcr_get_info's form
+        self.info = L.TcrInfo(abi_version=L.ABI_VERSION, frames=height, features=width, forward_flops_per_utt=self.forward_flops)
+        self.info.num_moving = sum(d["numel"] for d in self.table if not d["trainable"])
+        self.info.num_trainable = self.num_params - self.info.num_moving
+        self.num_trainable, self.num_moving = int(self.info.num_trainable), int(self.info.num_moving)
+        self.frames, self.features = height, width
 
     def close(self):
         if getattr(self, "_h", None):
@@ -42,11 +57,94 @@ class DsCnn:
         except Exception:
             pass
 
+    @property
+    def _stream(self):
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _f32(self, *shape):
+        return torch.empty(shape, dtype=torch.float32, device=self.device)
+
+    @staticmethod
+    def _ptr(t, dtype=torch.float32):
+        return None if t is None else _checked(t, dtype)
+
+    @property
+    def trainable_names(self):
+        """The TF variables the reference's graph trains (weights, biases, beta), in table order; the moving statistics are not."""
+        return [d["name"] for d in self.table if d["trainable"]]
+
     def pack(self, values: Dict[str, np.ndarray]) -> torch.Tensor:
         flat = np.zeros(self.num_params, np.float32)
         for d in self.table:
             flat[d["offset"]:d["offset"] + d["numel"]] = np.asarray(values[d["name"]], np.float32).ravel()
         return torch.from_numpy(flat).to(self.device)
+
+    def new_variables(self, seed: int = 0) -> torch.Tensor:
+        """Flat variables as the reference initialises them before a restore: Xavier-uniform weights (slim's default), zero biases /
+        beta / moving mean, unit moving variance.  Host-side RNG, not TF's."""
+        rng = np.random.default_rng(seed)
+        flat = np.zeros(self.num_params, np.float32)
+        for d in self.table:
+            sl = slice(d["offset"], d["offset"] + d["numel"])
+            if d["kind"] == "weight":
+                shp = d["shape"]
+                fan_in, fan_out = int(np.prod(shp[:-1])), int(np.prod(shp[:-2])) * shp[-1]
+                lim = np.sqrt(6.0 / (fan_in + fan_out))
+                flat[sl] = rng.uniform(-lim, lim, d["numel"]).astype(np.float32)
+            elif d["kind"] == "moving_variance":
+                flat[sl] = 1.0
+        return torch.from_numpy(flat).to(self.device)
+
+    def variables_to_dict(self, params: torch.Tensor) -> Dict[str, np.ndarray]:
+        p = params.detach().cpu().numpy()
+        return {d["name"]: p[d["offset"]:d["offset"] + d["numel"]].reshape(d["shape"]).copy() for d in self.table}
+
+    def variables_from_dict(self, values: Dict[str, np.ndarray], params: torch.Tensor, strict: bool = True, only=None):
+        """Restores `params` by TF name, as Engine.variables_from_dict (only: predicate on names; the ones it rejects are skipped)."""
+        p = params.detach().cpu().numpy().copy()
+        for d in self.table:
+            if only is not None and not only(d["name"]):
+                continue
+            if d["name"] not in values:
+                if strict:
+                    raise KeyError(d["name"])
+                continue
+            v = np.asarray(values[d["name"]], np.float32)
+            if v.size != d["numel"]:
+                raise ValueError(f"{d['name']}: expected {d['shape']}, got {v.shape}")
+            p[d["offset"]:d["offset"] + d["numel"]] = v.ravel()
+        params.copy_(torch.from_numpy(p))
+
+    # ------------------------------------------------------------------ front-end and evaluation
+    def set_frontend(self, sample_rate=16000, clip_duration_ms=1000, window_size_ms=40.0, window_stride_ms=20.0, num_mel_bins=64,
+                     num_mfccs=40, lower_edge_hertz=80.0, upper_edge_hertz=7600.0, preprocess_method="mfcc"):
+        """The wav front-end in front of conv_1 (tcr_dscnn_set_frontend), from the reference's flags; its (T, F) must be the handle's
+        (height, width)."""
+        c = frontend_config(self.lib, sample_rate, clip_duration_ms, window_size_ms, window_stride_ms, num_mel_bins, num_mfccs,
+                            lower_edge_hertz, upper_edge_hertz, preprocess_method)
+        c.num_classes, c.max_batch, c.device = self.num_classes, self.max_batch, self.device.index
+        with torch.cuda.device(self.device):
+            L.check(self.lib, self.lib.tcr_dscnn_set_frontend(self._h, C.byref(c)), "tcr_dscnn_set_frontend")
+        assert frontend_shape(c) == (self.height, self.width)
+        self.cfg = c
+        return self
+
+    def _input(self, inputs: torch.Tensor, input_is_features: bool):
+        n = inputs.shape[0]
+        if input_is_features:
+            return self._ptr(inputs.reshape(n, self.height, self.width).contiguous()), L.TCR_INPUT_FEATURES
+        inputs = inputs.reshape(n, -1)
+        if inputs.dtype == torch.int16:
+            return self._ptr(inputs, torch.int16), L.TCR_INPUT_WAV_PCM16
+        return self._ptr(inputs), L.TCR_INPUT_WAV_F32
+
+    def mfcc(self, wav: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Front-end only: fp32 or int16 wav [n, clip_samples] -> features [n, height, width]."""
+        n = wav.shape[0]
+        ptr, kind = self._input(wav, False)
+        out = out if out is not None else self._f32(n, self.height, self.width)
+        L.check(self.lib, self.lib.tcr_dscnn_mfcc_forward(self._h, ptr, kind, self._ptr(out), n, self._stream), "tcr_dscnn_mfcc_forward")
+        return out
 
     def forward(self, features: torch.Tensor, params: torch.Tensor):
         n = features.shape[0]
@@ -57,3 +155,32 @@ class DsCnn:
         L.check(self.lib, self.lib.tcr_dscnn_forward(self._h, features.data_ptr(), params.data_ptr(), n, logits.data_ptr(),
                                                      probs.data_ptr(), stream), "tcr_dscnn_forward")
         return logits, probs
+
+    def forward_input(self, inputs: torch.Tensor, params: torch.Tensor, input_is_features: bool = False, logits=None, probs=None):
+        """The evaluation forward from fp32 wav, int16 PCM (decode_wav scaling on the device) or features: (logits, probs)."""
+        n = inputs.shape[0]
+        ptr, kind = self._input(inputs, input_is_features)
+        logits = logits if logits is not None else self._f32(n, self.num_classes)
+        probs = probs if probs is not None else self._f32(n, self.num_classes)
+        L.check(self.lib, self.lib.tcr_dscnn_forward_input(self._h, ptr, kind, self._ptr(params), n, self._ptr(logits), self._ptr(probs),
+                                                           self._stream), "tcr_dscnn_forward_input")
+        return logits, probs
+
+    def eval_accumulate(self, scores: torch.Tensor, onehot: torch.Tensor, counts: Optional[torch.Tensor] = None, topk: int = 5) -> torch.Tensor:
+        """Adds one batch to the device-resident evaluation counts, as Engine.eval_accumulate (tcr_dscnn_eval_accumulate)."""
+        n, c = scores.shape[0], self.num_classes
+        if counts is None:
+            counts = torch.zeros(c * c + 2, dtype=torch.int64, device=self.device)
+        assert counts.is_cuda and counts.dtype == torch.int64 and counts.numel() == c * c + 2
+        L.check(self.lib, self.lib.tcr_dscnn_eval_accumulate(self._h, self._ptr(scores), self._ptr(onehot), n, int(topk),
+                                                             counts.data_ptr(), self._stream), "tcr_dscnn_eval_accumulate")
+        return counts
+
+    def listener(self, streams: int, hop_frames: int, chunk_samples: int, params: Optional[torch.Tensor] = None) -> Listener:
+        """A continuous-audio listener on this handle (tcr_dscnn_listener_create); pushes take `params` only (moving is None)."""
+        return Listener(self, streams, hop_frames, chunk_samples, params, None)
+
+
+def _checked(t: torch.Tensor, dtype):
+    assert t.is_cuda and t.dtype == dtype and t.is_contiguous(), f"expected contiguous {dtype} CUDA tensor"
+    return t.data_ptr()

@@ -52,7 +52,33 @@ def _set_optimizer(a, optimizer, slots2_ptr):
         a.optimizer, a.rho, a.momentum = L.TCR_OPT_RMSPROP, float(o["decay"]), float(o["momentum"])
 
 
+def frontend_config(lib, sample_rate=16000, clip_duration_ms=1000, window_size_ms=40.0, window_stride_ms=20.0, num_mel_bins=64,
+                    num_mfccs=40, lower_edge_hertz=80.0, upper_edge_hertz=7600.0, preprocess_method="mfcc") -> "L.TcrConfig":
+    """tcr_config_default with the front-end fields set from the reference's flags (the fields tcr_dscnn_set_frontend reads)."""
+    if preprocess_method not in _FEATURES:
+        raise NotImplementedError(f"preprocess_method {preprocess_method}")
+    c = L.TcrConfig()
+    L.check(lib, lib.tcr_config_default(C.byref(c)), "tcr_config_default")
+    c.sample_rate = int(sample_rate)
+    # the reference's integer truncations (factory/audio_nets.py:63-64, :89)
+    c.clip_samples = int(sample_rate * clip_duration_ms / 1000)
+    c.window_size_samples = int(sample_rate * window_size_ms / 1000)
+    c.window_stride_samples = int(sample_rate * window_stride_ms / 1000)
+    c.num_mel_bins, c.num_mfccs = int(num_mel_bins), int(num_mfccs)
+    c.lower_edge_hertz, c.upper_edge_hertz = float(lower_edge_hertz), float(upper_edge_hertz)
+    c.feature_kind = _FEATURES[preprocess_method]
+    return c
+
+
+def frontend_shape(c: "L.TcrConfig"):
+    """(T, F) of a front-end configuration: frames and features per clip."""
+    frames = 1 + (c.clip_samples - c.window_size_samples) // c.window_stride_samples
+    return frames, (c.num_mfccs if c.feature_kind == L.TCR_FEATURE_MFCC else c.num_mel_bins)
+
+
 class Engine:
+    _LISTENER_CREATE = "tcr_listener_create"
+
     def __init__(self, model="TCResNet8", width_multiplier=1.0, num_classes=12, sample_rate=16000,
                  clip_duration_ms=1000, window_size_ms=40.0, window_stride_ms=20.0, num_mel_bins=64, num_mfccs=40,
                  lower_edge_hertz=80.0, upper_edge_hertz=7600.0, preprocess_method="mfcc", max_batch=512,
@@ -66,19 +92,11 @@ class Engine:
             raise NotImplementedError(f"preprocess_method {preprocess_method}")
         self.lib = L.load()
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
-        c = L.TcrConfig()
-        L.check(self.lib, self.lib.tcr_config_default(C.byref(c)), "tcr_config_default")
+        c = frontend_config(self.lib, sample_rate, clip_duration_ms, window_size_ms, window_stride_ms, num_mel_bins, num_mfccs,
+                            lower_edge_hertz, upper_edge_hertz, preprocess_method)
         c.model = _MODELS[model]
         c.width_multiplier = float(width_multiplier)
         c.num_classes = int(num_classes)
-        c.sample_rate = int(sample_rate)
-        # the reference's integer truncations (factory/audio_nets.py:63-64, :89)
-        c.clip_samples = int(sample_rate * clip_duration_ms / 1000)
-        c.window_size_samples = int(sample_rate * window_size_ms / 1000)
-        c.window_stride_samples = int(sample_rate * window_stride_ms / 1000)
-        c.num_mel_bins, c.num_mfccs = int(num_mel_bins), int(num_mfccs)
-        c.lower_edge_hertz, c.upper_edge_hertz = float(lower_edge_hertz), float(upper_edge_hertz)
-        c.feature_kind = _FEATURES[preprocess_method]
         c.max_batch = int(max_batch)
         c.bn_decay, c.bn_epsilon = float(bn_decay), float(bn_epsilon)
         c.dropout_keep_prob, c.label_smoothing = float(dropout_keep_prob), float(label_smoothing)
@@ -415,18 +433,19 @@ class Engine:
 
 
 class Listener:
-    """S audio streams scored with a sliding window (include/tcr_b200.h, tcr_listener_*).  Each push takes `chunk_samples` new
+    """S audio streams scored with a sliding window (include/tcr_b200.h, tcr_listener_*) by an Engine or a dscnn.DsCnn (moving None).  Each push takes `chunk_samples` new
     samples per stream and returns the softmax of K = chunk_samples / (hop_frames * window_stride_samples) windows per stream;
     window k of a stream (counted from its reset) is the clip starting k * hop_frames strides into the stream after
     (T - hop_frames) * stride + (window - stride) zeros, scored exactly as Engine.forward scores it in evaluation mode."""
 
-    def __init__(self, engine: Engine, streams: int, hop_frames: int, chunk_samples: int, params: Optional[torch.Tensor] = None,
+    def __init__(self, engine, streams: int, hop_frames: int, chunk_samples: int, params: Optional[torch.Tensor] = None,
                  moving: Optional[torch.Tensor] = None):
         self.eng, self.params, self.moving = engine, params, moving
         self._p = C.c_void_p()
         cfg = L.TcrListenerConfig(int(streams), int(hop_frames), int(chunk_samples))
+        create = engine._LISTENER_CREATE
         with torch.cuda.device(engine.device):
-            L.check(engine.lib, engine.lib.tcr_listener_create(engine._h, C.byref(cfg), C.byref(self._p)), "tcr_listener_create")
+            L.check(engine.lib, getattr(engine.lib, create)(engine._h, C.byref(cfg), C.byref(self._p)), create)
         self.streams, self.hop_frames, self.chunk_samples = int(streams), int(hop_frames), int(chunk_samples)
         self.windows = self.chunk_samples // (self.hop_frames * int(engine.cfg.window_stride_samples))
 

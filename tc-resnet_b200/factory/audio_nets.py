@@ -4,7 +4,8 @@ executing on the CUDA engine instead of building a TF graph.
 `train_audio.py` / `evaluate_audio.py` look the class up by NAME (`eval(f"audio_nets.{args.model}")`,
 train_audio.py:32), call `Model(args, dataset)`, then `model.build(wavs, labels, is_training)` and hand the model
 to the trainer / evaluator, which touch only the attributes set here and `session.run`.  TCResNet8Model and
-TCResNet14Model are on the accelerated path; the other entries of `_available_nets` (baselines the north star
+TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model are on it for evaluation, deployment and streaming (their
+training is out of scope and raises NotImplementedError); the other entries of `_available_nets` (baselines the north star
 does not name) are registered so the CLI accepts them but raise NotImplementedError when built.
 """
 from __future__ import annotations
@@ -17,6 +18,7 @@ import torch
 from ..common import utils
 from ..common.model_loader import EMA_SUFFIX
 from ..datasets import preprocessor_factory
+from ..dscnn import DsCnn
 from ..engine import OPTIMIZER_DEFAULTS, OPTIMIZER_SLOT_NAMES, Engine
 from ..runtime import InvalidArgumentError, Node
 from .base import TFModel
@@ -109,6 +111,10 @@ class AudioNetModel(TFModel):
 
     def build_loss(self, logits, scores, labels):
         return Node("total_loss", []), Node("model_loss", []), {}
+
+    def infer(self, inputs: torch.Tensor, input_is_features: bool = False) -> torch.Tensor:
+        """Softmax outputs [n, classes] of the evaluation forward on wav (fp32 / int16) or features (DeployedModel)."""
+        return self.engine.forward(inputs, self.params, self.moving, is_training=False, input_is_features=input_is_features)["probs"]
 
     def build_deployable_model(self, include_preprocess=True):
         """The deploy graph of the reference (factory/audio_nets.py:87-125: placeholder [input_batch_size, samples, 1] ->
@@ -460,8 +466,7 @@ class DeployedModel:
         self._graph, self._out, self._calls = None, None, 0
 
     def _run(self):
-        m = self.model
-        return m.engine.forward(self._in, m.params, m.moving, is_training=False, input_is_features=not self.include_preprocess)
+        return self.model.infer(self._in, input_is_features=not self.include_preprocess)
 
     def __call__(self, x) -> np.ndarray:
         x = torch.as_tensor(np.asarray(x, np.float32)).reshape(self._in.shape)
@@ -480,7 +485,7 @@ class DeployedModel:
                 self._graph = g
             self._graph.replay()
         self._calls += 1
-        return self._out["probs"].cpu().numpy()
+        return self._out.cpu().numpy()
 
 
 class StreamingModel:
@@ -555,8 +560,107 @@ Res8Model = _baseline("Res8Model", [("--weight_decay", 0.00001)])
 Res8NarrowModel = _baseline("Res8NarrowModel", [("--weight_decay", 0.00001)])
 Res15Model = _baseline("Res15Model", [("--weight_decay", 0.00001)])
 Res15NarrowModel = _baseline("Res15NarrowModel", [("--weight_decay", 0.00001)])
-DSCNNSModel = _baseline("DSCNNSModel", [("--weight_decay", 0.0)])
-DSCNNMModel = _baseline("DSCNNMModel", [("--weight_decay", 0.0)])
-DSCNNLModel = _baseline("DSCNNLModel", [("--weight_decay", 0.0)])
 ResNet2D8Model = _baseline("ResNet2D8Model", _TC)
 ResNet2D8PoolModel = _baseline("ResNet2D8PoolModel", _TC)
+
+
+class DsCnnModel(AudioNetModel):
+    """DSCNN{S,M,L}Model (factory/audio_nets.py:299-359, audio_nets/ds_cnn.py) in evaluation mode on dscnn.DsCnn: the handle runs the
+    model's front-end (tcr_dscnn_set_frontend), the forward with the BatchNorm moving statistics held in its flat parameters
+    (`moving` is None), the device evaluation counts, the deployable model and the listener.  Variables are restored by their TF
+    names ("DSCNN/conv_1/weights", ...), with the same --use_ema, --ignore_missing_vars and include / exclude scope rules as
+    TC-ResNet.  Training is out of scope."""
+    dscnn_size: Optional[str] = None
+
+    @staticmethod
+    def add_arguments(parser):
+        parser.add_argument("--weight_decay", default=0.0, type=float)
+
+    def build_inference(self, inputs, is_training=True):
+        if is_training:
+            raise NotImplementedError(f"{type(self).__name__}: training DS-CNN is out of scope on the CUDA path; evaluation "
+                                      "(evaluate_audio.py), the deployable model and the listener (listen_audio.py) are supported")
+        a = self.args
+        if getattr(a, "device_dataset", False):
+            raise NotImplementedError(f"{type(self).__name__}: --device_dataset serves the TC-ResNet models only")
+        self.engine = self._new_engine(max(int(getattr(a, 'batch_size', 1) or 1), int(getattr(a, 'input_batch_size', 1) or 1)))
+        self.params, self.moving, self.slots = self.engine.new_variables(seed=getattr(a, "seed", 0) or 0), None, None
+        n = int(getattr(a, 'batch_size', 1) or 1)
+        dev = self.engine.device
+        self._h_wav = torch.empty(n, self.engine.cfg.clip_samples, dtype=torch.float32).pin_memory()
+        self._h_hot = torch.empty(n, a.num_classes, dtype=torch.float32).pin_memory()
+        self._d_wav, self._d_hot = self._h_wav.to(dev), self._h_hot.to(dev)
+        return Node("logits", [None, a.num_classes]), {}
+
+    def _new_engine(self, max_batch: int) -> DsCnn:
+        a = self.args
+        clip = int(a.sample_rate * a.clip_duration_ms / 1000)
+        window, stride = int(a.sample_rate * a.window_size_ms / 1000), int(a.sample_rate * a.window_stride_ms / 1000)
+        if stride <= 0 or clip < window:
+            raise ValueError(f"bad window / stride / clip ({window} / {stride} / {clip} samples)")
+        height = 1 + (clip - window) // stride
+        width = a.num_mfccs if a.preprocess_method == "mfcc" else a.num_mel_bins
+        eng = DsCnn(self.dscnn_size, height, width, a.num_classes, max_batch)
+        return eng.set_frontend(a.sample_rate, a.clip_duration_ms, a.window_size_ms, a.window_stride_ms, a.num_mel_bins, a.num_mfccs,
+                                a.lower_edge_hertz, a.upper_edge_hertz, a.preprocess_method)
+
+    def infer(self, inputs: torch.Tensor, input_is_features: bool = False) -> torch.Tensor:
+        return self.engine.forward_input(inputs, self.params, input_is_features=input_is_features)[1]
+
+    def get_variables(self, with_slots=True) -> Dict[str, np.ndarray]:
+        """{TF name: array} of every variable, the moving statistics included (there is no optimizer state)."""
+        return self.engine.variables_to_dict(self.params)
+
+    def set_variables(self, values: Dict[str, np.ndarray], strict=True, restore=None):
+        """Variables by TF name (restore: predicate on names, model_loader.restore_filter); optimizer slots and shadows in the
+        checkpoint are ignored (evaluation with --use_ema has already put the shadows under the variables' names)."""
+        if restore is not None:
+            values = {k: v for k, v in values.items() if restore(k)}
+        self.engine.variables_from_dict(values, self.params, strict=strict, only=restore)
+
+    def execute(self, names: Set[str], feed) -> Dict[str, object]:
+        """One evaluation session.run: the batch from the dataset, the forward from its samples, the device counts when
+        `metric_counts` is fetched, and total_loss = model_loss = the batch's mean softmax cross-entropy (label smoothing as
+        --label_smoothing; the DS-CNN graph has no regularisation loss), from the logits in float64."""
+        if "train_op" in names:
+            raise NotImplementedError(f"{type(self).__name__}: training DS-CNN is out of scope on the CUDA path")
+        wav_np, hot_np = self.dataset.next_batch()
+        n = wav_np.shape[0]
+        if n != self.args.batch_size:
+            raise InvalidArgumentError(f"bad batch: {wav_np.shape}")
+        self._h_wav.copy_(torch.from_numpy(wav_np.reshape(n, -1)))
+        self._h_hot.copy_(torch.from_numpy(hot_np))
+        self._d_wav.copy_(self._h_wav, non_blocking=True)
+        self._d_hot.copy_(self._h_hot, non_blocking=True)
+        logits, probs = self.engine.forward_input(self._d_wav, self.params)
+        vals: Dict[str, object] = {"learning_rate": np.float32(self.lr_schedule(self.global_step))}
+        if "metric_counts" in names:                            # evaluation counts stay on the device until read_metric_counts()
+            if self._counts is None:
+                self._counts = torch.zeros(self.args.num_classes ** 2 + 2, dtype=torch.int64, device=self.engine.device)
+            self.engine.eval_accumulate(probs, self._d_hot, self._counts, topk=5)
+            vals["metric_counts"] = None
+        lg = logits.cpu().numpy().astype(np.float64)            # the D2H read synchronises the forward
+        ls = float(getattr(self.args, "label_smoothing", 0.0) or 0.0)
+        target = hot_np.astype(np.float64) * (1.0 - ls) + ls / lg.shape[1]
+        mx = lg.max(axis=1, keepdims=True)
+        logp = lg - mx - np.log(np.exp(lg - mx).sum(axis=1, keepdims=True))
+        loss = np.float32(-(target * logp).sum(axis=1).mean())
+        vals.update(total_loss=loss, model_loss=loss, global_step=np.int64(self.global_step), labels=hot_np, audio_original=wav_np)
+        if "outputs" in names or "logits" in names:
+            vals["outputs"], vals["logits"] = probs.cpu().numpy(), lg.astype(np.float32)
+        if "audio" in names:
+            vals["audio"] = self.engine.mfcc(self._d_wav).unsqueeze(-1).cpu().numpy()
+        self._last = vals
+        return vals
+
+
+class DSCNNSModel(DsCnnModel):
+    dscnn_size = "S"
+
+
+class DSCNNMModel(DsCnnModel):
+    dscnn_size = "M"
+
+
+class DSCNNLModel(DsCnnModel):
+    dscnn_size = "L"
