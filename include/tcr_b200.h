@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 11
+#define TCR_ABI_VERSION 12
 
 enum {
   TCR_OK = 0,
@@ -409,10 +409,24 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
  * (audio_nets/ds_cnn.py:20-118; factory/audio_nets.py DSCNN{S,M,L}Model.build_inference; BASELINE.json config 5).
  * features [n, height, width] (== [N,H,W,1]); params = one flat fp32 buffer laid out by tcr_dscnn_param_table
  * (TF variable names "DSCNN/conv_1/weights", ".../batch_norm/moving_mean", "DSCNN/fc1/biases", ...), the BatchNorm moving
- * statistics included.  size: 'S', 'M' or 'L' (64, 172 and 276 channels; the head takes up to 320). */
+ * statistics included.  size: 'S', 'M' or 'L' (64, 172 and 276 channels; the head takes up to 320).
+ *
+ * The same handle also runs the two Sainath & Parada CNNs of the reference's KWSModel (audio_nets/kws.py), evaluation mode (ABI 12):
+ *   size TCR_KWS_TRAD_FPOOL3 ('P', --architecture trad_fpool3): 20x8 conv 1 -> 64 + ReLU, max-pool 1x3 / stride 1x3, 10x4 conv
+ *     64 -> 64 + ReLU (every conv VALID, bias-free), then flatten (NHWC order) and the matmuls linear_weights [K, 32],
+ *     first_fc_weights [32, 128], final_fc_weights [128, classes], softmax.  Needs height >= 29 and width >= 19.
+ *   size TCR_KWS_ONE_FSTRIDE4 ('F', --architecture one_fstride4): height x 8 conv 1 -> 186, stride 4 in frequency + ReLU, then
+ *     first_linear_weights [K, 32], first_fc_weights [32, 128], second_fc_weights [128, 128], final_fc_weights [128, classes].
+ *     Needs width >= 8 and height x width <= 51,200 (its conv stages a whole utterance in shared memory).
+ * Their variables are top-level TF names ("first_weights", ...), all of kind TCR_KIND_WEIGHT; below the geometry bound create
+ * returns TCR_ERR_UNSUPPORTED, naming it.  Every tcr_dscnn_* entry point below serves them unchanged; forward_partial's layers
+ * are [conv1 + pool, conv2] for 'P' and [conv] for 'F', each written NHWC ([n, hout, wout, cout], the pooled width for 'P''s
+ * first), and, as for DS-CNN, the head is not among them. */
+#define TCR_KWS_TRAD_FPOOL3 'P'
+#define TCR_KWS_ONE_FSTRIDE4 'F'
 typedef struct tcr_dscnn tcr_dscnn;
 typedef struct tcr_dscnn_config {
-  int32_t size;          /* 'S' | 'M' | 'L' */
+  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 */
   int32_t height;        /* frames, 49 */
   int32_t width;         /* coefficients, 40 (10 in the reference's DS-CNN recipes) */
   int32_t num_classes;   /* 12 */

@@ -8,6 +8,9 @@
 //                          the input rows (+halo) and both filter banks are staged in shared memory, the depthwise result
 //                          never leaves the SM, the pointwise conv is a register-tiled 4 positions x 4 channels contraction
 //   dscnn_head_kernel      global average pool + fully connected (+bias) + softmax
+// and the KWS baselines of audio_nets/kws.py on the same handle (sizes 'P' trad_fpool3, 'F' one_fstride4): kws_conv_kernel (FMA
+// first layers), kws_bsplit_kernel + kws_conv2_tc_kernel (trad_fpool3's 64 -> 64 conv on wgmma), kws_lin_kernel + kws_head_kernel
+// (the dense head).
 // BatchNorm here has no gamma (slim default scale=False) and uses the moving statistics; bias + BN fold into one
 // per-channel (scale, shift) pair computed while staging.
 #ifndef TCR_EMU
@@ -27,17 +30,26 @@
 namespace tcr {
 
 struct DsLayerDev {
-  int type;                 // 0 conv, 1 separable
+  int type;                 // 0 conv, 1 separable, 2 (kLayerKws) VALID bias-free conv + ReLU of the KWS baselines
   int cin, cout, kh, kw, sh, sw, hin, win, hout, wout, pt, pl;
   int64_t w, b, beta, mm, mv;                // conv / depthwise
   int64_t pw, pb, pbeta, pmm, pmv;           // pointwise (separable only)
 };
 
 constexpr int kDsMaxLayers = 8;
+constexpr int kLayerKws = 2;
 struct DsNet {
   int nlayers, n, classes;
   DsLayerDev layer[kDsMaxLayers];
   int64_t fcw, fcb;
+};
+
+// A layer of the KWS baselines (audio_nets/kws.py): VALID, bias-free convolution + ReLU, in [n][hin][win][cin] -> out
+// [n][hout][wout][cout] NHWC, w [kh][kw][cin][cout] at params + w; wout counts pooled columns where the layer max-pools over width
+// (hout rows are walked in tiles of RH by the FMA kernel).
+struct KwsConv {
+  int cin, cout, kh, kw, sh, sw, hin, win, hout, wout, RH;
+  int64_t w;
 };
 
 __device__ __forceinline__ void fold_bn(const float* p, int64_t b, int64_t beta, int64_t mm, int64_t mv, int c, float eps,
@@ -874,6 +886,289 @@ __global__ void __launch_bounds__(kTcThreads, 1) dscnn_conv_tc_kernel(DsLayerDev
     q.run(K >> 3, npos, sc, sf, out, ((size_t)n * L.hout + h0) * L.wout, tid & 127);
   }
 }
+
+// ---- cnn-trad-fpool3's second convolution (audio_nets/kws.py:242-254) as an implicit GEMM on wgmma (3xTF32) ----
+// 10 x 4 VALID, 64 -> 64 channels, ReLU: M = output positions flattened over (utterance, oh, ow), K = 40 taps x 64 channels = 2,560,
+// N = 64.  The 655 KB filter bank cannot stay in shared memory, so K is streamed in chunks of 32 (half a tap's channels) through
+// a ring of kC2Stages stages, each holding that chunk's A (128 rows, hi / lo) and B (64 columns, hi / lo):
+//   warps 0-7   producers: thread 0 bulk-copies the chunk's B (split once per forward by kws_bsplit_kernel into the stage's exact
+//               image) and the 256 threads gather A, the 128-byte channel halves of the NHWC input at (oh + i, ow + j), split it
+//               and store it in the K-major layout, the next chunk's gathers already in flight; one arrival each, the bulk
+//               copy's bytes on the same `full` barrier;
+//   warps 8-11  consumer warpgroup: per chunk 3 passes x 4 k-steps of two wgmma m64n64k8 (rows 0-63, 64-127), one commit group
+//               per chunk kept in flight: once the previous chunk's group has completed its stage is handed back (`empty`).
+//               Every kC2Flush chunks (K = 256) the accumulators are folded into a register sum with fp32 adds and restarted
+//               (scale-d = 0): the error of the tensor cores' own accumulation grows with K, and over all 2,560 at once it reached
+//               2.1e-5 of the layer's maximum, over the 1e-5 layer bound; in blocks of 256 it is 1.1e-6 to 1.5e-6.
+// A tile is 128 consecutive output rows, so tiles span utterances and the last one is partial (its missing rows are zero A rows
+// whose accumulator rows are not stored); the grid is persistent and walks the tiles with its own stride.
+constexpr int kC2Chunk = 32, kC2Stages = 4, kC2Producers = 256, kC2Threads = kC2Producers + 128, kC2Flush = 8;
+constexpr int kC2Lbb = 64 * 4;                                          // B image: K-chunk-of-4 stride in floats (no padding)
+constexpr int kC2AFloats = 2 * (kC2Chunk / 4) * kLbaFull;              // A hi, lo [8][kLbaFull]
+constexpr int kC2BFloats = 2 * (kC2Chunk / 4) * kC2Lbb;                // B hi, lo [8][64 x 4]: 16 KB, one bulk copy
+constexpr int kC2StageFloats = kC2AFloats + kC2BFloats;                // 49,408 bytes, a multiple of 16
+
+// Filter bank w [K][64] -> the B stage image of every chunk c: hi then lo, element (co, k) at (k % 32 / 4) * 256 + co * 4 + k % 4.
+__global__ void __launch_bounds__(256) kws_bsplit_kernel(int K, const float* __restrict__ w, float* __restrict__ img) {
+  pdl_wait();
+  for (int i = blockIdx.x * 256 + threadIdx.x; i < K * 64; i += gridDim.x * 256) {
+    const int k = i >> 6, co = i & 63, kk = k % kC2Chunk;
+    const float v = __ldg(w + i), hi = tf32_hi(v);
+    float* dst = img + (size_t)(k / kC2Chunk) * kC2BFloats + (kk >> 2) * kC2Lbb + co * 4 + (kk & 3);
+    dst[0] = hi;
+    dst[kC2BFloats / 2] = v - hi;
+  }
+}
+
+// D[64 x 64] = A B^T (ACC = 0: the accumulator's old value is ignored, scale-d = 0) or D += A B^T (ACC = 1)
+template <int ACC>
+__device__ __forceinline__ void wgmma_m64n64k8_tf32_sd(float (&d)[32], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "n"(ACC)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+
+__global__ void __launch_bounds__(kC2Threads, 1) kws_conv2_tc_kernel(KwsConv L, int n_utt, const float* __restrict__ bimg,
+                                                                     const float* __restrict__ in, float* __restrict__ out) {
+  TCR_DYNAMIC_SMEM(smem_raw);
+  __shared__ uint64_t full[kC2Stages], empty[kC2Stages];
+  float* smem = reinterpret_cast<float*>(smem_raw);
+  const int tid = threadIdx.x;
+  const int npos = L.hout * L.wout, rows = n_utt * npos, ntiles = (rows + 127) / 128;
+  const int cpt = L.cin / kC2Chunk, nchunks = L.kh * L.kw * cpt;       // chunks per tap, per tile
+  if (tid == 0) {
+    for (int s = 0; s < kC2Stages; ++s) {
+      mbar_init(&full[s], kC2Producers + 1);                           // + thread 0's expect_tx
+      mbar_init(&empty[s], 128);
+    }
+  }
+  pdl_wait();
+  __syncthreads();
+  if (tid < kC2Producers) {
+    const int q = tid & 7, m0 = tid >> 3;                              // float4 q of a row's 32 channels; rows m0 + 32 r
+    int64_t base[4];
+    bool ok[4];
+    uint32_t g = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int row = tile * 128 + m0 + 32 * r;
+        ok[r] = row < rows;
+        const int rr = ok[r] ? row : 0, n = rr / npos, p = rr - n * npos, oh = p / L.wout, ow = p - oh * L.wout;
+        base[r] = (((int64_t)n * L.hin + oh) * L.win + ow) * L.cin + 4 * q;
+      }
+      auto load = [&](int c, float4 (&v)[4]) {                        // chunk c's A rows of this thread, into registers
+        const int tap = c / cpt, ti = tap / L.kw, tj = tap - ti * L.kw;
+        const int64_t off = ((int64_t)ti * L.win + tj) * L.cin + (c - tap * cpt) * kC2Chunk;
+#pragma unroll
+        for (int r = 0; r < 4; ++r) v[r] = ok[r] ? ldg4(in + base[r] + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+      };
+      float4 v[4], nxt[4];
+      load(0, v);
+      for (int c = 0; c < nchunks; ++c, ++g) {
+        const int s = g % kC2Stages;
+        if (c + 1 < nchunks) load(c + 1, nxt);                         // in flight while this chunk is split and stored
+        if (g >= kC2Stages) mbar_wait(&empty[s], ((g / kC2Stages) - 1) & 1);      // the MMAs of chunk g - kC2Stages are done
+        float* a_hi = smem + (size_t)s * kC2StageFloats;
+        float* a_lo = a_hi + (kC2Chunk / 4) * kLbaFull;
+        if (tid == 0) {
+          mbar_expect_tx(&full[s], kC2BFloats * 4);
+          tma_load_1d(a_hi + kC2AFloats, bimg + (size_t)c * kC2BFloats, kC2BFloats * 4, &full[s]);
+        }
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          float4 hi, lo;
+          tf32_split(v[r], hi, lo);
+          st4(a_hi + q * kLbaFull + 4 * (m0 + 32 * r), hi);
+          st4(a_lo + q * kLbaFull + 4 * (m0 + 32 * r), lo);
+          v[r] = nxt[r];
+        }
+        fence_proxy_async();                                           // operand stores -> visible to the async proxy (wgmma)
+        mbar_arrive(&full[s]);
+      }
+    }
+  } else {
+    const int wtid = tid - kC2Producers;
+    uint32_t g = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      float acc[2][32], sum[2][32];                                    // acc is (re)started by the block's first MMA (scale-d = 0)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { sum[0][i] = 0.f; sum[1][i] = 0.f; }
+      for (int cb = 0; cb < nchunks; cb += kC2Flush) {                // nchunks is a multiple of kC2Flush (host side)
+#pragma unroll
+        for (int cc = 0; cc < kC2Flush; ++cc, ++g) {
+          const int s = g % kC2Stages;
+          mbar_wait(&full[s], (g / kC2Stages) & 1);
+          const float* a_hi = smem + (size_t)s * kC2StageFloats;
+          const float* b_hi = a_hi + kC2AFloats;
+          const uint64_t da_hi = gmma_desc(smem_u32(a_hi), kLbaFull * 4u, 128u);
+          const uint64_t da_lo = gmma_desc(smem_u32(a_hi + (kC2Chunk / 4) * kLbaFull), kLbaFull * 4u, 128u);
+          const uint64_t db_hi = gmma_desc(smem_u32(b_hi), kC2Lbb * 4u, 128u);
+          const uint64_t db_lo = gmma_desc(smem_u32(b_hi + kC2BFloats / 2), kC2Lbb * 4u, 128u);
+          wgmma_fence();
+#pragma unroll
+          for (int pass = 0; pass < 3; ++pass) {                       // lo*hi, hi*lo, hi*hi
+            const uint64_t da0 = pass == 0 ? da_lo : da_hi, db0 = pass == 1 ? db_lo : db_hi;
+#pragma unroll
+            for (int ks = 0; ks < kC2Chunk / 8; ++ks) {
+              const uint64_t da = da0 + (uint64_t)((2 * ks * kLbaFull * 4) >> 4), db = db0 + (uint64_t)((2 * ks * kC2Lbb * 4) >> 4);
+              if (cc == 0 && pass == 0 && ks == 0) {
+                wgmma_m64n64k8_tf32_sd<0>(acc[0], da, db);
+                wgmma_m64n64k8_tf32_sd<0>(acc[1], da + (uint64_t)((64 * 16) >> 4), db);
+              } else {
+                wgmma_m64n64k8_tf32_sd<1>(acc[0], da, db);
+                wgmma_m64n64k8_tf32_sd<1>(acc[1], da + (uint64_t)((64 * 16) >> 4), db);
+              }
+            }
+          }
+          wgmma_commit();
+          if (cc > 0) {
+            wgmma_wait_1();                                            // the previous chunk's MMAs have read their stage
+            mbar_arrive(&empty[(g - 1) % kC2Stages]);
+          }
+        }
+        wgmma_wait_all();
+        mbar_arrive(&empty[(g - 1) % kC2Stages]);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) { sum[0][i] += acc[0][i]; sum[1][i] += acc[1][i]; }
+      }
+      // ReLU + NHWC store: accumulator row m of the tile is output row tile * 128 + m (d[4 j + 2 h + e] = D[16 w + l / 4 + 8 h][8 j + 2 (l % 4) + e])
+      const int r0 = 16 * (wtid >> 5) + ((wtid & 31) >> 2), c0 = 2 * (wtid & 3);
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int qq = 0; qq < 4; ++qq) {                               // rows r0, r0 + 8, r0 + 64, r0 + 72
+          const int row = tile * 128 + r0 + 8 * (qq & 1) + 64 * (qq >> 1);
+          if (row < rows) {
+            const float* a = &sum[qq >> 1][4 * j + 2 * (qq & 1)];
+            *reinterpret_cast<float2*>(out + (size_t)row * 64 + 8 * j + c0) = make_float2(fmaxf(a[0], 0.f), fmaxf(a[1], 0.f));
+          }
+        }
+    }
+  }
+}
+
+// ---- cnn-trad-fpool3's first convolution + ReLU + 1 x 3 max-pool (audio_nets/kws.py:223-240) as an implicit GEMM on wgmma ----
+// 20 x 8 VALID, 1 -> 64 channels, 3xTF32: K = 160 taps, N = 64.  The accumulator rows of a tile are 42 pooled outputs x their 3
+// pre-pool columns (row m: pooled output tile * 42 + m / 3, column 3 * owp + m % 3; rows 126 and 127 are zero), flattened over
+// (utterance, oh, owp), so a pooling window never straddles tiles and only the pooled map reaches HBM.  Persistent, lock-step
+// (like dscnn_conv_tc): the split filter bank stays in shared memory for all the CTA's tiles; per tile and half of K, every thread
+// gathers its row's 4-tap chunks straight from the feature map (4 taps of a chunk are 4 consecutive columns of one row, read
+// through L1) into the K-major A operand (hi / lo), then the four warpgroups each issue the 3 passes x 10 k-steps of one
+// m64n32k8 quarter of the accumulator.  Epilogue: ReLU into shared memory (over the A region), then the max over each row
+// triple, stored NHWC.  WIN: utterance n is a listener window (ds_window).
+constexpr int kC1Pooled = 42, kC1Half = 20;                           // pooled outputs per tile; K chunks of 4 per half of K
+constexpr int kC1Ep = 65;                                              // epilogue scratch row stride (floats)
+TCR_HD inline size_t conv1_tc_smem_floats(int K4) { return 2 * (size_t)K4 * gmma_lbb(64) + 2 * (size_t)kC1Half * kLbaFull; }
+// D[64 x 32] = A B^T (ACC = 0, scale-d = 0) or D += A B^T (ACC = 1)
+template <int ACC>
+__device__ __forceinline__ void wgmma_m64n32k8_tf32_sd(float (&d)[16], uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "n"(ACC)
+      : "memory");
+}
+
+template <bool WIN>
+__global__ void __launch_bounds__(kTcThreads, 1) kws_conv1_tc_kernel(KwsConv L, int n_utt, const float* __restrict__ params,
+                                                                     const float* __restrict__ in, float* __restrict__ out,
+                                                                     WindowView win) {
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* smem = reinterpret_cast<float*>(smem_raw);
+  const int tid = threadIdx.x;
+  const int K = L.kh * L.kw, K4 = K / 4;                              // host side: K4 == 2 * kC1Half, kw a multiple of 4
+  constexpr int LBB = gmma_lbb(64);
+  float *b_hi = smem, *b_lo = b_hi + (size_t)K4 * LBB;
+  float *a_hi = b_lo + (size_t)K4 * LBB, *a_lo = a_hi + kC1Half * kLbaFull;
+  float* ep = a_hi;                                                   // [128][kC1Ep] once the tile's MMAs are done
+  stage_b<kTcThreads, 64, 1>(params + L.w, K, b_hi, b_lo, tid);
+  pdl_wait();
+  const int per_utt = L.hout * L.wout, total = n_utt * per_utt, ntiles = (total + kC1Pooled - 1) / kC1Pooled;
+  const int g = tid >> 7, wtid = tid & 127, m0 = 64 * (g & 1), col0 = 32 * (g >> 1);    // this warpgroup's quarter
+  const uint64_t da_hi = gmma_desc(smem_u32(a_hi + 4 * m0), kLbaFull * 4u, 128u), da_lo = gmma_desc(smem_u32(a_lo + 4 * m0), kLbaFull * 4u, 128u);
+  const uint64_t db_hi = gmma_desc(smem_u32(b_hi + 4 * col0), LBB * 4u, 128u), db_lo = gmma_desc(smem_u32(b_lo + 4 * col0), LBB * 4u, 128u);
+  fence_proxy_async();                                                // the B operand was written through the generic proxy
+  const int m = tid & 127, cq = tid >> 7;                             // the gather: A row m, chunks cq + 4 j of each half
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int p = tile * kC1Pooled + m / 3;
+    const bool ok = m < 3 * kC1Pooled && p < total;
+    const float* xr = in;
+    if (ok) {
+      const int n = p / per_utt, r = p - n * per_utt, oh = r / L.wout, owp = r - oh * L.wout;
+      const float* utt;
+      if constexpr (WIN) utt = ds_window(in, n, win);
+      else utt = in + (int64_t)n * L.hin * L.win;
+      xr = utt + (int64_t)oh * L.win + 3 * owp + (m - 3 * (m / 3));
+    }
+    float acc[16];
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      for (int c = cq; c < kC1Half; c += 4) {
+        const int k0 = 4 * (half * kC1Half + c), i = k0 / L.kw, j = k0 - i * L.kw;
+        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (ok) {
+          const float* s = xr + i * L.win + j;
+          v = make_float4(__ldg(s), __ldg(s + 1), __ldg(s + 2), __ldg(s + 3));
+        }
+        float4 hi, lo;
+        tf32_split(v, hi, lo);
+        st4(a_hi + c * kLbaFull + 4 * m, hi);
+        st4(a_lo + c * kLbaFull + 4 * m, lo);
+      }
+      fence_proxy_async();                                            // operand stores -> visible to the async proxy (wgmma)
+      __syncthreads();
+      wgmma_fence();
+      // opaque copies: the per-k-step descriptors are formed here, not hoisted out of the tile loop (60 of them would spill)
+      uint64_t dal = da_lo, dah = da_hi, dbl = db_lo, dbh = db_hi;
+      asm volatile("" : "+l"(dal), "+l"(dah), "+l"(dbl), "+l"(dbh));
+#pragma unroll
+      for (int pass = 0; pass < 3; ++pass) {                          // lo*hi, hi*lo, hi*hi
+        const uint64_t da0 = pass == 0 ? dal : dah, db0 = pass == 1 ? dbl : dbh;
+#pragma unroll
+        for (int ks = 0; ks < kC1Half / 2; ++ks) {
+          const uint64_t da = da0 + (uint64_t)((2 * ks * kLbaFull * 4) >> 4);
+          const uint64_t db = db0 + (uint64_t)(((2 * ks + half * kC1Half) * LBB * 4) >> 4);
+          if (half == 0 && pass == 0 && ks == 0) wgmma_m64n32k8_tf32_sd<0>(acc, da, db);
+          else wgmma_m64n32k8_tf32_sd<1>(acc, da, db);
+        }
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      __syncthreads();                                                // every warpgroup has read A: refill it / reuse it as `ep`
+    }
+    // ReLU into ep (d[4 j + 2 h + e] = D[m0 + 16 w + l / 4 + 8 h][col0 + 8 j + 2 (l % 4) + e]), then the max over row triples
+    const int r0 = m0 + 16 * (wtid >> 5) + ((wtid & 31) >> 2), c0 = col0 + 2 * (wtid & 3);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        ep[(r0 + 8 * h) * kC1Ep + c0 + 8 * j] = fmaxf(acc[4 * j + 2 * h], 0.f);
+        ep[(r0 + 8 * h) * kC1Ep + c0 + 8 * j + 1] = fmaxf(acc[4 * j + 2 * h + 1], 0.f);
+      }
+    __syncthreads();
+    for (int idx = tid; idx < kC1Pooled * 64; idx += kTcThreads) {
+      const int pp = idx >> 6, co = idx & 63, po = tile * kC1Pooled + pp;
+      if (po < total) {
+        const float* e = ep + 3 * pp * kC1Ep + co;
+        out[(int64_t)po * 64 + co] = fmaxf(fmaxf(e[0], e[kC1Ep]), e[2 * kC1Ep]);
+      }
+    }
+    __syncthreads();                                                  // ep is the next tile's A
+  }
+}
 #endif
 
 // ---- head: one CTA per utterance ----
@@ -932,6 +1227,176 @@ __global__ void __launch_bounds__(256) dscnn_head_kernel(int npos, int C, int cl
   }
 }
 
+// ---- KWS baselines: FMA convolution, one CTA per (utterance, tile of L.RH output rows), blockIdx.x = n * tiles + tile ----
+// cnn-trad-fpool3's first layer (20 x 8, 1 -> 64, ReLU, max-pool 1 x 3 / stride 3: POOL = 3, only the pooled map is stored) and
+// cnn-one-fstride4's only one (T x 8, stride 4 in frequency, 1 -> 186); the emulator build, which has no wgmma, also runs the
+// 64 -> 64 second layer of trad_fpool3 here.  The tile's input rows are staged in shared memory.  A thread owns CPT consecutive
+// output channels (CPT = 4: float4 filter loads, cout a multiple of 4; CPT = 1: any channel count) and RT output rows x CT output
+// columns x POOL pre-pool columns, so one filter load feeds RT * CT * POOL * CPT FMAs and one input load CPT.  Consecutive threads
+// take consecutive channel groups: a warp's filter loads are one coalesced row and its input loads broadcasts.  Rows and columns
+// past the tile re-read its last one and are not stored.  WIN: utterance n is a listener window (ds_window).
+constexpr int kKwsMaxStaged = 51200;                                  // floats of input rows the FMA kernel stages (200 KB)
+TCR_HD inline int kws_stage_floats(const KwsConv& L) { return ((L.RH - 1) * L.sh + L.kh) * L.win * L.cin; }
+template <int POOL, int CPT, int RT, int CT, bool WIN>
+__global__ void __launch_bounds__(256, 2) kws_conv_kernel(KwsConv L, const float* __restrict__ params, const float* __restrict__ in,
+                                                       float* __restrict__ out, WindowView win) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* xs = reinterpret_cast<float*>(smem_raw);
+  const int tpu = (L.hout + L.RH - 1) / L.RH, tid = threadIdx.x;
+  const int n = blockIdx.x / tpu, h0 = (blockIdx.x - n * tpu) * L.RH, rh = imin(L.RH, L.hout - h0);
+  const int rowlen = L.win * L.cin, staged = ((rh - 1) * L.sh + L.kh) * rowlen;
+  const float* src;
+  if constexpr (WIN) src = ds_window(in, n, win) + (int64_t)h0 * L.sh * rowlen;
+  else src = in + ((int64_t)n * L.hin + (int64_t)h0 * L.sh) * rowlen;
+  for (int i = tid; i < staged; i += blockDim.x) xs[i] = src[i];
+  __syncthreads();
+  const int ncg = L.cout / CPT, ncol = (L.wout + CT - 1) / CT;
+  const int ntask = ncg * ncol * ((rh + RT - 1) / RT);
+  for (int task = tid; task < ntask; task += blockDim.x) {
+    const int cg = task % ncg, t1 = task / ncg, ow0 = (t1 % ncol) * CT, r0 = (t1 / ncol) * RT;
+    int xoff[RT][CT];                                             // staged-tile offset of each (row, column)'s first tap
+#pragma unroll
+    for (int r = 0; r < RT; ++r)
+#pragma unroll
+      for (int q = 0; q < CT; ++q) xoff[r][q] = imin(r0 + r, rh - 1) * L.sh * rowlen + imin(ow0 + q, L.wout - 1) * POOL * L.sw * L.cin;
+    float acc[RT][CT][POOL][CPT];
+#pragma unroll
+    for (int r = 0; r < RT; ++r)
+#pragma unroll
+      for (int q = 0; q < CT; ++q)
+#pragma unroll
+        for (int e = 0; e < POOL; ++e)
+#pragma unroll
+          for (int k = 0; k < CPT; ++k) acc[r][q][e][k] = 0.f;
+    const float* wc = params + L.w + CPT * cg;
+    for (int i = 0; i < L.kh; ++i)
+      for (int j = 0; j < L.kw; ++j) {
+        const float* xb = xs + i * rowlen + j * L.cin;
+        const float* wb = wc + (int64_t)(i * L.kw + j) * L.cin * L.cout;
+        for (int ci = 0; ci < L.cin; ++ci) {
+          float wv[CPT];
+          if constexpr (CPT == 4) {
+            const float4 w4 = ldg4(wb + (int64_t)ci * L.cout);
+            wv[0] = w4.x; wv[1] = w4.y; wv[2] = w4.z; wv[3] = w4.w;
+          } else {
+            wv[0] = __ldg(wb + (int64_t)ci * L.cout);
+          }
+#pragma unroll
+          for (int r = 0; r < RT; ++r)
+#pragma unroll
+            for (int q = 0; q < CT; ++q)
+#pragma unroll
+              for (int e = 0; e < POOL; ++e) {
+                const float x = xb[xoff[r][q] + e * L.sw * L.cin + ci];
+#pragma unroll
+                for (int k = 0; k < CPT; ++k) acc[r][q][e][k] = fmaf(x, wv[k], acc[r][q][e][k]);
+              }
+        }
+      }
+#pragma unroll
+    for (int r = 0; r < RT; ++r)
+#pragma unroll
+      for (int q = 0; q < CT; ++q) {
+        if (r0 + r < rh && ow0 + q < L.wout) {
+          float* o = out + (((int64_t)n * L.hout + h0 + r0 + r) * L.wout + ow0 + q) * L.cout + CPT * cg;
+#pragma unroll
+          for (int k = 0; k < CPT; ++k) {
+            float v = 0.f;                                        // ReLU, then the max over the pooling window
+#pragma unroll
+            for (int e = 0; e < POOL; ++e) v = fmaxf(v, acc[r][q][e][k]);
+            o[k] = v;
+          }
+        }
+      }
+  }
+}
+
+// ---- KWS baselines' dense head: flatten -> lin (K x 32) -> 128 (-> 128) -> classes, no nonlinearity, then softmax ----
+// The matrices are applied one at a time, in the reference's order.  lin is split over K: CTA (utterance group, K chunk s) stages
+// kKwsLinK rows of the weights once for kKwsLinU utterances and writes partial sums part[s][u][32]; kws_head_kernel adds the
+// chunks in order, so the logits of an utterance do not depend on the batch it is in.
+constexpr int kKwsLinK = 256, kKwsLinU = 64, kKwsHeadU = 16;
+constexpr size_t kKwsLinSmem = (size_t)(kKwsLinK * 32 + kKwsLinU * (kKwsLinK + 1)) * 4;
+struct KwsHead { int K, nsplit, nfc, classes; int64_t lin, fc[2], out; };
+
+__global__ void __launch_bounds__(256) kws_lin_kernel(KwsHead H, int n, const float* __restrict__ params, const float* __restrict__ in,
+                                                      float* __restrict__ part) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* ws = reinterpret_cast<float*>(smem_raw);                 // [kKwsLinK][32]
+  float* xs = ws + kKwsLinK * 32;                                 // [kKwsLinU][kKwsLinK + 1]
+  const int s = blockIdx.x % H.nsplit, u0 = (blockIdx.x / H.nsplit) * kKwsLinU, tid = threadIdx.x;
+  const int k0 = s * kKwsLinK, kc = imin(kKwsLinK, H.K - k0), nu = imin(kKwsLinU, n - u0);
+  for (int i = tid; i < kc * 32; i += blockDim.x) ws[i] = __ldg(params + H.lin + (int64_t)k0 * 32 + i);
+  for (int i = tid; i < nu * kc; i += blockDim.x) {               // K need not be a multiple of 4 (one_fstride4: 1,674)
+    const int u = i / kc, k = i - u * kc;
+    xs[u * (kKwsLinK + 1) + k] = in[(int64_t)(u0 + u) * H.K + k0 + k];
+  }
+  __syncthreads();
+  const int lane = tid & 31, warp = tid >> 5;                     // lane = output column, warp = utterances warp + 8 i
+  float acc[kKwsLinU / 8];
+#pragma unroll
+  for (int i = 0; i < kKwsLinU / 8; ++i) acc[i] = 0.f;
+  for (int k = 0; k < kc; ++k) {
+    const float w = ws[k * 32 + lane];
+#pragma unroll
+    for (int i = 0; i < kKwsLinU / 8; ++i) acc[i] = fmaf(xs[(warp + 8 * i) * (kKwsLinK + 1) + k], w, acc[i]);
+  }
+#pragma unroll
+  for (int i = 0; i < kKwsLinU / 8; ++i)
+    if (warp + 8 * i < nu) part[((int64_t)s * n + u0 + warp + 8 * i) * 32 + lane] = acc[i];
+}
+
+// kKwsHeadU utterances per CTA of 128 threads: every weight of the 128-wide matrices is loaded once per CTA.
+__global__ void __launch_bounds__(128) kws_head_kernel(KwsHead H, int n, const float* __restrict__ params, const float* __restrict__ part,
+                                                       float* __restrict__ logits, float* __restrict__ probs) {
+  pdl_wait();
+  __shared__ float h[2][kKwsHeadU][128];
+  __shared__ float s_logit[kKwsHeadU][kMaxClasses];
+  const int u0 = blockIdx.x * kKwsHeadU, nu = imin(kKwsHeadU, n - u0), tid = threadIdx.x, C = H.classes;
+  for (int i = tid; i < kKwsHeadU * 32; i += blockDim.x) {
+    const int u = i >> 5, j = i & 31;
+    float a = 0.f;
+    if (u < nu)
+      for (int s = 0; s < H.nsplit; ++s) a += part[((int64_t)s * n + u0 + u) * 32 + j];
+    h[0][u][j] = a;
+  }
+  __syncthreads();
+  int cur = 0, width = 32;
+  for (int m = 0; m < H.nfc; ++m, cur ^= 1, width = 128) {
+    const float* W = params + H.fc[m];
+    float acc[kKwsHeadU];
+#pragma unroll
+    for (int u = 0; u < kKwsHeadU; ++u) acc[u] = 0.f;
+    for (int k = 0; k < width; ++k) {
+      const float w = __ldg(W + k * 128 + tid);
+#pragma unroll
+      for (int u = 0; u < kKwsHeadU; ++u) acc[u] = fmaf(h[cur][u][k], w, acc[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < kKwsHeadU; ++u) h[cur ^ 1][u][tid] = acc[u];
+    __syncthreads();
+  }
+  for (int i = tid; i < nu * C; i += blockDim.x) {
+    const int u = i / C, c = i - u * C;
+    float a = 0.f;
+    for (int k = 0; k < 128; ++k) a = fmaf(h[cur][u][k], __ldg(params + H.out + k * C + c), a);
+    s_logit[u][c] = a;
+    if (logits) logits[(int64_t)(u0 + u) * C + c] = a;
+  }
+  __syncthreads();
+  if (!probs) return;
+  for (int i = tid; i < nu * C; i += blockDim.x) {
+    const int u = i / C, c = i - u * C;
+    float mx = -3.0e38f;
+    for (int k = 0; k < C; ++k) mx = fmaxf(mx, s_logit[u][k]);
+    float se = 0.f;
+    for (int k = 0; k < C; ++k) se += expf(s_logit[u][k] - mx);
+    probs[(int64_t)(u0 + u) * C + c] = expf(s_logit[u][c] - mx) / se;
+  }
+}
+
 }  // namespace tcr
 
 // ------------------------------------------------------------------------------------------------
@@ -955,6 +1420,12 @@ struct tcr_dscnn {
 #endif
   Frontend fe;               // tcr_dscnn_set_frontend: the wav front-end in front of conv_1 (fe.frames == 0: none yet)
   float* feat = nullptr;     // [max_batch, height, width]: the features of a wav-input forward
+  // KWS baselines ('P', 'F'): layers of type kLayerKws, their pooling, the dense head and its buffers
+  bool kws = false;
+  int pool[kDsMaxLayers] = {};
+  KwsHead head = {};
+  float* part = nullptr;     // [head.nsplit][max_batch][32]: lin's partial sums per K chunk
+  float* bimg = nullptr;     // trad_fpool3: conv2's filter bank split into hi / lo B stage images (kws_bsplit_kernel)
 };
 
 #ifndef TCR_EMU
@@ -985,6 +1456,16 @@ static int ds_encode_in_map(CUtensorMap* map, const float* base, int c, int w, i
 }
 #endif
 
+static int ds_fail(int code, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  set_error(buf);
+  return code;
+}
+
 static void ds_same(int len, int k, int s, int* out, int* lead) {
   *out = (len + s - 1) / s;
   const int total = std::max((*out - 1) * s + k - len, 0);
@@ -994,13 +1475,29 @@ static void ds_same(int len, int k, int s, int* out, int* lead) {
 extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   if (!cfg || !out) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   *out = nullptr;
-  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L') { set_error("DS-CNN size must be 'S', 'M' or 'L'"); return TCR_ERR_INVALID; }
+  const bool kws = cfg->size == TCR_KWS_TRAD_FPOOL3 || cfg->size == TCR_KWS_ONE_FSTRIDE4;
+  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws) {
+    set_error("DS-CNN size must be 'S', 'M' or 'L', or a KWS baseline: 'P' (trad_fpool3) or 'F' (one_fstride4)");
+    return TCR_ERR_INVALID;
+  }
   if (cfg->max_batch <= 0 || cfg->height <= 0 || cfg->width <= 0 || cfg->num_classes <= 0 || cfg->num_classes > kMaxClasses) {
     set_error("bad DS-CNN configuration");
     return TCR_ERR_INVALID;
   }
+  if (cfg->size == TCR_KWS_TRAD_FPOOL3 && (cfg->height < 29 || cfg->width < 19)) {
+    return ds_fail(TCR_ERR_UNSUPPORTED, "trad_fpool3 needs height >= 29 and width >= 19 (its 20x8 conv, 1x3 pool and 10x4 conv are "
+                   "VALID), got %d x %d", cfg->height, cfg->width);
+  }
+  if (cfg->size == TCR_KWS_ONE_FSTRIDE4 && (int64_t)cfg->height * cfg->width > kKwsMaxStaged) {
+    return ds_fail(TCR_ERR_UNSUPPORTED, "one_fstride4 needs height x width <= %d (its conv stages a whole utterance in shared "
+                   "memory), got %d x %d", kKwsMaxStaged, cfg->height, cfg->width);
+  }
+  if (cfg->size == TCR_KWS_ONE_FSTRIDE4 && cfg->width < 8) {
+    return ds_fail(TCR_ERR_UNSUPPORTED, "one_fstride4 needs width >= 8 (its T x 8 conv is VALID), got %d", cfg->width);
+  }
   tcr_dscnn* d = new tcr_dscnn();
   d->cfg = *cfg;
+  d->kws = kws;
   if (const char* e = getenv("TCR_DSCNN_TC")) { d->use_tc = e[0] != '0'; d->tc_ws = e[0] != '1'; }
   struct Def { int type, depth, kh, kw, sh, sw; const char* scope; };
   std::vector<Def> defs;
@@ -1032,6 +1529,41 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   };
   int h = cfg->height, w = cfg->width, cin = 1;
   d->net.nlayers = 0;
+  if (kws) {
+    // audio_nets/kws.py create_trad_fpool3_model (204-290) / create_one_fstride4_model (408-487): top-level TF variables
+    auto conv = [&](const char* name, int cout, int kh, int kw, int sw, int pool) {
+      DsLayerDev L;
+      memset(&L, 0, sizeof(L));
+      L.type = kLayerKws; L.cin = cin; L.cout = cout; L.kh = kh; L.kw = kw; L.sh = 1; L.sw = sw; L.hin = h; L.win = w;
+      L.hout = h - kh + 1;
+      const int wconv = (w - kw) / sw + 1;
+      L.wout = wconv / pool;
+      L.w = add(name, TCR_KIND_WEIGHT, {kh, kw, cin, cout});
+      d->flops += 2ll * L.hout * wconv * kh * kw * cin * cout;
+      d->pool[d->net.nlayers] = pool;
+      d->net.layer[d->net.nlayers++] = L;
+      d->act_floats = std::max(d->act_floats, (size_t)L.hout * L.wout * cout);
+      h = L.hout; w = L.wout; cin = cout;
+    };
+    const bool trad = cfg->size == TCR_KWS_TRAD_FPOOL3;
+    if (trad) {
+      conv("first_weights", 64, 20, 8, 1, 3);
+      conv("second_weights", 64, 10, 4, 1, 1);
+    } else {
+      conv("first_weights", 186, cfg->height, 8, 4, 1);
+    }
+    KwsHead& H = d->head;
+    H.K = h * w * cin;
+    H.nsplit = (H.K + kKwsLinK - 1) / kKwsLinK;
+    H.classes = cfg->num_classes;
+    H.lin = add(trad ? "linear_weights" : "first_linear_weights", TCR_KIND_WEIGHT, {H.K, 32});
+    H.fc[0] = add("first_fc_weights", TCR_KIND_WEIGHT, {32, 128});
+    H.nfc = 1;
+    if (!trad) H.fc[H.nfc++] = add("second_fc_weights", TCR_KIND_WEIGHT, {128, 128});
+    H.out = add("final_fc_weights", TCR_KIND_WEIGHT, {128, cfg->num_classes});
+    d->flops += 2ll * H.K * 32 + 2ll * 32 * 128 + (trad ? 0 : 2ll * 128 * 128) + 2ll * 128 * cfg->num_classes;
+    defs.clear();
+  }
   for (const Def& df : defs) {
     DsLayerDev L;
     memset(&L, 0, sizeof(L));
@@ -1065,9 +1597,11 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     h = L.hout; w = L.wout; cin = df.depth;
   }
   d->net.classes = cfg->num_classes;
-  d->net.fcw = add("DSCNN/fc1/weights", TCR_KIND_WEIGHT, {cin, cfg->num_classes});
-  d->net.fcb = add("DSCNN/fc1/biases", TCR_KIND_BETA, {cfg->num_classes});
-  d->flops += 2ll * cin * cfg->num_classes;
+  if (!kws) {
+    d->net.fcw = add("DSCNN/fc1/weights", TCR_KIND_WEIGHT, {cin, cfg->num_classes});
+    d->net.fcb = add("DSCNN/fc1/biases", TCR_KIND_BETA, {cfg->num_classes});
+    d->flops += 2ll * cin * cfg->num_classes;
+  }
   d->n_params = off;
   if (cudaSetDevice(cfg->device) != cudaSuccess) { delete d; set_error("cudaSetDevice failed"); return TCR_ERR_CUDA; }
 #ifndef TCR_EMU
@@ -1079,6 +1613,16 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
       set_error("cudaMalloc failed for the DS-CNN activation buffers");
       return TCR_ERR_CUDA;
     }
+  if (kws) {
+    const DsLayerDev& L1 = d->net.layer[d->net.nlayers - 1];
+    const bool split = L1.cin == 64 && L1.cout == 64;
+    if (cudaMalloc((void**)&d->part, (size_t)d->head.nsplit * cfg->max_batch * 32 * sizeof(float)) != cudaSuccess ||
+        (split && cudaMalloc((void**)&d->bimg, (size_t)2 * L1.kh * L1.kw * 64 * 64 * sizeof(float)) != cudaSuccess)) {
+      tcr_dscnn_destroy(d);
+      set_error("cudaMalloc failed for the KWS head / filter buffers");
+      return TCR_ERR_CUDA;
+    }
+  }
   *out = d;
   return TCR_OK;
 }
@@ -1089,6 +1633,8 @@ extern "C" int tcr_dscnn_destroy(tcr_dscnn* d) {
     if (d->act[i]) cudaFree(d->act[i]);
   frontend_free(&d->fe);
   if (d->feat) cudaFree(d->feat);
+  if (d->part) cudaFree(d->part);
+  if (d->bimg) cudaFree(d->bimg);
   delete d;
   return TCR_OK;
 }
@@ -1147,6 +1693,72 @@ static int ds_launch_conv(tcr_dscnn* d, const DsLayerDev& L, const float* params
   return TCR_OK;
 }
 
+// A layer of the KWS baselines.  trad_fpool3's two convs run on wgmma at every geometry the handle accepts: conv1 + pool on
+// kws_conv1_tc_kernel, conv2 on kws_bsplit_kernel then kws_conv2_tc_kernel.  one_fstride4's conv runs on the FMA kernel, and so does
+// every layer in the emulator build, which has no wgmma.
+template <bool WIN>
+static int kws_launch_conv(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s,
+                           WindowView win) {
+  const DsLayerDev& D = d->net.layer[l];
+  KwsConv L = {D.cin, D.cout, D.kh, D.kw, D.sh, D.sw, D.hin, D.win, D.hout, D.wout, std::min(D.hout, 8), D.w};
+#ifndef TCR_EMU
+  if (D.cin == 1 && D.cout == 64 && d->pool[l] == 3 && D.sh == 1 && D.sw == 1 && D.kw % 4 == 0 && D.kh * D.kw == 8 * kC1Half) {
+    const int64_t pooled = (int64_t)n * D.hout * D.wout;
+    const int grid = (int)std::min<int64_t>((pooled + kC1Pooled - 1) / kC1Pooled, d->sms);
+    const size_t smem = conv1_tc_smem_floats(D.kh * D.kw / 4) * 4;
+    auto kfn = kws_conv1_tc_kernel<WIN>;
+    static SmemOptIn optin_c1;
+    if (optin_c1.ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_conv1_tc: shared memory opt-in failed");
+    TCR_LAUNCH(WIN ? "kws_conv1_tc:win" : "kws_conv1_tc", kfn, dim3(grid), dim3(kTcThreads), smem, s, L, (int)n, params, in, out, win);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_conv1_tc launch failed");
+    return TCR_OK;
+  }
+  if (D.cin == 64 && D.cout == 64 && (D.kh * D.kw * D.cin) % (kC2Chunk * kC2Flush) == 0 && d->bimg) {
+    const int K = D.kh * D.kw * D.cin;
+    TCR_LAUNCH("kws_bsplit", kws_bsplit_kernel, dim3((K * 64 + 255) / 256), dim3(256), 0, s, K, params + D.w, d->bimg);
+    const int64_t rows = (int64_t)n * D.hout * D.wout;
+    const int grid = (int)std::min<int64_t>((rows + 127) / 128, d->sms);
+    const size_t smem = (size_t)kC2Stages * kC2StageFloats * 4;
+    static SmemOptIn optin_tc;
+    if (optin_tc.ensure(kws_conv2_tc_kernel, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_conv2_tc: shared memory opt-in failed");
+    TCR_LAUNCH("kws_conv2_tc", kws_conv2_tc_kernel, dim3(grid), dim3(kC2Threads), smem, s, L, (int)n, d->bimg, in, out);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_conv2_tc launch failed");
+    return TCR_OK;
+  }
+#endif
+  const size_t smem = (size_t)kws_stage_floats(L) * 4;
+  if (smem > kKwsMaxStaged * sizeof(float))
+    return ds_fail(TCR_ERR_UNSUPPORTED, "KWS layer %d: %zu bytes of input rows do not fit in shared memory", l, smem);
+  const int tiles = (int)((int64_t)n * ((D.hout + L.RH - 1) / L.RH));
+  // a pooled layer (trad_fpool3's first, in the emulator build): 4 channels x 2 rows x 2 pooled columns (x 3) per thread; any
+  // other (one_fstride4's single output row of 186 channels; conv2 in the emulator build): one channel x 5 columns
+  const bool pooled = d->pool[l] == 3;
+  if (!pooled && d->pool[l] != 1) return ds_fail(TCR_ERR_UNSUPPORTED, "KWS layer %d: pooling by %d", l, d->pool[l]);
+  if (pooled && D.cout % 4) return ds_fail(TCR_ERR_UNSUPPORTED, "KWS layer %d: a pooled layer needs a multiple of 4 channels", l);
+  auto kfn = pooled ? kws_conv_kernel<3, 4, 2, 2, WIN> : kws_conv_kernel<1, 1, 1, 5, WIN>;
+#ifndef TCR_EMU
+  static SmemOptIn optin3, optin1;
+  if ((pooled ? optin3 : optin1).ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_conv: shared memory opt-in failed");
+#endif
+  TCR_LAUNCH(WIN ? "kws_conv:win" : "kws_conv", kfn, dim3(tiles), dim3(256), smem, s, L, params, in, out, win);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_conv launch failed");
+  return TCR_OK;
+}
+
+// flatten -> lin (split over K) -> the 128-wide matrices -> logits, softmax
+static int kws_head(tcr_dscnn* d, const float* params, const float* in, int n, float* logits, float* probs, cudaStream_t s) {
+  const KwsHead& H = d->head;
+#ifndef TCR_EMU
+  static SmemOptIn optin;
+  if (optin.ensure(kws_lin_kernel, kKwsLinSmem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_lin: shared memory opt-in failed");
+#endif
+  TCR_LAUNCH("kws_lin", kws_lin_kernel, dim3(H.nsplit * ((n + kKwsLinU - 1) / kKwsLinU)), dim3(256), kKwsLinSmem, s, H, n, params, in,
+             d->part);
+  TCR_LAUNCH("kws_head", kws_head_kernel, dim3((n + kKwsHeadU - 1) / kKwsHeadU), dim3(128), 0, s, H, n, params, d->part, logits, probs);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "KWS head launch failed");
+  return TCR_OK;
+}
+
 // Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC), or for l == 0 with `win` the windows it describes.
 // The kernel is chosen here, once for every entry point: wgmma where the layer's shape fits the tensor-core kernels
 // (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.  The warp-specialised block kernel reads its input through a TMA map
@@ -1155,6 +1767,10 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
                            const WindowView* win = nullptr) {
   const DsLayerDev& L = d->net.layer[l];
   const float eps = 1e-3f;
+  if (L.type == kLayerKws) {
+    if (win) return kws_launch_conv<true>(d, l, params, in, out, n, s, *win);
+    return kws_launch_conv<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
+  }
   if (L.type == 0) {
     if (win) return ds_launch_conv<true>(d, L, params, in, out, n, s, *win);
     return ds_launch_conv<false>(d, L, params, in, out, n, s, WindowView{0, 0, 0});
@@ -1223,6 +1839,7 @@ int tcr::dscnn_forward(tcr_dscnn* d, const float* feat, const float* params, int
     if (rc != TCR_OK) return rc;
     in = out;
   }
+  if (d->kws) return kws_head(d, params, in, n, logits, probs, s);
   const DsLayerDev& last = d->net.layer[d->net.nlayers - 1];
   if (last.cout > 320) { set_error("DS-CNN head supports up to 320 channels"); return TCR_ERR_UNSUPPORTED; }
   TCR_LAUNCH("dscnn_head", dscnn_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes, d->net.fcw,
@@ -1239,16 +1856,6 @@ extern "C" int tcr_dscnn_forward(tcr_dscnn* d, const float* features, const floa
   if (!d || !features || !params) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   if (n <= 0 || n > d->cfg.max_batch) { set_error("n outside [1, max_batch]"); return TCR_ERR_INVALID; }
   return dscnn_forward(d, features, params, n, logits, probs, (cudaStream_t)stream, nullptr);
-}
-
-static int ds_fail(int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  set_error(buf);
-  return code;
 }
 
 extern "C" int tcr_dscnn_set_frontend(tcr_dscnn* d, const tcr_config* cfg) {

@@ -1,5 +1,6 @@
 """DS-CNN forward (inference) on the CUDA path: the reference's 2-D-conv comparison model
-(audio_nets/ds_cnn.py; DSCNN{S,M,L}Model.build_inference in factory/audio_nets.py:298-358).  Training DS-CNN is out of scope
+(audio_nets/ds_cnn.py; DSCNN{S,M,L}Model.build_inference in factory/audio_nets.py:298-358), and on the same handle the KWS
+baselines cnn-trad-fpool3 (size 'P') and cnn-one-fstride4 ('F') of audio_nets/kws.py.  Training DS-CNN is out of scope
 (SURVEY.md 2 #13): weights come from a checkpoint keyed by the TF variable names in `self.table`.
 
 With a front-end (set_frontend) the handle also takes audio: `mfcc`, `forward_input`, `eval_accumulate` and `listener` mirror
@@ -14,6 +15,9 @@ import torch
 
 from . import _lib as L
 from .engine import Listener, frontend_config, frontend_shape
+
+# tcr_dscnn_config.size of the KWS baselines (include/tcr_b200.h): KWSModel --architecture -> size code
+KWS_SIZES = {"trad_fpool3": "P", "one_fstride4": "F"}
 
 
 class DsCnn:
@@ -81,12 +85,18 @@ class DsCnn:
 
     def new_variables(self, seed: int = 0) -> torch.Tensor:
         """Flat variables as the reference initialises them before a restore: Xavier-uniform weights (slim's default), zero biases /
-        beta / moving mean, unit moving variance.  Host-side RNG, not TF's."""
+        beta / moving mean, unit moving variance; the KWS baselines ('P', 'F') draw every weight from
+        truncated_normal(stddev=0.01) (audio_nets/kws.py), values past two sigma redrawn.  Host-side RNG, not TF's."""
         rng = np.random.default_rng(seed)
         flat = np.zeros(self.num_params, np.float32)
         for d in self.table:
             sl = slice(d["offset"], d["offset"] + d["numel"])
-            if d["kind"] == "weight":
+            if d["kind"] == "weight" and self.size in KWS_SIZES.values():
+                v = rng.standard_normal(d["numel"])
+                while (bad := np.abs(v) > 2.0).any():
+                    v[bad] = rng.standard_normal(int(bad.sum()))
+                flat[sl] = (0.01 * v).astype(np.float32)
+            elif d["kind"] == "weight":
                 shp = d["shape"]
                 fan_in, fan_out = int(np.prod(shp[:-1])), int(np.prod(shp[:-2])) * shp[-1]
                 lim = np.sqrt(6.0 / (fan_in + fan_out))

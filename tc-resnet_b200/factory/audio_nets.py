@@ -4,8 +4,8 @@ executing on the CUDA engine instead of building a TF graph.
 `train_audio.py` / `evaluate_audio.py` look the class up by NAME (`eval(f"audio_nets.{args.model}")`,
 train_audio.py:32), call `Model(args, dataset)`, then `model.build(wavs, labels, is_training)` and hand the model
 to the trainer / evaluator, which touch only the attributes set here and `session.run`.  TCResNet8Model and
-TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model are on it for evaluation, deployment and streaming (their
-training is out of scope and raises NotImplementedError); the other entries of `_available_nets` (baselines the north star
+TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model and KWSModel (--architecture trad_fpool3 / one_fstride4) are on it
+for evaluation, deployment and streaming (their training is out of scope and raises NotImplementedError); the other entries of `_available_nets` (baselines the north star
 does not name) are registered so the CLI accepts them but raise NotImplementedError when built.
 """
 from __future__ import annotations
@@ -18,7 +18,7 @@ import torch
 from ..common import utils
 from ..common.model_loader import EMA_SUFFIX
 from ..datasets import preprocessor_factory
-from ..dscnn import DsCnn
+from ..dscnn import KWS_SIZES, DsCnn
 from ..engine import OPTIMIZER_DEFAULTS, OPTIMIZER_SLOT_NAMES, Engine
 from ..runtime import InvalidArgumentError, Node
 from .base import TFModel
@@ -555,7 +555,6 @@ def _baseline(name, flags):
 
 
 _TC = [("--weight_decay", 0.0001), ("--dropout_keep_prob", 0.5), ("--width_multiplier", 1.0)]
-KWSModel = _baseline("KWSModel", [("--architecture", "conv")])
 Res8Model = _baseline("Res8Model", [("--weight_decay", 0.00001)])
 Res8NarrowModel = _baseline("Res8NarrowModel", [("--weight_decay", 0.00001)])
 Res15Model = _baseline("Res15Model", [("--weight_decay", 0.00001)])
@@ -618,10 +617,14 @@ class DsCnnModel(AudioNetModel):
             values = {k: v for k, v in values.items() if restore(k)}
         self.engine.variables_from_dict(values, self.params, strict=strict, only=restore)
 
+    def _regularization(self) -> float:
+        """The regularisation term of total_loss: none in the DS-CNN graph."""
+        return 0.0
+
     def execute(self, names: Set[str], feed) -> Dict[str, object]:
         """One evaluation session.run: the batch from the dataset, the forward from its samples, the device counts when
-        `metric_counts` is fetched, and total_loss = model_loss = the batch's mean softmax cross-entropy (label smoothing as
-        --label_smoothing; the DS-CNN graph has no regularisation loss), from the logits in float64."""
+        `metric_counts` is fetched, and model_loss = the batch's mean softmax cross-entropy (label smoothing as --label_smoothing),
+        from the logits in float64; total_loss = model_loss + _regularization()."""
         if "train_op" in names:
             raise NotImplementedError(f"{type(self).__name__}: training DS-CNN is out of scope on the CUDA path")
         wav_np, hot_np = self.dataset.next_batch()
@@ -644,8 +647,8 @@ class DsCnnModel(AudioNetModel):
         target = hot_np.astype(np.float64) * (1.0 - ls) + ls / lg.shape[1]
         mx = lg.max(axis=1, keepdims=True)
         logp = lg - mx - np.log(np.exp(lg - mx).sum(axis=1, keepdims=True))
-        loss = np.float32(-(target * logp).sum(axis=1).mean())
-        vals.update(total_loss=loss, model_loss=loss, global_step=np.int64(self.global_step), labels=hot_np, audio_original=wav_np)
+        ce = -(target * logp).sum(axis=1).mean()
+        vals.update(total_loss=np.float32(ce + self._regularization()), model_loss=np.float32(ce), global_step=np.int64(self.global_step), labels=hot_np, audio_original=wav_np)
         if "outputs" in names or "logits" in names:
             vals["outputs"], vals["logits"] = probs.cpu().numpy(), lg.astype(np.float32)
         if "audio" in names:
@@ -664,3 +667,39 @@ class DSCNNMModel(DsCnnModel):
 
 class DSCNNLModel(DsCnnModel):
     dscnn_size = "L"
+
+
+# KWSModel --architecture choices (factory/audio_nets.py:222-224); KWS_SIZES names the two on the CUDA path
+KWS_ARCHITECTURES = ["single_fc", "conv", "low_latency_conv", "low_latency_svdf", "tiny_conv", "one_fstride4", "trad_fpool3"]
+
+
+class KWSModel(DsCnnModel):
+    """KWSModel (factory/audio_nets.py:205-224, audio_nets/kws.py) for --architecture trad_fpool3 and one_fstride4, the two Sainath &
+    Parada CNNs of the reference's recipes, in evaluation mode on the DS-CNN handle (size codes 'P' / 'F', dscnn.KWS_SIZES).  The
+    variables are top-level TF names ("first_weights", ...).  --weight_decay keeps TFModel's default of 1e-4, and total_loss adds
+    the reference's L2 term over every weight (build_loss: weight_decay * sum(tf.nn.l2_loss(w))).  The other five architectures and
+    training are out of scope."""
+
+    @staticmethod
+    def add_arguments(parser):
+        parser.add_argument("--architecture", default="conv", type=str, choices=KWS_ARCHITECTURES)
+
+    @property
+    def dscnn_size(self) -> str:
+        arch = self.args.architecture
+        if arch not in KWS_SIZES:
+            raise NotImplementedError(f"KWSModel --architecture {arch} is not on the CUDA path; supported: "
+                                      + ", ".join(KWS_SIZES))
+        return KWS_SIZES[arch]
+
+    def build_inference(self, inputs, is_training=True):
+        self.dscnn_size                                          # an unsupported architecture is refused first
+        if is_training:
+            raise NotImplementedError(f"KWSModel --architecture {self.args.architecture}: training the KWS baselines is out of "
+                                      "scope on the CUDA path; evaluation (evaluate_audio.py), the deployable model and the "
+                                      "listener (listen_audio.py) are supported")
+        return super().build_inference(inputs, is_training=False)
+
+    def _regularization(self) -> float:
+        wd = float(self.args.weight_decay)
+        return wd * 0.5 * float((self.params.double() ** 2).sum()) if wd else 0.0

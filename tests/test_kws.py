@@ -1,0 +1,263 @@
+"""The KWS baselines (KWSModel --architecture trad_fpool3 / one_fstride4, audio_nets/kws.py) on the DS-CNN handle, without a GPU:
+the parameter table and FLOPs, the oracle against an independent torch restatement, the refusals, every FMA kernel on the CPU
+emulator against the oracle, the arithmetic of conv2's 3xTF32 wgmma kernel, and the Python surface."""
+import ctypes as C
+import os
+import shlex
+
+import numpy as np
+import pytest
+import torch
+import torch.nn.functional as F
+
+from oracle import kws_oracle as K
+from tcr_harness import NumpyBackend, rel_err
+
+import tcresnet_b200  # noqa: F401
+from tcresnet_b200 import _lib as L
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+TCR_ERR_INVALID, TCR_ERR_UNSUPPORTED = 1, 3           # include/tcr_b200.h
+
+
+@pytest.fixture(scope="module")
+def emu():
+    return NumpyBackend()
+
+
+def create(lib, arch, h, w, max_batch=4, classes=12):
+    handle = C.c_void_p()
+    rc = lib.tcr_dscnn_create(C.byref(L.TcrDscnnConfig(ord(K.CODES.get(arch, arch)), h, w, classes, max_batch, 0)), C.byref(handle))
+    return rc, handle
+
+
+def table(lib, handle):
+    descs, count, nparams, flops = C.POINTER(L.TcrParamDesc)(), C.c_int32(), C.c_int64(), C.c_int64()
+    L.check(lib, lib.tcr_dscnn_param_table(handle, C.byref(descs), C.byref(count), C.byref(nparams), C.byref(flops)), "table")
+    rows = [(descs[i].name.decode(), tuple(descs[i].shape[:descs[i].rank]), descs[i].kind) for i in range(count.value)]
+    return rows, nparams.value, flops.value
+
+
+def expected_table(arch, T, Fq, classes=12):
+    """The issue's formulas: H1 = T - 19, W1 = F - 7, Wp = W1 // 3, H2 = H1 - 9, W2 = Wp - 3 (trad); W = (F - 8) // 4 + 1 (fstride4)."""
+    if arch == "trad_fpool3":
+        H1, W1 = T - 19, Fq - 7
+        Wp = W1 // 3
+        H2, W2 = H1 - 9, Wp - 3
+        k = H2 * W2 * 64
+        rows = [("first_weights", (20, 8, 1, 64)), ("second_weights", (10, 4, 64, 64)), ("linear_weights", (k, 32)),
+                ("first_fc_weights", (32, 128)), ("final_fc_weights", (128, classes))]
+        flops = 2 * H1 * W1 * 160 * 64 + 2 * H2 * W2 * 2560 * 64 + 2 * k * 32 + 2 * 32 * 128 + 2 * 128 * classes
+    else:
+        W = (Fq - 8) // 4 + 1
+        k = W * 186
+        rows = [("first_weights", (T, 8, 1, 186)), ("first_linear_weights", (k, 32)), ("first_fc_weights", (32, 128)),
+                ("second_fc_weights", (128, 128)), ("final_fc_weights", (128, classes))]
+        flops = 2 * W * T * 8 * 186 + 2 * k * 32 + 2 * 32 * 128 + 2 * 128 * 128 + 2 * 128 * classes
+    return rows, sum(int(np.prod(s)) for _, s in rows), flops
+
+
+@pytest.mark.parametrize("arch", ["trad_fpool3", "one_fstride4"])
+@pytest.mark.parametrize("T,Fq", [(49, 40), (98, 40), (49, 64)])
+def test_parameter_table_and_flops(emu, arch, T, Fq):
+    rc, h = create(emu.lib, arch, T, Fq)
+    assert rc == 0
+    try:
+        rows, nparams, flops = table(emu.lib, h)
+        exp_rows, exp_params, exp_flops = expected_table(arch, T, Fq)
+        assert [(n, s) for n, s, _ in rows] == exp_rows
+        assert all(L.KIND_NAMES[kind] == "weight" for _, _, kind in rows)
+        assert (nparams, flops) == (exp_params, exp_flops)
+        spec = K.build_spec(arch, T, Fq)
+        assert spec.var_names == [n for n, _ in exp_rows] and K.forward_flops(spec) == flops
+        if (T, Fq) == (49, 40):
+            assert (nparams, flops) == {"trad_fpool3": (523776, 76024832), "one_fstride4": (148496, 1463584)}[arch]
+    finally:
+        emu.lib.tcr_dscnn_destroy(h)
+
+
+def test_trad_fpool3_flop_split():
+    """conv1 20,275,200, conv2 55,050,240, lin 688,128, fc 8,192, out 3,072 at 49 x 40."""
+    assert 2 * 30 * 33 * 160 * 64 == 20275200 and 2 * 21 * 8 * 2560 * 64 == 55050240 and 2 * 10752 * 32 == 688128
+    assert 20275200 + 55050240 + 688128 + 8192 + 3072 == 76024832
+
+
+@pytest.mark.parametrize("arch,T,Fq", [("trad_fpool3", 49, 40), ("trad_fpool3", 29, 19), ("one_fstride4", 49, 40),
+                                       ("one_fstride4", 49, 11)])
+def test_oracle_matches_independent_torch_restatement(arch, T, Fq):
+    spec = K.build_spec(arch, T, Fq)
+    p = K.init_variables(spec, 0)
+    x = np.random.RandomState(1).randn(3, T, Fq)
+    t = torch.tensor(x)[:, None]                                       # NCHW
+    acts = []
+    for name, stride, pool in spec.convs:
+        t = F.relu(F.conv2d(t, torch.tensor(p[name]).permute(3, 2, 0, 1), stride=stride))
+        if pool > 1:
+            t = F.max_pool2d(t, (1, pool), (1, pool))
+        acts.append(t.permute(0, 2, 3, 1).numpy())
+    y = t.permute(0, 2, 3, 1).reshape(3, -1)
+    for m in spec.mats:
+        y = y @ torch.tensor(p[m])
+    ref = y.numpy()
+    got = K.forward(spec, p, x)
+    assert rel_err(got, ref) <= 1e-12
+    for l, (a, r) in enumerate(zip(K.forward_layers(spec, p, x), acts)):
+        assert a.shape == r.shape == (3,) + K.conv_geometry(arch, T, Fq)[l]
+        assert rel_err(a, r) <= 1e-12, l
+
+
+def _err(lib):
+    return lib.tcr_last_error().decode()
+
+
+def test_refusals(emu):
+    lib = emu.lib
+    for arch, T, Fq, bound in (("trad_fpool3", 28, 40, "height >= 29"), ("trad_fpool3", 49, 18, "width >= 19"),
+                               ("one_fstride4", 49, 7, "width >= 8"), ("one_fstride4", 400, 129, "height x width <= 51200")):
+        rc, h = create(lib, arch, T, Fq)
+        assert rc == TCR_ERR_UNSUPPORTED and bound in _err(lib) and not h.value, (arch, T, Fq, _err(lib))
+    for arch, T, Fq in (("trad_fpool3", 29, 19), ("one_fstride4", 1, 8), ("one_fstride4", 400, 128)):   # accepted extremes
+        rc, h = create(lib, arch, T, Fq)
+        assert rc == 0
+        lib.tcr_dscnn_destroy(h)
+    rc, h = create(lib, "Q", 49, 40)
+    assert rc == TCR_ERR_INVALID and "'P' (trad_fpool3) or 'F' (one_fstride4)" in _err(lib)
+    rc, h = create(lib, "trad_fpool3", 49, 40)
+    try:
+        lis = C.c_void_p()
+        assert lib.tcr_dscnn_listener_create(h, C.byref(L.TcrListenerConfig(1, 1, 320)), C.byref(lis)) == TCR_ERR_INVALID
+        assert "no front-end" in _err(lib)
+    finally:
+        lib.tcr_dscnn_destroy(h)
+
+
+class KwsNet:
+    """One KWS handle with the oracle's seeded variables on a tests/tcr_harness backend."""
+
+    def __init__(self, b, arch, T, Fq, max_batch, seed=0):
+        self.b, self.lib, self.arch = b, b.lib, arch
+        self.spec = K.build_spec(arch, T, Fq)
+        self.p = K.init_variables(self.spec, seed)
+        rc, self.h = create(self.lib, arch, T, Fq, max_batch)
+        L.check(self.lib, rc, "tcr_dscnn_create")
+        self.params = b.upload(K.flatten(self.spec, self.p))
+
+    def close(self):
+        self.lib.tcr_dscnn_destroy(self.h)
+
+    def forward(self, feat):
+        b, n = self.b, feat.shape[0]
+        d_feat, logits, probs = b.upload(feat), b.empty(n, 12), b.empty(n, 12)
+        L.check(self.lib, self.lib.tcr_dscnn_forward(self.h, b.ptr(d_feat), b.ptr(self.params), n, b.ptr(logits), b.ptr(probs),
+                                                     b.stream), "tcr_dscnn_forward")
+        b.sync()
+        return b.download(logits), b.download(probs)
+
+    def layer_output(self, feat, k):
+        """Output of conv layer k - 1 (tcr_dscnn_forward_partial) with one utterance of NaN padding after it."""
+        b, n = self.b, feat.shape[0]
+        shape = K.conv_geometry(self.arch, self.spec.h, self.spec.w)[k - 1]
+        d_feat, out = b.upload(feat), b.empty(n + 1, *shape)
+        L.check(self.lib, self.lib.tcr_dscnn_forward_partial(self.h, b.ptr(d_feat), b.ptr(self.params), n, k, b.ptr(out), b.stream),
+                "tcr_dscnn_forward_partial")
+        b.sync()
+        got = b.download(out)
+        assert np.isnan(got[n]).all(), f"layer {k - 1} stored past the last utterance"
+        assert np.isfinite(got[:n]).all(), f"layer {k - 1} left positions unwritten"
+        return got[:n]
+
+
+def check_net(net, feat, layer_output=None):
+    """Each conv layer on the path's own input to it against kws_oracle.layer, within 1e-5 of the layer's maximum (layer_output(k):
+    the path's output of layer k - 1, net.layer_output by default), then logits and softmax against the fp64 oracle within 1e-4,
+    with the arg-max equal wherever the oracle's top-2 margin exceeds the error."""
+    spec, p = net.spec, net.p
+    layer_output = layer_output or (lambda k: net.layer_output(feat, k))
+    errs, x = [], feat.astype(np.float64)
+    for k in range(1, len(spec.convs) + 1):
+        out = layer_output(k)
+        errs.append(rel_err(out, K.layer(spec, p, k - 1, x)))
+        x = out.astype(np.float64)
+    assert max(errs) <= 1e-5, errs
+    logits, probs = net.forward(feat)
+    ref = K.forward(spec, p, feat.astype(np.float64))
+    err = np.abs(logits - ref).max()
+    assert err <= 1e-4 * np.abs(ref).max(), err / np.abs(ref).max()
+    e = np.exp(ref - ref.max(1, keepdims=True))
+    # a softmax moves by at most twice its logits' largest change: on the larger logits of MFCC input that exceeds 2e-5
+    np.testing.assert_allclose(probs, e / e.sum(1, keepdims=True), atol=max(2e-5, 2 * err))
+    top2 = np.sort(ref, 1)[:, -2:]
+    clear = top2[:, 1] - top2[:, 0] > 2 * err
+    assert np.array_equal(logits.argmax(1)[clear], ref.argmax(1)[clear])
+    return errs
+
+
+@pytest.mark.parametrize("arch,T,Fq,n", [("one_fstride4", 49, 40, 3), ("one_fstride4", 98, 40, 2), ("trad_fpool3", 29, 19, 3),
+                                         ("trad_fpool3", 49, 40, 1)])
+def test_emulated_forward_matches_oracle(emu, arch, T, Fq, n):
+    """The FMA kernels (kws_conv for every conv layer here, kws_lin at K = 10,752 for trad_fpool3 49 x 40, kws_head) on the CPU
+    emulator, layer by layer and end to end."""
+    net = KwsNet(emu, arch, T, Fq, n)
+    try:
+        check_net(net, np.random.RandomState(n).randn(n, T, Fq).astype(np.float32))
+    finally:
+        net.close()
+
+
+def _tf32(a):
+    return (np.ascontiguousarray(a, np.float32).view(np.uint32) & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+def _split(a):
+    hi = _tf32(a)
+    return hi.astype(np.float64), _tf32(np.float32(a) - hi).astype(np.float64)
+
+
+def test_conv2_3xtf32_split_meets_the_layer_bound():
+    """NumPy emulation of kws_conv2_tc's arithmetic at K = 2,560 on trad_fpool3's own conv1 output: TF32 products of split
+    operands, lo*hi + hi*lo + hi*hi.  Three passes land well inside the 1e-5 per-layer bound the GPU test holds the kernel to;
+    dropping any one pass misses it."""
+    spec = K.build_spec("trad_fpool3", 49, 40)
+    p = K.init_variables(spec, 0)
+    feat = np.random.RandomState(2).randn(2, 49, 40)
+    a = K.layer(spec, p, 0, feat).astype(np.float32)                   # conv2's input as the GPU holds it
+    ref = K.layer(spec, p, 1, a.astype(np.float64))
+    (a_hi, a_lo), (w_hi, w_lo) = _split(a), _split(p["second_weights"])
+    mm = {(i, j): K._conv_valid(u, v, (1, 1)) for i, u in enumerate((a_hi, a_lo)) for j, v in enumerate((w_hi, w_lo)) if i + j < 2}
+    err = {name: rel_err(np.maximum(sum(mm[t] for t in terms), 0), ref) for name, terms in
+           (("3", [(1, 0), (0, 1), (0, 0)]), ("no lo*hi", [(0, 1), (0, 0)]), ("no hi*lo", [(1, 0), (0, 0)]),
+            ("no hi*hi", [(1, 0), (0, 1)]))}
+    assert err["3"] < 1e-6, err
+    assert min(err["no lo*hi"], err["no hi*lo"], err["no hi*hi"]) > 1e-5, err
+
+
+def _recipe_lines():
+    return [x for x in open(os.path.join(ROOT, "tests", "golden", "reference_recipes.txt")) if x.rstrip().split()[-2:-1] ==
+            ["--architecture"]]
+
+
+def test_kws_recipe_lines_parse():
+    from tcresnet_b200 import evaluate_audio, train_audio
+    lines = _recipe_lines()
+    assert len(lines) == 6
+    for line in lines:
+        mod = train_audio if line.startswith("python train_audio.py") else evaluate_audio
+        args = mod.parse_arguments(shlex.split(line)[2:])
+        assert args.model == "KWSModel" and args.architecture in ("trad_fpool3", "one_fstride4")
+        assert args.weight_decay == 1e-4 and args.num_mfccs == 40
+
+
+def test_unsupported_architecture_and_training_raise():
+    from tcresnet_b200 import evaluate_audio, train_audio
+    from tcresnet_b200.factory import audio_nets
+    from tcresnet_b200.runtime import Node
+    lines = _recipe_lines()
+    ev = [x for x in lines if x.startswith("python evaluate_audio.py")][0]
+    args = evaluate_audio.parse_arguments(shlex.split(ev)[2:-1] + ["conv"])
+    assert args.architecture == "conv"
+    with pytest.raises(NotImplementedError, match="conv is not on the CUDA path; supported: trad_fpool3, one_fstride4"):
+        audio_nets.KWSModel(args, None).build(Node("wav", [None, 16000, 1]), Node("labels", [None, 12]), is_training=False)
+    tr = [x for x in lines if x.startswith("python train_audio.py") and x.rstrip().endswith("trad_fpool3")][0]
+    args = train_audio.parse_arguments(shlex.split(tr)[2:])
+    with pytest.raises(NotImplementedError, match="training the KWS baselines is out of scope.*evaluation"):
+        audio_nets.KWSModel(args, None).build(Node("wav", [None, 16000, 1]), Node("labels", [None, 12]), is_training=True)
