@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 12
+#define TCR_ABI_VERSION 13
 
 enum {
   TCR_OK = 0,
@@ -421,17 +421,34 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
  * Their variables are top-level TF names ("first_weights", ...), all of kind TCR_KIND_WEIGHT; below the geometry bound create
  * returns TCR_ERR_UNSUPPORTED, naming it.  Every tcr_dscnn_* entry point below serves them unchanged; forward_partial's layers
  * are [conv1 + pool, conv2] for 'P' and [conv] for 'F', each written NHWC ([n, hout, wout, cout], the pooled width for 'P''s
- * first), and, as for DS-CNN, the head is not among them. */
+ * first), and, as for DS-CNN, the head is not among them.
+ *
+ * And the paper's 2-D ablations of TC-ResNet8 (audio_nets/tc_resnet.py ResNet2D8 / ResNet2D8Pool), evaluation mode (ABI 13):
+ *   size TCR_RES2D8 ('R'): conv0 3x3 1 -> c0 + BN + ReLU, then three residual blocks of c1, c2, c3 channels: conv{i}_0 3x3 at stride
+ *     s + BN + ReLU, conv{i}_1 3x3 + BN, plus the shortcut, then ReLU.  Where a block changes the channel count, s = 2 and the
+ *     shortcut is down (1x1 / stride 2 + BN + ReLU); else s = 1 and the shortcut is the block's input.  Then the global average
+ *     pool, fc (1x1, no bias) and softmax.  Every conv is TF SAME (leading pad = total // 2) and bias-free; BatchNorm has gamma,
+ *     eps 1e-3, the moving statistics.
+ *   size TCR_RES2D8_POOL ('A'): the same with a 4x4 / stride 4 VALID average pool after conv0.  Needs height >= 4 and width >= 4.
+ *   Channels: [c0, c1, c2, c3] = int(x * width_multiplier) of [16, 24, 32, 48], then c0 = int((3 width c1 + 10 c1 c2) /
+ *   (9 + 10 c2)); every count must be in [1, 128].
+ * Variables as tcr_param_table's TCResNet8 rows under the scope "ResNet2D8" / "ResNet2D8Pool", with 2-D shapes ("ResNet2D8/
+ * conv0/weights" [3, 3, 1, c0], ".../block0/down/weights" [1, 1, c0, c1], ".../conv0/BatchNorm/gamma", ..., ".../fc/weights"
+ * [1, 1, c3, classes], ".../fc2/weights" [1, 1, c3, 2], then the moving statistics); fc2 is loaded but not computed.
+ * forward_partial's layers are [conv0 (+ pool), block0, block1, block2], each NHWC. */
 #define TCR_KWS_TRAD_FPOOL3 'P'
 #define TCR_KWS_ONE_FSTRIDE4 'F'
+#define TCR_RES2D8 'R'
+#define TCR_RES2D8_POOL 'A'
 typedef struct tcr_dscnn tcr_dscnn;
 typedef struct tcr_dscnn_config {
-  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 */
+  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 | TCR_RES2D8 | TCR_RES2D8_POOL */
   int32_t height;        /* frames, 49 */
   int32_t width;         /* coefficients, 40 (10 in the reference's DS-CNN recipes) */
   int32_t num_classes;   /* 12 */
   int32_t max_batch;
   int32_t device;
+  double width_multiplier; /* TCR_RES2D8 / TCR_RES2D8_POOL only (0 means 1.0); must be 0 for the other sizes.  ABI 13 */
 } tcr_dscnn_config;
 int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out);
 int tcr_dscnn_destroy(tcr_dscnn* d);

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtcr_b200.so")
 
 TCR_MODEL_TCRESNET8 = 8
 TCR_MODEL_TCRESNET14 = 14
-ABI_VERSION = 12       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
+ABI_VERSION = 13       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
 TCR_INPUT_WAV_F32, TCR_INPUT_FEATURES, TCR_INPUT_WAV_PCM16 = 0, 1, 2
 TCR_OPT_MOMENTUM, TCR_OPT_ADAM, TCR_OPT_RMSPROP = 0, 1, 2
 TCR_FEATURE_MFCC = 0
@@ -59,7 +59,7 @@ class TcrKernelStat(C.Structure):
 
 class TcrDscnnConfig(C.Structure):
     _fields_ = [("size", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("num_classes", C.c_int32),
-                ("max_batch", C.c_int32), ("device", C.c_int32)]
+                ("max_batch", C.c_int32), ("device", C.c_int32), ("width_multiplier", C.c_double)]
 
 
 class TcrStepArgs(C.Structure):

@@ -10,7 +10,8 @@
 //   dscnn_head_kernel      global average pool + fully connected (+bias) + softmax
 // and the KWS baselines of audio_nets/kws.py on the same handle (sizes 'P' trad_fpool3, 'F' one_fstride4): kws_conv_kernel (FMA
 // first layers), kws_bsplit_kernel + kws_conv2_tc_kernel (trad_fpool3's 64 -> 64 conv on wgmma), kws_lin_kernel + kws_head_kernel
-// (the dense head).
+// (the dense head); and the 2-D ablations of TC-ResNet8 ('R' ResNet2D8, 'A' ResNet2D8Pool): res2d_conv0_kernel (conv0, the pool
+// fused), res2d_block_kernel (one fused residual block), res2d_head_kernel (dscnn_head without the bias).
 // BatchNorm here has no gamma (slim default scale=False) and uses the moving statistics; bias + BN fold into one
 // per-channel (scale, shift) pair computed while staging.
 #ifndef TCR_EMU
@@ -30,7 +31,8 @@
 namespace tcr {
 
 struct DsLayerDev {
-  int type;                 // 0 conv, 1 separable, 2 (kLayerKws) VALID bias-free conv + ReLU of the KWS baselines
+  int type;                 // 0 conv, 1 separable, 2 (kLayerKws) VALID bias-free conv + ReLU of the KWS baselines, 3 (kLayerRes2d)
+                            // a layer of the 2-D ablations (its R2Conv0 / R2Block is in the handle)
   int cin, cout, kh, kw, sh, sw, hin, win, hout, wout, pt, pl;
   int64_t w, b, beta, mm, mv;                // conv / depthwise
   int64_t pw, pb, pbeta, pmm, pmv;           // pointwise (separable only)
@@ -38,6 +40,7 @@ struct DsLayerDev {
 
 constexpr int kDsMaxLayers = 8;
 constexpr int kLayerKws = 2;
+constexpr int kLayerRes2d = 3;
 struct DsNet {
   int nlayers, n, classes;
   DsLayerDev layer[kDsMaxLayers];
@@ -1172,9 +1175,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) kws_conv1_tc_kernel(KwsConv L, 
 #endif
 
 // ---- head: one CTA per utterance ----
-__global__ void __launch_bounds__(256) dscnn_head_kernel(int npos, int C, int classes, int64_t fcw, int64_t fcb,
-                                                         const float* __restrict__ params, const float* __restrict__ in,
-                                                         float* __restrict__ logits, float* __restrict__ probs) {
+// Global average pool, fully connected layer and softmax; BIAS = false is the bias-free fc of the 2-D ablations (res2d_head_kernel).
+template <bool BIAS>
+__device__ __forceinline__ void dscnn_head(int npos, int C, int classes, int64_t fcw, int64_t fcb, const float* __restrict__ params,
+                                           const float* __restrict__ in, float* __restrict__ logits, float* __restrict__ probs) {
   pdl_wait();
   __shared__ __align__(16) float s_red[1024];
   __shared__ float s_pool[320];
@@ -1212,7 +1216,7 @@ __global__ void __launch_bounds__(256) dscnn_head_kernel(int npos, int C, int cl
   }
   __syncthreads();
   if (tid < classes) {
-    float acc = params[fcb + tid];
+    float acc = BIAS ? params[fcb + tid] : 0.f;
     for (int k = 0; k < C; ++k) acc = fmaf(s_pool[k], params[fcw + (int64_t)k * classes + tid], acc);
     s_logit[tid] = acc;
     if (logits) logits[(size_t)n * classes + tid] = acc;
@@ -1225,6 +1229,11 @@ __global__ void __launch_bounds__(256) dscnn_head_kernel(int npos, int C, int cl
     for (int k = 0; k < classes; ++k) se += expf(s_logit[k] - mx);
     probs[(size_t)n * classes + tid] = expf(s_logit[tid] - mx) / se;
   }
+}
+__global__ void __launch_bounds__(256) dscnn_head_kernel(int npos, int C, int classes, int64_t fcw, int64_t fcb,
+                                                         const float* __restrict__ params, const float* __restrict__ in,
+                                                         float* __restrict__ logits, float* __restrict__ probs) {
+  dscnn_head<true>(npos, C, classes, fcw, fcb, params, in, logits, probs);
 }
 
 // ---- KWS baselines: FMA convolution, one CTA per (utterance, tile of L.RH output rows), blockIdx.x = n * tiles + tile ----
@@ -1397,6 +1406,239 @@ __global__ void __launch_bounds__(128) kws_head_kernel(KwsHead H, int n, const f
   }
 }
 
+// ---- ResNet2D8 / ResNet2D8Pool: the paper's 2-D ablations of TC-ResNet8 (audio_nets/tc_resnet.py:6-54, 73-101, debug_2d) ----
+// Evaluation mode.  No conv has a bias, and BatchNorm has gamma (TCResNet_arg_scope: center and scale):
+// (beta, gamma, moving mean, moving variance) fold into scale = gamma / sqrt(var + eps) and shift = beta - mean * scale.
+// Channel counts need not be multiples of 4 (conv0 has 23 at 98 x 40): the block kernel's shared-memory tiles pad them to a
+// multiple of 4 with zeros, and zero scale and shift keep the padded intermediate channels at 0.
+constexpr int kR2MaxChannels = 128;
+struct R2Bn { int64_t beta, gamma, mm, mv; };
+__device__ __forceinline__ void r2_fold(const float* p, const R2Bn& bn, int c, int C, float eps, float* sc, float* sf) {
+  float s = 0.f, t = 0.f;
+  if (c < C) {
+    s = p[bn.gamma + c] / sqrtf(p[bn.mv + c] + eps);
+    t = fmaf(-p[bn.mm + c], s, p[bn.beta + c]);
+  }
+  sc[c] = s;
+  sf[c] = t;
+}
+TCR_HD inline int r2_pad4(int c) { return (c + 3) & ~3; }
+
+// conv0: 3 x 3 / stride 1 SAME conv of the single-channel features + BN + ReLU; for ResNet2D8Pool (pool = 4) the 4 x 4 / stride 4
+// VALID average pool in the epilogue, so only the pooled map is stored.  One CTA per (utterance, tile of RH output rows),
+// blockIdx.x = n * tiles + tile.  The tile's RH * pool + 2 input rows, with SAME's one-pixel zero border, the taps and the folded
+// BatchNorm are staged in shared memory.  A thread owns one channel (its 9 taps and BatchNorm in registers) and walks output
+// positions 256 / cout apart.  WIN: utterance n is a listener window (ds_window); the border is zeros there too, never the
+// neighbouring history frames.
+struct R2Conv0 { int hin, win, hout, wout, cout, pool, RH; int64_t w; R2Bn bn; };
+TCR_HD inline size_t r2_conv0_smem_floats(const R2Conv0& L) { return (size_t)(L.RH * L.pool + 2) * (L.win + 2) + 11 * (size_t)L.cout; }
+template <bool WIN>
+__global__ void __launch_bounds__(256) res2d_conv0_kernel(R2Conv0 L, const float* __restrict__ params, const float* __restrict__ in,
+                                                          float* __restrict__ out, float eps, WindowView win) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* xs = reinterpret_cast<float*>(smem_raw);
+  const int tpu = (L.hout + L.RH - 1) / L.RH, tid = threadIdx.x;
+  const int n = blockIdx.x / tpu, h0 = (blockIdx.x - n * tpu) * L.RH, rh = imin(L.RH, L.hout - h0);
+  const int xr = L.RH * L.pool + 2, xc = L.win + 2, r0 = h0 * L.pool - 1;       // staged rows, padded width, first input row
+  float *ws = xs + xr * xc, *sc = ws + 9 * L.cout, *sf = sc + L.cout;
+  const float* src;
+  if constexpr (WIN) src = ds_window(in, n, win);
+  else src = in + (int64_t)n * L.hin * L.win;
+  for (int i = tid; i < xr * xc; i += blockDim.x) {
+    const int h = r0 + i / xc, w = i % xc - 1;
+    xs[i] = (h >= 0 && h < L.hin && w >= 0 && w < L.win) ? src[(int64_t)h * L.win + w] : 0.f;
+  }
+  for (int i = tid; i < 9 * L.cout; i += blockDim.x) ws[i] = params[L.w + i];
+  for (int c = tid; c < L.cout; c += blockDim.x) r2_fold(params, L.bn, c, L.cout, eps, sc, sf);
+  __syncthreads();
+  const float inv = 1.f / (float)(L.pool * L.pool);
+  const int c = tid % L.cout, pstep = blockDim.x / L.cout, npos = rh * L.wout;   // cout <= kR2MaxChannels < blockDim.x
+  if (tid >= pstep * L.cout) return;
+  float wk[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) wk[k] = ws[k * L.cout + c];
+  const float s = sc[c], t = sf[c];
+  int r = (tid / L.cout) / L.wout, ow = (tid / L.cout) - r * L.wout;
+  for (int pos = tid / L.cout; pos < npos; pos += pstep) {
+    float sum = 0.f;
+    for (int py = 0; py < L.pool; ++py)
+      for (int px = 0; px < L.pool; ++px) {
+        const float* xb = xs + (r * L.pool + py) * xc + ow * L.pool + px;
+        float acc = 0.f;
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+#pragma unroll
+          for (int j = 0; j < 3; ++j) acc = fmaf(xb[i * xc + j], wk[3 * i + j], acc);
+        sum += fmaxf(fmaf(acc, s, t), 0.f);
+      }
+    out[(((int64_t)n * L.hout + h0 + r) * L.wout + ow) * L.cout + c] = L.pool == 1 ? sum : sum * inv;
+    ow += pstep;
+    while (ow >= L.wout) { ow -= L.wout; ++r; }
+  }
+}
+
+// A residual block: conv_0 (3 x 3 / stride s, SAME with leading pads pt, pl) + BN + ReLU, conv_1 (3 x 3 / stride 1, SAME) + BN, the
+// shortcut (down: 1 x 1 / stride s + BN + ReLU where the channel count changes, else the input), the add and ReLU.  One CTA per
+// (utterance, tile of RH x WT output positions), blockIdx.x = n * tiles + tile.  The tile's input (rows and columns of conv_0's
+// receptive field around the RH + 2 x WT + 2 intermediate positions conv_1 reads) is staged once; conv_0's output for those
+// positions, zero outside the map (conv_1's SAME border), stays in shared memory.  The filter banks pass through shared memory in
+// slices of COT output channels, conv_0's first and then conv_1's with the matching slice of down.
+struct R2Block {
+  int cin, cout, s, hin, win, hout, wout, pt, pl, down;
+  int RH, WT, COT;
+  int64_t w0, w1, wd;
+  R2Bn bn0, bn1, bnd;
+};
+// Shared-memory layout in floats: x the input tile [xr][xc][cin padded], m the intermediate [RH + 2][WT + 2][cout padded], w one
+// filter slice ([9][cin or cout padded][COT], then down's [cin padded][COT]), tab the six folded-BatchNorm tables.
+struct R2Smem { size_t m, w, tab, floats; int xr, xc; };
+TCR_HD inline R2Smem r2_block_smem(const R2Block& B) {
+  const int cip = r2_pad4(B.cin), cop = r2_pad4(B.cout);
+  R2Smem S;
+  S.xr = (B.RH + 1) * B.s + 3;
+  S.xc = (B.WT + 1) * B.s + 3;
+  S.m = (size_t)S.xr * S.xc * cip;
+  S.w = S.m + (size_t)(B.RH + 2) * (B.WT + 2) * cop;
+  S.tab = S.w + (size_t)(9 * (cip > cop ? cip : cop) + (B.down ? cip : 0)) * B.COT;
+  S.floats = S.tab + 6 * (size_t)cop;
+  return S;
+}
+
+// K x K conv of a staged tile for one slice of cot output channels: output position p (npos of them, `cols` per row) reads the
+// [.][xc][cip] tile x0 at row (p / cols) * s + i, column (p % cols) * s + j; w is [K * K][cip][cot].  Tasks of kR2TM positions
+// (NRT apart) x 4 channels, so that one float4 of the filter feeds kR2TM positions; epi(p, cg, acc) takes each result.
+constexpr int kR2TM = 4;
+template <int K, class Epi>
+__device__ __forceinline__ void r2_conv(const float* x0, int xc, int cip, int s, int npos, int cols, const float* w, int cot, Epi epi) {
+  const int ncg = cot >> 2, NRT = (npos + kR2TM - 1) / kR2TM;
+  for (int task = threadIdx.x; task < NRT * ncg; task += blockDim.x) {
+    const int cg = task % ncg, rt = task / ncg;
+    const float* xr[kR2TM];
+#pragma unroll
+    for (int m = 0; m < kR2TM; ++m) {
+      const int p = imin(rt + m * NRT, npos - 1), r = p / cols, c = p - r * cols;
+      xr[m] = x0 + ((size_t)r * s * xc + (size_t)c * s) * cip;
+    }
+    float4 acc[kR2TM];
+#pragma unroll
+    for (int m = 0; m < kR2TM; ++m) acc[m] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int i = 0; i < K; ++i)
+      for (int j = 0; j < K; ++j) {
+        const float* wk = w + (size_t)(i * K + j) * cip * cot + 4 * cg;
+        const int xo = (i * xc + j) * cip;
+#pragma unroll 2
+        for (int ci = 0; ci < cip; ci += 4) {
+          const float4 w0 = ld4(wk + (ci + 0) * cot), w1 = ld4(wk + (ci + 1) * cot), w2 = ld4(wk + (ci + 2) * cot), w3 = ld4(wk + (ci + 3) * cot);
+#pragma unroll
+          for (int m = 0; m < kR2TM; ++m) {
+            const float4 x = ld4(xr[m] + xo + ci);
+            float4& a = acc[m];
+            a.x = fmaf(x.x, w0.x, a.x); a.y = fmaf(x.x, w0.y, a.y); a.z = fmaf(x.x, w0.z, a.z); a.w = fmaf(x.x, w0.w, a.w);
+            a.x = fmaf(x.y, w1.x, a.x); a.y = fmaf(x.y, w1.y, a.y); a.z = fmaf(x.y, w1.z, a.z); a.w = fmaf(x.y, w1.w, a.w);
+            a.x = fmaf(x.z, w2.x, a.x); a.y = fmaf(x.z, w2.y, a.y); a.z = fmaf(x.z, w2.z, a.z); a.w = fmaf(x.z, w2.w, a.w);
+            a.x = fmaf(x.w, w3.x, a.x); a.y = fmaf(x.w, w3.y, a.y); a.z = fmaf(x.w, w3.z, a.z); a.w = fmaf(x.w, w3.w, a.w);
+          }
+        }
+      }
+#pragma unroll
+    for (int m = 0; m < kR2TM; ++m)
+      if (rt + m * NRT < npos) epi(rt + m * NRT, cg, acc[m]);
+  }
+}
+
+// Filter slice: w [taps][C][CO] at params + off -> ws [taps][cp][cot], output channels co0 .. co0 + cot, zeros past C and CO.
+__device__ __forceinline__ void r2_stage_slice(float* ws, const float* params, int64_t off, int taps, int C, int cp, int CO, int co0, int cot) {
+  for (int i = threadIdx.x; i < taps * cp * cot; i += blockDim.x) {
+    const int co = i % cot, ci = (i / cot) % cp, k = i / (cot * cp);
+    ws[i] = (ci < C && co0 + co < CO) ? params[off + ((int64_t)k * C + ci) * CO + co0 + co] : 0.f;
+  }
+}
+
+__global__ void __launch_bounds__(256) res2d_block_kernel(R2Block B, const float* __restrict__ params, const float* __restrict__ in,
+                                                          float* __restrict__ out, float eps) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* smem = reinterpret_cast<float*>(smem_raw);
+  const R2Smem S = r2_block_smem(B);
+  const int cip = r2_pad4(B.cin), cop = r2_pad4(B.cout), tid = threadIdx.x;
+  const int tcols = (B.wout + B.WT - 1) / B.WT, tpu = ((B.hout + B.RH - 1) / B.RH) * tcols;
+  const int n = blockIdx.x / tpu, t = blockIdx.x - n * tpu, h0 = (t / tcols) * B.RH, w0 = (t % tcols) * B.WT;
+  const int rh = imin(B.RH, B.hout - h0), wt = imin(B.WT, B.wout - w0), mc = wt + 2;
+  float *xs = smem, *ms = smem + S.m, *ws = smem + S.w, *tab = smem + S.tab;
+  float *sc0 = tab, *sf0 = tab + cop, *sc1 = tab + 2 * cop, *sf1 = tab + 3 * cop, *scd = tab + 4 * cop, *sfd = tab + 5 * cop;
+  // input rows (h0 - 1) * s - pt + [0, xr), columns (w0 - 1) * s - pl + [0, xc): conv_0's taps for intermediate rows h0 - 1 ..
+  // h0 + RH and columns w0 - 1 .. w0 + WT; zeros outside the map and past cin
+  {
+    const int xh0 = (h0 - 1) * B.s - B.pt, xw0 = (w0 - 1) * B.s - B.pl;
+    const float* src = in + (int64_t)n * B.hin * B.win * B.cin;
+    for (int i = tid; i < S.xr * S.xc * cip; i += blockDim.x) {
+      const int c = i % cip, cell = i / cip, h = xh0 + cell / S.xc, w = xw0 + cell % S.xc;
+      xs[i] = (c < B.cin && h >= 0 && h < B.hin && w >= 0 && w < B.win) ? src[((int64_t)h * B.win + w) * B.cin + c] : 0.f;
+    }
+  }
+  for (int c = tid; c < cop; c += blockDim.x) {
+    r2_fold(params, B.bn0, c, B.cout, eps, sc0, sf0);
+    r2_fold(params, B.bn1, c, B.cout, eps, sc1, sf1);
+    if (B.down) r2_fold(params, B.bnd, c, B.cout, eps, scd, sfd);
+  }
+  // conv_0 + BN + ReLU -> ms [rh + 2][wt + 2][cop]
+  for (int co0 = 0; co0 < cop; co0 += B.COT) {
+    const int cot = imin(B.COT, cop - co0);
+    __syncthreads();                                              // the previous slice's readers are done
+    r2_stage_slice(ws, params, B.w0, 9, B.cin, cip, B.cout, co0, cot);
+    __syncthreads();
+    r2_conv<3>(xs, S.xc, cip, B.s, (rh + 2) * mc, mc, ws, cot, [&](int p, int cg, float4 a) {
+      const int r = p / mc, c = p - r * mc, h = h0 - 1 + r, w = w0 - 1 + c, co = co0 + 4 * cg;
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (h >= 0 && h < B.hout && w >= 0 && w < B.wout) v = bn_relu4(a, ld4(sc0 + co), ld4(sf0 + co));
+      st4(ms + (size_t)p * cop + co, v);
+    });
+  }
+  // conv_1 + BN, the shortcut, add, ReLU -> out
+  for (int co0 = 0; co0 < cop; co0 += B.COT) {
+    const int cot = imin(B.COT, cop - co0);
+    __syncthreads();
+    r2_stage_slice(ws, params, B.w1, 9, B.cout, cop, B.cout, co0, cot);
+    float* wd = ws + (size_t)9 * cop * cot;
+    if (B.down) r2_stage_slice(wd, params, B.wd, 1, B.cin, cip, B.cout, co0, cot);
+    __syncthreads();
+    r2_conv<3>(ms, mc, cop, 1, rh * wt, wt, ws, cot, [&](int p, int cg, float4 a) {
+      const int r = p / wt, c = p - r * wt, co = co0 + 4 * cg;
+      const float4 s1 = ld4(sc1 + co), t1 = ld4(sf1 + co);
+      float4 v = make_float4(fmaf(a.x, s1.x, t1.x), fmaf(a.y, s1.y, t1.y), fmaf(a.z, s1.z, t1.z), fmaf(a.w, s1.w, t1.w));
+      // the shortcut's input cell: output (h0 + r, w0 + c) reads input ((h0 + r) * s, (w0 + c) * s)
+      const float* xb = xs + ((size_t)((r + 1) * B.s + B.pt) * S.xc + (size_t)(c + 1) * B.s + B.pl) * cip;
+      float4 sh;
+      if (B.down) {
+        float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int ci = 0; ci < cip; ++ci) {
+          const float x = xb[ci];
+          const float4 k = ld4(wd + (size_t)ci * cot + 4 * cg);
+          d.x = fmaf(x, k.x, d.x); d.y = fmaf(x, k.y, d.y); d.z = fmaf(x, k.z, d.z); d.w = fmaf(x, k.w, d.w);
+        }
+        sh = bn_relu4(d, ld4(scd + co), ld4(sfd + co));
+      } else {
+        sh = ld4(xb + co);
+      }
+      v = make_float4(fmaxf(v.x + sh.x, 0.f), fmaxf(v.y + sh.y, 0.f), fmaxf(v.z + sh.z, 0.f), fmaxf(v.w + sh.w, 0.f));
+      float* o = out + (((int64_t)n * B.hout + h0 + r) * B.wout + w0 + c) * B.cout + co;
+      if ((B.cout & 3) == 0) {
+        st4(o, v);
+      } else {
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+        for (int k = 0; k < 4 && co + k < B.cout; ++k) o[k] = vv[k];
+      }
+    });
+  }
+}
+
+// head: global average pool, fc (no bias), softmax
+__global__ void __launch_bounds__(256) res2d_head_kernel(int npos, int C, int classes, int64_t fcw, const float* __restrict__ params,
+                                                         const float* __restrict__ in, float* __restrict__ logits, float* __restrict__ probs) {
+  dscnn_head<false>(npos, C, classes, fcw, 0, params, in, logits, probs);
+}
+
 }  // namespace tcr
 
 // ------------------------------------------------------------------------------------------------
@@ -1426,6 +1668,11 @@ struct tcr_dscnn {
   KwsHead head = {};
   float* part = nullptr;     // [head.nsplit][max_batch][32]: lin's partial sums per K chunk
   float* bimg = nullptr;     // trad_fpool3: conv2's filter bank split into hi / lo B stage images (kws_bsplit_kernel)
+  // 2-D ablations ('R', 'A'): layer 0 is conv0 (+ pool), layers 1-3 the residual blocks; fc's offset
+  bool res2d = false;
+  R2Conv0 r2conv0 = {};
+  R2Block r2block[3] = {};
+  int64_t r2fc = 0;
 };
 
 #ifndef TCR_EMU
@@ -1472,14 +1719,115 @@ static void ds_same(int len, int k, int s, int* out, int* lead) {
   *lead = total / 2;
 }
 
+// The 2-D ablations' layers and variables: conv0 (+ pool), three residual blocks, fc and the dead fc2, named and ordered as
+// tcr_param_table's TCResNet8 rows (tcr_api.cu): per conv its weights, BatchNorm beta and gamma, then fc and fc2, then the moving
+// statistics per conv.  Also each kernel's tile plan, and the refusals of what the kernels cannot run.
+template <class Add>
+static int res2d_define(tcr_dscnn* d, Add& add) {
+  const tcr_dscnn_config& c = d->cfg;
+  const bool pool = c.size == TCR_RES2D8_POOL;
+  const char* model = pool ? "ResNet2D8Pool" : "ResNet2D8";
+  const double wm = c.width_multiplier == 0.0 ? 1.0 : c.width_multiplier;
+  int ch[4] = {16, 24, 32, 48};
+  for (int& x : ch) x = (int)((double)x * wm);                     // int(x * width_multiplier), tc_resnet.py:75
+  if (ch[0] >= 1 && ch[1] >= 1)                                    // first_c, tc_resnet.py:80: exact integers, one rounded division
+    ch[0] = (int)((double)(3ll * c.width * ch[0] + 10ll * ch[0] * ch[1]) / (double)(9 + 10ll * ch[1]));
+  for (int i = 0; i < 4; ++i)
+    if (ch[i] < 1 || ch[i] > kR2MaxChannels)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "%s at width_multiplier %g and width %d needs %d channels in %s; res2d_block takes 1 to %d",
+                     model, wm, c.width, ch[i], i ? "a block" : "conv0", kR2MaxChannels);
+  struct Conv { std::string name; int k, cin, cout; int64_t w; R2Bn bn; };
+  std::vector<Conv> convs = {{"conv0", 3, 1, ch[0], 0, {}}};
+  for (int i = 0, cin = ch[0]; i < 3; cin = ch[++i]) {
+    const std::string b = "block" + std::to_string(i) + "/";
+    if (ch[i + 1] != cin) convs.push_back({b + "down", 1, cin, ch[i + 1], 0, {}});
+    convs.push_back({b + "conv" + std::to_string(i) + "_0", 3, cin, ch[i + 1], 0, {}});
+    convs.push_back({b + "conv" + std::to_string(i) + "_1", 3, ch[i + 1], ch[i + 1], 0, {}});
+  }
+  const std::string scope = std::string(model) + "/";
+  for (Conv& cv : convs) {
+    cv.w = add(scope + cv.name + "/weights", TCR_KIND_WEIGHT, {cv.k, cv.k, cv.cin, cv.cout});
+    cv.bn.beta = add(scope + cv.name + "/BatchNorm/beta", TCR_KIND_BETA, {cv.cout});
+    cv.bn.gamma = add(scope + cv.name + "/BatchNorm/gamma", TCR_KIND_GAMMA, {cv.cout});
+  }
+  d->r2fc = add(scope + "fc/weights", TCR_KIND_WEIGHT, {1, 1, ch[3], c.num_classes});
+  add(scope + "fc2/weights", TCR_KIND_WEIGHT, {1, 1, ch[3], 2});
+  for (Conv& cv : convs) {
+    cv.bn.mm = add(scope + cv.name + "/BatchNorm/moving_mean", TCR_KIND_MOVING_MEAN, {cv.cout});
+    cv.bn.mv = add(scope + cv.name + "/BatchNorm/moving_variance", TCR_KIND_MOVING_VAR, {cv.cout});
+  }
+  auto layer = [&](int hin, int win, int hout, int wout, int cin, int cout) {
+    DsLayerDev L;
+    memset(&L, 0, sizeof(L));
+    L.type = kLayerRes2d; L.cin = cin; L.cout = cout; L.hin = hin; L.win = win; L.hout = hout; L.wout = wout;
+    d->net.layer[d->net.nlayers++] = L;
+    d->act_floats = std::max(d->act_floats, (size_t)hout * wout * cout);
+  };
+  const size_t kSmemLimit = 227 * 1024;                            // sm_90's opt-in shared memory per block
+  const int64_t kGridX = 2147483647;
+  R2Conv0& L0 = d->r2conv0;
+  L0 = {c.height, c.width, pool ? c.height / 4 : c.height, pool ? c.width / 4 : c.width, ch[0], pool ? 4 : 1, 0, convs[0].w, convs[0].bn};
+  L0.RH = std::min(L0.hout, pool ? 2 : 8);                         // 8 conv rows per CTA
+  if (r2_conv0_smem_floats(L0) * 4 > kSmemLimit)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res2d_conv0 needs %zu bytes of shared memory at width %d, the limit is %zu",
+                   r2_conv0_smem_floats(L0) * 4, c.width, kSmemLimit);
+  if ((int64_t)c.max_batch * ((L0.hout + L0.RH - 1) / L0.RH) > kGridX)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res2d_conv0: max_batch %d x %d row tiles exceeds the grid's %lld CTAs", c.max_batch,
+                   (L0.hout + L0.RH - 1) / L0.RH, (long long)kGridX);
+  layer(c.height, c.width, L0.hout, L0.wout, 1, ch[0]);
+  d->flops += 2ll * c.height * c.width * 9 * ch[0];
+  int h = L0.hout, w = L0.wout, cin = ch[0];
+  size_t ci = 1;
+  for (int i = 0; i < 3; ++i) {
+    R2Block& B = d->r2block[i];
+    memset(&B, 0, sizeof(B));
+    B.cin = cin; B.cout = ch[i + 1]; B.down = B.cout != cin; B.s = B.down ? 2 : 1; B.hin = h; B.win = w;
+    ds_same(h, 3, B.s, &B.hout, &B.pt);
+    ds_same(w, 3, B.s, &B.wout, &B.pl);
+    if (B.down) { B.wd = convs[ci].w; B.bnd = convs[ci].bn; ++ci; }
+    B.w0 = convs[ci].w; B.bn0 = convs[ci].bn; ++ci;
+    B.w1 = convs[ci].w; B.bn1 = convs[ci].bn; ++ci;
+    // tile plan: up to 8 x 16 output positions and every output channel at once; filter slices of down to 32 channels keep it
+    // near 100 KB of shared memory (two CTAs per SM), and past 200 KB the tile shrinks.  Then balanced, so that the last tile
+    // of a row or column is not a sliver.  The plan depends on the geometry alone, so an utterance's bits do not depend on n.
+    B.RH = std::min(B.hout, 8); B.WT = std::min(B.wout, 16); B.COT = r2_pad4(B.cout);
+    auto bytes = [&] { return r2_block_smem(B).floats * 4; };
+    while (bytes() > 100 * 1024 && B.COT > 32) B.COT = r2_pad4(B.COT / 2);
+    while (bytes() > 200 * 1024 && (B.RH > 1 || B.WT > 1)) {
+      if (B.WT > B.RH) B.WT = std::max(1, B.WT / 2);
+      else B.RH = std::max(1, B.RH / 2);
+    }
+    B.RH = (B.hout + (B.hout + B.RH - 1) / B.RH - 1) / ((B.hout + B.RH - 1) / B.RH);
+    B.WT = (B.wout + (B.wout + B.WT - 1) / B.WT - 1) / ((B.wout + B.WT - 1) / B.WT);
+    if (bytes() > kSmemLimit)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "res2d_block %d needs %zu bytes of shared memory, the limit is %zu", i, bytes(), kSmemLimit);
+    const int64_t tiles = (int64_t)((B.hout + B.RH - 1) / B.RH) * ((B.wout + B.WT - 1) / B.WT);
+    if ((int64_t)c.max_batch * tiles > kGridX)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "res2d_block %d: max_batch %d x %lld tiles exceeds the grid's %lld CTAs", i, c.max_batch,
+                     (long long)tiles, (long long)kGridX);
+    layer(h, w, B.hout, B.wout, cin, B.cout);
+    d->flops += 2ll * B.hout * B.wout * (9ll * cin * B.cout + 9ll * B.cout * B.cout + (B.down ? (int64_t)cin * B.cout : 0));
+    h = B.hout; w = B.wout; cin = B.cout;
+  }
+  d->flops += 2ll * ch[3] * c.num_classes;
+  return TCR_OK;
+}
+
 extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   if (!cfg || !out) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   *out = nullptr;
   const bool kws = cfg->size == TCR_KWS_TRAD_FPOOL3 || cfg->size == TCR_KWS_ONE_FSTRIDE4;
-  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws) {
-    set_error("DS-CNN size must be 'S', 'M' or 'L', or a KWS baseline: 'P' (trad_fpool3) or 'F' (one_fstride4)");
+  const bool res2d = cfg->size == TCR_RES2D8 || cfg->size == TCR_RES2D8_POOL;
+  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws && !res2d) {
+    set_error("DS-CNN size must be 'S', 'M' or 'L', or a KWS baseline: 'P' (trad_fpool3) or 'F' (one_fstride4), or a 2-D ablation: "
+              "'R' (ResNet2D8) or 'A' (ResNet2D8Pool)");
     return TCR_ERR_INVALID;
   }
+  if (!res2d && cfg->width_multiplier != 0.0)
+    return ds_fail(TCR_ERR_INVALID, "width_multiplier (%g) applies to ResNet2D8 / ResNet2D8Pool only; it must be 0 for size '%c'",
+                   cfg->width_multiplier, (char)cfg->size);
+  if (res2d && !(cfg->width_multiplier >= 0.0 && cfg->width_multiplier < 1e6))
+    return ds_fail(TCR_ERR_INVALID, "bad width_multiplier %g", cfg->width_multiplier);
   if (cfg->max_batch <= 0 || cfg->height <= 0 || cfg->width <= 0 || cfg->num_classes <= 0 || cfg->num_classes > kMaxClasses) {
     set_error("bad DS-CNN configuration");
     return TCR_ERR_INVALID;
@@ -1492,12 +1840,17 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     return ds_fail(TCR_ERR_UNSUPPORTED, "one_fstride4 needs height x width <= %d (its conv stages a whole utterance in shared "
                    "memory), got %d x %d", kKwsMaxStaged, cfg->height, cfg->width);
   }
+  if (cfg->size == TCR_RES2D8_POOL && (cfg->height < 4 || cfg->width < 4)) {
+    return ds_fail(TCR_ERR_UNSUPPORTED, "ResNet2D8Pool needs height >= 4 and width >= 4 (res2d_conv0's 4x4 / stride 4 average pool is "
+                   "VALID), got %d x %d", cfg->height, cfg->width);
+  }
   if (cfg->size == TCR_KWS_ONE_FSTRIDE4 && cfg->width < 8) {
     return ds_fail(TCR_ERR_UNSUPPORTED, "one_fstride4 needs width >= 8 (its T x 8 conv is VALID), got %d", cfg->width);
   }
   tcr_dscnn* d = new tcr_dscnn();
   d->cfg = *cfg;
   d->kws = kws;
+  d->res2d = res2d;
   if (const char* e = getenv("TCR_DSCNN_TC")) { d->use_tc = e[0] != '0'; d->tc_ws = e[0] != '1'; }
   struct Def { int type, depth, kh, kw, sh, sw; const char* scope; };
   std::vector<Def> defs;
@@ -1564,6 +1917,12 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     d->flops += 2ll * H.K * 32 + 2ll * 32 * 128 + (trad ? 0 : 2ll * 128 * 128) + 2ll * 128 * cfg->num_classes;
     defs.clear();
   }
+  if (res2d) {
+    const int rc = res2d_define(d, add);
+    if (rc != TCR_OK) { delete d; return rc; }
+    h = d->net.layer[3].hout; w = d->net.layer[3].wout; cin = d->net.layer[3].cout;
+    defs.clear();
+  }
   for (const Def& df : defs) {
     DsLayerDev L;
     memset(&L, 0, sizeof(L));
@@ -1597,7 +1956,7 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     h = L.hout; w = L.wout; cin = df.depth;
   }
   d->net.classes = cfg->num_classes;
-  if (!kws) {
+  if (!kws && !res2d) {
     d->net.fcw = add("DSCNN/fc1/weights", TCR_KIND_WEIGHT, {cin, cfg->num_classes});
     d->net.fcb = add("DSCNN/fc1/biases", TCR_KIND_BETA, {cfg->num_classes});
     d->flops += 2ll * cin * cfg->num_classes;
@@ -1759,6 +2118,35 @@ static int kws_head(tcr_dscnn* d, const float* params, const float* in, int n, f
   return TCR_OK;
 }
 
+// A layer of the 2-D ablations: 0 is conv0 (+ pool) on res2d_conv0_kernel, 1-3 the residual blocks on res2d_block_kernel.
+template <bool WIN>
+static int res2d_launch(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s, WindowView win) {
+  const float eps = 1e-3f;
+  if (l == 0) {
+    const R2Conv0& L = d->r2conv0;
+    const size_t smem = r2_conv0_smem_floats(L) * 4;
+    auto kfn = res2d_conv0_kernel<WIN>;
+#ifndef TCR_EMU
+    static SmemOptIn optin;
+    if (optin.ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res2d_conv0: shared memory opt-in failed");
+#endif
+    const unsigned grid = (unsigned)((int64_t)n * ((L.hout + L.RH - 1) / L.RH));
+    TCR_LAUNCH(WIN ? "res2d_conv0:win" : "res2d_conv0", kfn, dim3(grid), dim3(256), smem, s, L, params, in, out, eps, win);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res2d_conv0 launch failed");
+    return TCR_OK;
+  }
+  const R2Block& B = d->r2block[l - 1];
+  const size_t smem = r2_block_smem(B).floats * 4;
+#ifndef TCR_EMU
+  static SmemOptIn optin;
+  if (optin.ensure(res2d_block_kernel, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res2d_block: shared memory opt-in failed");
+#endif
+  const unsigned grid = (unsigned)((int64_t)n * ((B.hout + B.RH - 1) / B.RH) * ((B.wout + B.WT - 1) / B.WT));
+  TCR_LAUNCH("res2d_block", res2d_block_kernel, dim3(grid), dim3(256), smem, s, B, params, in, out, eps);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res2d_block launch failed");
+  return TCR_OK;
+}
+
 // Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC), or for l == 0 with `win` the windows it describes.
 // The kernel is chosen here, once for every entry point: wgmma where the layer's shape fits the tensor-core kernels
 // (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.  The warp-specialised block kernel reads its input through a TMA map
@@ -1770,6 +2158,10 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
   if (L.type == kLayerKws) {
     if (win) return kws_launch_conv<true>(d, l, params, in, out, n, s, *win);
     return kws_launch_conv<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
+  }
+  if (L.type == kLayerRes2d) {
+    if (win) return res2d_launch<true>(d, l, params, in, out, n, s, *win);
+    return res2d_launch<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
   }
   if (L.type == 0) {
     if (win) return ds_launch_conv<true>(d, L, params, in, out, n, s, *win);
@@ -1841,6 +2233,12 @@ int tcr::dscnn_forward(tcr_dscnn* d, const float* feat, const float* params, int
   }
   if (d->kws) return kws_head(d, params, in, n, logits, probs, s);
   const DsLayerDev& last = d->net.layer[d->net.nlayers - 1];
+  if (d->res2d) {
+    TCR_LAUNCH("res2d_head", res2d_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes, d->r2fc,
+               params, in, logits, probs);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res2d_head launch failed");
+    return TCR_OK;
+  }
   if (last.cout > 320) { set_error("DS-CNN head supports up to 320 channels"); return TCR_ERR_UNSUPPORTED; }
   TCR_LAUNCH("dscnn_head", dscnn_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes, d->net.fcw,
              d->net.fcb, params, in, logits, probs);

@@ -1,6 +1,7 @@
 """DS-CNN forward (inference) on the CUDA path: the reference's 2-D-conv comparison model
 (audio_nets/ds_cnn.py; DSCNN{S,M,L}Model.build_inference in factory/audio_nets.py:298-358), and on the same handle the KWS
-baselines cnn-trad-fpool3 (size 'P') and cnn-one-fstride4 ('F') of audio_nets/kws.py.  Training DS-CNN is out of scope
+baselines cnn-trad-fpool3 (size 'P') and cnn-one-fstride4 ('F') of audio_nets/kws.py, and the paper's 2-D ablations of TC-ResNet8,
+ResNet2D8 ('R') and ResNet2D8Pool ('A') of audio_nets/tc_resnet.py.  Training DS-CNN is out of scope
 (SURVEY.md 2 #13): weights come from a checkpoint keyed by the TF variable names in `self.table`.
 
 With a front-end (set_frontend) the handle also takes audio: `mfcc`, `forward_input`, `eval_accumulate` and `listener` mirror
@@ -18,18 +19,20 @@ from .engine import Listener, frontend_config, frontend_shape
 
 # tcr_dscnn_config.size of the KWS baselines (include/tcr_b200.h): KWSModel --architecture -> size code
 KWS_SIZES = {"trad_fpool3": "P", "one_fstride4": "F"}
+# and of the 2-D ablations, by TF scope; they alone take a width multiplier
+RES2D_SIZES = {"ResNet2D8": "R", "ResNet2D8Pool": "A"}
 
 
 class DsCnn:
     _LISTENER_CREATE = "tcr_dscnn_listener_create"
 
     def __init__(self, size: str = "S", height: int = 49, width: int = 40, num_classes: int = 12, max_batch: int = 512,
-                 device: int | None = None):
+                 device: int | None = None, width_multiplier: float = 0.0):
         if not torch.cuda.is_available():
             raise L.TcrError("tcresnet_b200.DsCnn needs a CUDA device (there is no CPU fallback)")
         self.lib = L.load()
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
-        cfg = L.TcrDscnnConfig(ord(size), height, width, num_classes, max_batch, self.device.index)
+        cfg = L.TcrDscnnConfig(ord(size), height, width, num_classes, max_batch, self.device.index, width_multiplier)
         self._h = C.c_void_p()
         with torch.cuda.device(self.device):
             L.check(self.lib, self.lib.tcr_dscnn_create(C.byref(cfg), C.byref(self._h)), "tcr_dscnn_create")
@@ -85,7 +88,7 @@ class DsCnn:
 
     def new_variables(self, seed: int = 0) -> torch.Tensor:
         """Flat variables as the reference initialises them before a restore: Xavier-uniform weights (slim's default), zero biases /
-        beta / moving mean, unit moving variance; the KWS baselines ('P', 'F') draw every weight from
+        beta / moving mean, unit moving variance, unit gamma (the 2-D ablations' BatchNorm); the KWS baselines ('P', 'F') draw every weight from
         truncated_normal(stddev=0.01) (audio_nets/kws.py), values past two sigma redrawn.  Host-side RNG, not TF's."""
         rng = np.random.default_rng(seed)
         flat = np.zeros(self.num_params, np.float32)
@@ -101,7 +104,7 @@ class DsCnn:
                 fan_in, fan_out = int(np.prod(shp[:-1])), int(np.prod(shp[:-2])) * shp[-1]
                 lim = np.sqrt(6.0 / (fan_in + fan_out))
                 flat[sl] = rng.uniform(-lim, lim, d["numel"]).astype(np.float32)
-            elif d["kind"] == "moving_variance":
+            elif d["kind"] in ("moving_variance", "gamma"):
                 flat[sl] = 1.0
         return torch.from_numpy(flat).to(self.device)
 

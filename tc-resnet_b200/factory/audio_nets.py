@@ -4,8 +4,8 @@ executing on the CUDA engine instead of building a TF graph.
 `train_audio.py` / `evaluate_audio.py` look the class up by NAME (`eval(f"audio_nets.{args.model}")`,
 train_audio.py:32), call `Model(args, dataset)`, then `model.build(wavs, labels, is_training)` and hand the model
 to the trainer / evaluator, which touch only the attributes set here and `session.run`.  TCResNet8Model and
-TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model and KWSModel (--architecture trad_fpool3 / one_fstride4) are on it
-for evaluation, deployment and streaming (their training is out of scope and raises NotImplementedError); the other entries of `_available_nets` (baselines the north star
+TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model, KWSModel (--architecture trad_fpool3 / one_fstride4),
+ResNet2D8Model and ResNet2D8PoolModel are on it for evaluation, deployment and streaming (their training is out of scope and raises NotImplementedError); the other entries of `_available_nets` (baselines the north star
 does not name) are registered so the CLI accepts them but raise NotImplementedError when built.
 """
 from __future__ import annotations
@@ -18,7 +18,7 @@ import torch
 from ..common import utils
 from ..common.model_loader import EMA_SUFFIX
 from ..datasets import preprocessor_factory
-from ..dscnn import KWS_SIZES, DsCnn
+from ..dscnn import KWS_SIZES, RES2D_SIZES, DsCnn
 from ..engine import OPTIMIZER_DEFAULTS, OPTIMIZER_SLOT_NAMES, Engine
 from ..runtime import InvalidArgumentError, Node
 from .base import TFModel
@@ -554,13 +554,10 @@ def _baseline(name, flags):
                 "Baseline of the reference registered for CLI compatibility; not on the accelerated path."})
 
 
-_TC = [("--weight_decay", 0.0001), ("--dropout_keep_prob", 0.5), ("--width_multiplier", 1.0)]
 Res8Model = _baseline("Res8Model", [("--weight_decay", 0.00001)])
 Res8NarrowModel = _baseline("Res8NarrowModel", [("--weight_decay", 0.00001)])
 Res15Model = _baseline("Res15Model", [("--weight_decay", 0.00001)])
 Res15NarrowModel = _baseline("Res15NarrowModel", [("--weight_decay", 0.00001)])
-ResNet2D8Model = _baseline("ResNet2D8Model", _TC)
-ResNet2D8PoolModel = _baseline("ResNet2D8PoolModel", _TC)
 
 
 class DsCnnModel(AudioNetModel):
@@ -599,7 +596,7 @@ class DsCnnModel(AudioNetModel):
             raise ValueError(f"bad window / stride / clip ({window} / {stride} / {clip} samples)")
         height = 1 + (clip - window) // stride
         width = a.num_mfccs if a.preprocess_method == "mfcc" else a.num_mel_bins
-        eng = DsCnn(self.dscnn_size, height, width, a.num_classes, max_batch)
+        eng = DsCnn(self.dscnn_size, height, width, a.num_classes, max_batch, width_multiplier=self._width_multiplier())
         return eng.set_frontend(a.sample_rate, a.clip_duration_ms, a.window_size_ms, a.window_stride_ms, a.num_mel_bins, a.num_mfccs,
                                 a.lower_edge_hertz, a.upper_edge_hertz, a.preprocess_method)
 
@@ -619,6 +616,10 @@ class DsCnnModel(AudioNetModel):
 
     def _regularization(self) -> float:
         """The regularisation term of total_loss: none in the DS-CNN graph."""
+        return 0.0
+
+    def _width_multiplier(self) -> float:
+        """tcr_dscnn_config.width_multiplier: 0 (none) but for the 2-D ablations."""
         return 0.0
 
     def execute(self, names: Set[str], feed) -> Dict[str, object]:
@@ -703,3 +704,46 @@ class KWSModel(DsCnnModel):
     def _regularization(self) -> float:
         wd = float(self.args.weight_decay)
         return wd * 0.5 * float((self.params.double() ** 2).sum()) if wd else 0.0
+
+
+class _Res2dModel(DsCnnModel):
+    """ResNet2D8Model / ResNet2D8PoolModel (factory/audio_nets.py:412-460, audio_nets/tc_resnet.py:73-101): the paper's 2-D ablations
+    of TC-ResNet8, in evaluation mode on the DS-CNN handle (size codes 'R' / 'A', dscnn.RES2D_SIZES) with --width_multiplier.
+    Variables are restored by their TF names ("ResNet2D8/conv0/weights", ...).  total_loss adds build_loss's L2 term,
+    weight_decay * sum(tf.nn.l2_loss(v)) over every variable outside BatchNorm (the weights, fc2 included).  Training is out of
+    scope."""
+    scope: str = ""
+
+    add_arguments = staticmethod(_tc_flags)
+
+    @property
+    def dscnn_size(self) -> str:
+        return RES2D_SIZES[self.scope]
+
+    def _width_multiplier(self) -> float:
+        return float(self.args.width_multiplier)
+
+    def build_inference(self, inputs, is_training=True):
+        if is_training:
+            raise NotImplementedError(f"{type(self).__name__}: training the 2-D ablations is out of scope on the CUDA path; evaluation "
+                                      "(evaluate_audio.py), the deployable model and the listener (listen_audio.py) are supported")
+        if getattr(self.args, "device_dataset", False):
+            raise NotImplementedError(f"{type(self).__name__}: --device_dataset serves the TC-ResNet models only; evaluate from the "
+                                      "dataset on disk")
+        return super().build_inference(inputs, is_training=False)
+
+    def _regularization(self) -> float:
+        wd = float(self.args.weight_decay)
+        if not wd:
+            return 0.0
+        p = self.params.double()
+        return wd * 0.5 * sum(float((p[d["offset"]:d["offset"] + d["numel"]] ** 2).sum()) for d in self.engine.table
+                              if d["kind"] == "weight")
+
+
+class ResNet2D8Model(_Res2dModel):
+    scope = "ResNet2D8"
+
+
+class ResNet2D8PoolModel(_Res2dModel):
+    scope = "ResNet2D8Pool"
