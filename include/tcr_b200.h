@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 13
+#define TCR_ABI_VERSION 14
 
 enum {
   TCR_OK = 0,
@@ -435,14 +435,35 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
  * Variables as tcr_param_table's TCResNet8 rows under the scope "ResNet2D8" / "ResNet2D8Pool", with 2-D shapes ("ResNet2D8/
  * conv0/weights" [3, 3, 1, c0], ".../block0/down/weights" [1, 1, c0, c1], ".../conv0/BatchNorm/gamma", ..., ".../fc/weights"
  * [1, 1, c3, classes], ".../fc2/weights" [1, 1, c3, 2], then the moving statistics); fc2 is loaded but not computed.
- * forward_partial's layers are [conv0 (+ pool), block0, block1, block2], each NHWC. */
+ * forward_partial's layers are [conv0 (+ pool), block0, block1, block2], each NHWC.
+ *
+ * And Honk's ResNets as the reference builds them (audio_nets/res.py Res8 / Res8Narrow / Res15 / Res15Narrow), evaluation mode
+ * (ABI 14).  C channels throughout: 45, or 19 for the Narrow variants.  Every conv is 3x3, stride 1, TF SAME, bias-free and followed
+ * by ReLU; BatchNorm has no beta and no gamma (y = (x - mean) / sqrt(var + 1e-3), the moving statistics).
+ *   f_conv 1 -> C + ReLU (no BatchNorm); Res8 / Res8Narrow only: a 4x3 average pool at stride 1, VALID, so the blocks run on
+ *     (height - 3) x (width - 2); needs height >= 4 and width >= 3.
+ *   block i = 0 .. L / 2 - 1 on input x: a = BN_{conv2i_bn}(ReLU(conv{2i}(x))), y = BN_{conv2i+1_bn}(ReLU(conv{2i+1}(a)) + x) (no
+ *     ReLU after the add).  Res15 has L = 13 convs, so after its six blocks conv12: BN_{conv12_bn}(ReLU(conv12(y))).  Res8 has L = 6.
+ *   Res15 / Res15Narrow dilate: conv{k} has rate 2^(k / 3) (1, 1, 1, 2, 2, 2, 4, 4, 4, 8, 8, 8, 16), SAME pads `rate` zeros on
+ *     every side.  Res8 does not dilate.
+ *   Then the global average pool, fc (1x1, no bias) and softmax.
+ * Variables, all under the scope "Res" (slim's conv2d opens the sub-scope "Conv" inside conv{k}): "Res/f_conv/weights" [3, 3, 1, C],
+ * "Res/conv{k}/Conv/weights" [3, 3, C, C] for k = 0 .. L - 1, "Res/fc/weights" [1, 1, C, classes] (kind TCR_KIND_WEIGHT), then per
+ * k "Res/conv{k}_bn/moving_mean" and ".../moving_variance" [C].  width_multiplier must be 0.  forward_partial's layers are
+ * [f_conv (+ pool), conv0, .., conv{L-1}], each NHWC [n, h, w, C] after its epilogue (after BN for conv{2i} and conv12, after the
+ * add and BN for conv{2i+1}): 7 layers for Res8, 14 for Res15. */
 #define TCR_KWS_TRAD_FPOOL3 'P'
 #define TCR_KWS_ONE_FSTRIDE4 'F'
 #define TCR_RES2D8 'R'
 #define TCR_RES2D8_POOL 'A'
+#define TCR_RES8 'E'
+#define TCR_RES8_NARROW 'N'
+#define TCR_RES15 'D'
+#define TCR_RES15_NARROW 'T'
 typedef struct tcr_dscnn tcr_dscnn;
 typedef struct tcr_dscnn_config {
-  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 | TCR_RES2D8 | TCR_RES2D8_POOL */
+  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 | TCR_RES2D8 | TCR_RES2D8_POOL | TCR_RES8 |
+                            TCR_RES8_NARROW | TCR_RES15 | TCR_RES15_NARROW */
   int32_t height;        /* frames, 49 */
   int32_t width;         /* coefficients, 40 (10 in the reference's DS-CNN recipes) */
   int32_t num_classes;   /* 12 */

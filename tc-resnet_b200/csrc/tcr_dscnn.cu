@@ -11,7 +11,9 @@
 // and the KWS baselines of audio_nets/kws.py on the same handle (sizes 'P' trad_fpool3, 'F' one_fstride4): kws_conv_kernel (FMA
 // first layers), kws_bsplit_kernel + kws_conv2_tc_kernel (trad_fpool3's 64 -> 64 conv on wgmma), kws_lin_kernel + kws_head_kernel
 // (the dense head); and the 2-D ablations of TC-ResNet8 ('R' ResNet2D8, 'A' ResNet2D8Pool): res2d_conv0_kernel (conv0, the pool
-// fused), res2d_block_kernel (one fused residual block), res2d_head_kernel (dscnn_head without the bias).
+// fused), res2d_block_kernel (one fused residual block), res2d_head_kernel (dscnn_head without the bias); and Honk's ResNets of
+// audio_nets/res.py ('E' Res8, 'N' Res8Narrow, 'D' Res15, 'T' Res15Narrow): res_fconv_kernel (f_conv, Res8's pool fused),
+// res_conv_kernel (one dilated 3x3 conv, its residual add and BatchNorm in the epilogue), and res2d_head_kernel.
 // BatchNorm here has no gamma (slim default scale=False) and uses the moving statistics; bias + BN fold into one
 // per-channel (scale, shift) pair computed while staging.
 #ifndef TCR_EMU
@@ -32,15 +34,17 @@ namespace tcr {
 
 struct DsLayerDev {
   int type;                 // 0 conv, 1 separable, 2 (kLayerKws) VALID bias-free conv + ReLU of the KWS baselines, 3 (kLayerRes2d)
-                            // a layer of the 2-D ablations (its R2Conv0 / R2Block is in the handle)
+                            // a layer of the 2-D ablations (its R2Conv0 / R2Block is in the handle), 4 (kLayerRes) a layer of
+                            // Res8 / Res15 (its ResFconv / ResConv is in the handle)
   int cin, cout, kh, kw, sh, sw, hin, win, hout, wout, pt, pl;
   int64_t w, b, beta, mm, mv;                // conv / depthwise
   int64_t pw, pb, pbeta, pmm, pmv;           // pointwise (separable only)
 };
 
-constexpr int kDsMaxLayers = 8;
+constexpr int kDsMaxLayers = 16;      // Res15: f_conv and 13 convs (DsNet is host-only)
 constexpr int kLayerKws = 2;
 constexpr int kLayerRes2d = 3;
+constexpr int kLayerRes = 4;
 struct DsNet {
   int nlayers, n, classes;
   DsLayerDev layer[kDsMaxLayers];
@@ -1639,6 +1643,275 @@ __global__ void __launch_bounds__(256) res2d_head_kernel(int npos, int C, int cl
   dscnn_head<false>(npos, C, classes, fcw, 0, params, in, logits, probs);
 }
 
+// ---- Res8 / Res8Narrow / Res15 / Res15Narrow: Honk's ResNets as the reference builds them (audio_nets/res.py) ----
+// Evaluation mode.  Every conv is bias-free, TF SAME at stride 1 and followed by ReLU; BatchNorm has neither beta nor gamma
+// (center = scale = False), so the moving statistics fold into scale = 1 / sqrt(var + eps) and shift = -mean * scale.  The head is
+// res2d_head_kernel.
+struct ResBn { int64_t mm, mv; };
+__device__ __forceinline__ void res_fold(const float* p, const ResBn& bn, int c, int C, float eps, float* sc, float* sf) {
+  float s = 0.f, t = 0.f;
+  if (c < C) {
+    s = 1.f / sqrtf(p[bn.mv + c] + eps);
+    t = -p[bn.mm + c] * s;
+  }
+  sc[c] = s;
+  sf[c] = t;
+}
+
+// 4-byte global -> shared copy; invalid: the destination is zero-filled and nothing is read (cp.async with source size 0).
+__device__ __forceinline__ void res_cp4(float* dst, const float* src, bool valid) {
+#ifdef TCR_EMU
+  *dst = valid ? *src : 0.f;
+#else
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(valid ? 4u : 0u) : "memory");
+#endif
+}
+__device__ __forceinline__ void res_cp_commit() {
+#ifndef TCR_EMU
+  asm volatile("cp.async.commit_group;" ::: "memory");
+#endif
+}
+__device__ __forceinline__ void res_cp_wait_prev() {             // all but the most recent group have landed
+#ifndef TCR_EMU
+  asm volatile("cp.async.wait_group 1;" ::: "memory");
+#endif
+}
+
+// f_conv: 3 x 3 SAME conv of the single-channel features + ReLU; for Res8 (ph x pw = 4 x 3) the stride-1 VALID average pool in the
+// same launch, so that only the pooled map reaches HBM.  One CTA per (utterance, tile of RH output rows), blockIdx.x = n * tiles +
+// tile.  The tile's input rows with SAME's one-pixel zero border and the taps are staged; with the pool, the RH + ph - 1 rows of
+// conv outputs the tile's windows read are staged too.  A thread owns one channel and walks positions 256 / cout apart.  WIN:
+// utterance n is a listener window (ds_window); the border is zeros there too, never the neighbouring history frames.
+struct ResFconv { int hin, win, hout, wout, cout, ph, pw, RH; int64_t w; };
+TCR_HD inline size_t res_fconv_smem_floats(const ResFconv& L) {
+  const int cr = L.RH + L.ph - 1;                                 // conv rows of a full tile
+  return (size_t)(cr + 2) * (L.win + 2) + (L.ph > 1 ? (size_t)cr * L.win * L.cout : 0) + 9 * (size_t)L.cout;
+}
+template <bool WIN>
+__global__ void __launch_bounds__(256) res_fconv_kernel(ResFconv L, const float* __restrict__ params, const float* __restrict__ in,
+                                                        float* __restrict__ out, WindowView win) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* xs = reinterpret_cast<float*>(smem_raw);
+  const int tpu = (L.hout + L.RH - 1) / L.RH, tid = threadIdx.x, nt = blockDim.x;
+  const int n = blockIdx.x / tpu, h0 = (blockIdx.x - n * tpu) * L.RH, rh = imin(L.RH, L.hout - h0);
+  const int cr = rh + L.ph - 1, xc = L.win + 2;                   // conv rows of this tile, padded width
+  float* cs = xs + (size_t)(L.RH + L.ph + 1) * xc;
+  float* ws = cs + (L.ph > 1 ? (size_t)(L.RH + L.ph - 1) * L.win * L.cout : 0);
+  const float* src;
+  if constexpr (WIN) src = ds_window(in, n, win);
+  else src = in + (int64_t)n * L.hin * L.win;
+  {  // input rows h0 - 1 .. h0 + cr, columns -1 .. win
+    int r = tid / xc, c = tid - r * xc;
+    const int dr = nt / xc, dc = nt - dr * xc;
+    for (int i = tid; i < (cr + 2) * xc; i += nt) {
+      const int h = h0 - 1 + r, w = c - 1;
+      xs[i] = (h >= 0 && h < L.hin && w >= 0 && w < L.win) ? src[(int64_t)h * L.win + w] : 0.f;
+      r += dr;
+      c += dc;
+      if (c >= xc) { c -= xc; ++r; }
+    }
+  }
+  for (int i = tid; i < 9 * L.cout; i += nt) ws[i] = params[L.w + i];
+  __syncthreads();
+  const int c = tid % L.cout, lanes = nt / L.cout;                // cout <= 45 < blockDim.x
+  const bool active = tid < lanes * L.cout;
+  float wk[9];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) wk[k] = active ? ws[k * L.cout + c] : 0.f;
+  const int dr = lanes / L.win, dc = lanes - dr * L.win;
+  if (active) {
+    int r = (tid / L.cout) / L.win, ow = (tid / L.cout) - r * L.win;
+    for (int q = tid / L.cout; q < cr * L.win; q += lanes) {
+      const float* xb = xs + r * xc + ow;
+      float acc = 0.f;
+#pragma unroll
+      for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) acc = fmaf(xb[i * xc + j], wk[3 * i + j], acc);
+      const float v = fmaxf(acc, 0.f);
+      if (L.ph == 1) out[(((int64_t)n * L.hout + h0 + r) * L.wout + ow) * L.cout + c] = v;
+      else cs[((size_t)r * L.win + ow) * L.cout + c] = v;
+      r += dr;
+      ow += dc;
+      if (ow >= L.win) { ow -= L.win; ++r; }
+    }
+  }
+  if (L.ph == 1) return;                                          // uniform across the CTA
+  __syncthreads();
+  if (!active) return;
+  const float inv = 1.f / (float)(L.ph * L.pw);
+  const int pr = lanes / L.wout, pc = lanes - pr * L.wout;
+  int r = (tid / L.cout) / L.wout, ow = (tid / L.cout) - r * L.wout;
+  for (int q = tid / L.cout; q < rh * L.wout; q += lanes) {
+    float sum = 0.f;
+    for (int py = 0; py < L.ph; ++py)
+      for (int px = 0; px < L.pw; ++px) sum += cs[((size_t)(r + py) * L.win + ow + px) * L.cout + c];
+    out[(((int64_t)n * L.hout + h0 + r) * L.wout + ow) * L.cout + c] = sum * inv;
+    r += pr;
+    ow += pc;
+    if (ow >= L.wout) { ow -= L.wout; ++r; }
+  }
+}
+
+// conv{k}: 3 x 3 at dilation d, stride 1, SAME (d zeros on every side), C -> C, then ReLU.  RES = false: then BatchNorm.  RES = true
+// (conv{2i+1}, the second conv of block i): + the block's input `res`, then BatchNorm; there is no ReLU after the add.
+//
+// Persistent CTAs walk tiles of TR whole rows of one utterance (tile t: utterance t / tpu); channels are padded with zeros to CP
+// (45 -> 48, 19 -> 20).  Per CTA, once: the filter bank [9][CP][CP] and the folded BatchNorm.  Per tile, three stages, one per tap
+// row i: the TR input rows h0 + (i - 1) d .. that the tap row reads, [TR * W][XS] (positions XS floats apart, which keeps a warp's
+// eight positions on distinct banks), gathered by 4-byte cp.async (a row of C floats is not 16-byte aligned) with zero fill for
+// rows outside the map.  Stages are double-buffered: stage s + 1 is in flight while stage s runs.  A tap's column shift reads
+// the same slab d positions over; a position whose shifted column leaves the map reads a zero row instead.
+// A thread owns TM positions (SLOTS apart) x TN channels of the tile in registers: CP = 48 as 8 position lanes x 4 channel lanes of
+// 12 per warp, CP = 20 as 32 position lanes of all 20 channels.  The epilogue writes ReLU(acc) back into the stage's slab, then
+// the tile's rows, contiguous in HBM, are written coalesced with the residual and BatchNorm applied.
+// Residual aliasing: in a full forward `out` is the buffer holding the block input `res`; each thread reads its residual element
+// before it writes the same element, so neither pointer is __restrict__.
+constexpr int kResConvThreads = 256;
+template <int CP> struct ResTile;
+template <> struct ResTile<48> { static constexpr int CGW = 4, TM = 4; };
+template <> struct ResTile<20> { static constexpr int CGW = 1, TM = 2; };
+template <int CP> TCR_HD constexpr int res_xs() { return ((CP >> 2) & 1) ? CP : CP + 4; }
+template <int CP> TCR_HD constexpr int res_np_max() { return kResConvThreads / 32 * (32 / ResTile<CP>::CGW) * ResTile<CP>::TM; }
+template <int CP> TCR_HD inline size_t res_conv_smem_floats(int TR, int W) { return 9 * CP * CP + 3 * CP + 2 * (size_t)TR * W * res_xs<CP>(); }
+struct ResConv { int h, w, c, d, TR; int64_t wt; ResBn bn; };
+
+template <int CP, bool RES>
+__global__ void __launch_bounds__(kResConvThreads) res_conv_kernel(ResConv L, int n_utt, const float* __restrict__ params,
+                                                               const float* __restrict__ in, const float* res, float* out, float eps) {
+  constexpr int CGW = ResTile<CP>::CGW, TM = ResTile<CP>::TM, TN = CP / CGW, PG = 32 / CGW, SLOTS = kResConvThreads / 32 * PG;
+  constexpr int XS = res_xs<CP>();
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* ws = reinterpret_cast<float*>(smem_raw);
+  float *sc = ws + 9 * CP * CP, *sf = sc + CP, *zero = sf + CP, *xb = zero + CP;
+  const int tid = threadIdx.x, C = L.c, W = L.w, d = L.d, NP = L.TR * W, slab = NP * C;
+  const size_t buf = (size_t)NP * XS;
+  const int tpu = (L.h + L.TR - 1) / L.TR, ntiles = n_utt * tpu;
+  for (int i = tid; i < 9 * CP * CP; i += kResConvThreads) {
+    const int co = i % CP, ci = (i / CP) % CP, k = i / (CP * CP);
+    ws[i] = (ci < C && co < C) ? params[L.wt + ((int64_t)k * C + ci) * C + co] : 0.f;
+  }
+  for (int c = tid; c < CP; c += kResConvThreads) {
+    res_fold(params, L.bn, c, C, eps, sc, sf);
+    zero[c] = 0.f;
+  }
+  for (int i = tid; i < 2 * NP * (CP - C); i += kResConvThreads) {   // the padded channels of both slabs stay zero
+    const int p = i / (CP - C);
+    xb[(size_t)p * XS + C + (i - p * (CP - C))] = 0.f;
+  }
+  // this thread's element walk of a slab (element e of the tile's rows in HBM order -> position p, channel c), stepped without division
+  const int p0 = tid / C, c0 = tid - p0 * C, dp = kResConvThreads / C, dc = kResConvThreads - dp * C;
+  auto issue = [&](int s) {
+    const int t = blockIdx.x + (s / 3) * gridDim.x, i = s - (s / 3) * 3;
+    if (t >= ntiles) return;
+    const int u = t / tpu, hs = (t - u * tpu) * L.TR + (i - 1) * d;
+    const int elo = imax(0, -hs) * W * C, ehi = imax(0, imin(L.TR, L.h - hs)) * W * C;
+    const int64_t g0 = ((int64_t)u * L.h + hs) * W * C;
+    float* x = xb + (s & 1) * buf;
+    int p = p0, c = c0;
+    for (int e = tid; e < slab; e += kResConvThreads) {
+      const bool v = e >= elo && e < ehi;
+      res_cp4(x + (size_t)p * XS + c, v ? in + g0 + e : in, v);
+      p += dp;
+      c += dc;
+      if (c >= C) { c -= C; ++p; }
+    }
+  };
+  // this thread's register tile: positions slot + m * SLOTS of the tile, channels cg * TN ..
+  const int lane = tid & 31, slot = (tid >> 5) * PG + lane / CGW, cg = lane % CGW;
+  int pos[TM], col[TM];
+#pragma unroll
+  for (int m = 0; m < TM; ++m) {
+    pos[m] = slot + m * SLOTS;
+    col[m] = pos[m] % W;
+  }
+  const int nst = blockIdx.x < ntiles ? 3 * ((ntiles - 1 - blockIdx.x) / gridDim.x + 1) : 0;
+  float acc[TM][TN];
+  issue(0);
+  res_cp_commit();
+  for (int s = 0; s < nst; ++s) {
+    const int i = s % 3;
+    if (s + 1 < nst) issue(s + 1);
+    res_cp_commit();
+    res_cp_wait_prev();
+    __syncthreads();                                              // stage s has landed for every thread
+    float* x = xb + (s & 1) * buf;
+    if (i == 0) {
+#pragma unroll
+      for (int m = 0; m < TM; ++m)
+#pragma unroll
+        for (int k = 0; k < TN; ++k) acc[m][k] = 0.f;
+    }
+#pragma unroll 1
+    for (int j = 0; j < 3; ++j) {
+      const int sh = (j - 1) * d;
+      const float* xp[TM];
+#pragma unroll
+      for (int m = 0; m < TM; ++m) {
+        const int cc = col[m] + sh;
+        xp[m] = (pos[m] < NP && cc >= 0 && cc < W) ? x + (size_t)(pos[m] + sh) * XS : zero;
+      }
+      const float* wk = ws + (i * 3 + j) * CP * CP + cg * TN;
+#pragma unroll 1
+      for (int ci = 0; ci < CP; ci += 4) {
+        float4 xv[TM];
+#pragma unroll
+        for (int m = 0; m < TM; ++m) xv[m] = ld4(xp[m] + ci);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          float wv[TN];
+#pragma unroll
+          for (int k = 0; k < TN; k += 4) {
+            const float4 w4 = ld4(wk + (ci + q) * CP + k);
+            wv[k] = w4.x; wv[k + 1] = w4.y; wv[k + 2] = w4.z; wv[k + 3] = w4.w;
+          }
+#pragma unroll
+          for (int m = 0; m < TM; ++m) {
+            const float xq = q == 0 ? xv[m].x : q == 1 ? xv[m].y : q == 2 ? xv[m].z : xv[m].w;
+#pragma unroll
+            for (int k = 0; k < TN; ++k) acc[m][k] = fmaf(xq, wv[k], acc[m][k]);
+          }
+        }
+      }
+    }
+    if (i == 2) {
+      __syncthreads();                                            // every warp is done reading slab s & 1
+#pragma unroll
+      for (int m = 0; m < TM; ++m)
+        if (pos[m] < NP)
+#pragma unroll
+          for (int k = 0; k < TN; ++k)
+            if (cg * TN + k < C) x[(size_t)pos[m] * XS + cg * TN + k] = fmaxf(acc[m][k], 0.f);
+      __syncthreads();
+      const int t = blockIdx.x + (s / 3) * gridDim.x, u = t / tpu, h0 = (t - u * tpu) * L.TR;
+      const int64_t g0 = ((int64_t)u * L.h + h0) * W * C;
+      const int cnt = imin(L.TR, L.h - h0) * W * C;
+      // eight residual loads in flight before the first store: `out` may alias `res`, so the compiler cannot hoist them itself
+      constexpr int kRun = 8;
+      int p = p0, c = c0;
+      for (int e0 = tid; e0 < cnt; e0 += kRun * kResConvThreads) {
+        float r[kRun];
+#pragma unroll
+        for (int q = 0; q < kRun; ++q) {
+          const int e = e0 + q * kResConvThreads;
+          r[q] = (RES && e < cnt) ? res[g0 + e] : 0.f;
+        }
+#pragma unroll
+        for (int q = 0; q < kRun; ++q) {
+          const int e = e0 + q * kResConvThreads;
+          if (e < cnt) out[g0 + e] = fmaf(x[(size_t)p * XS + c] + r[q], sc[c], sf[c]);
+          p += dp;
+          c += dc;
+          if (c >= C) { c -= C; ++p; }
+        }
+      }
+    }
+    __syncthreads();                                              // slab s & 1 is free for stage s + 2
+  }
+}
+
 }  // namespace tcr
 
 // ------------------------------------------------------------------------------------------------
@@ -1673,6 +1946,11 @@ struct tcr_dscnn {
   R2Conv0 r2conv0 = {};
   R2Block r2block[3] = {};
   int64_t r2fc = 0;
+  // Res8 / Res15 ('E', 'N', 'D', 'T'): layer 0 is f_conv (+ pool), layer k + 1 conv{k}; fc's offset
+  bool res = false;
+  ResFconv rfconv = {};
+  ResConv rconv[13] = {};
+  int64_t rfc = 0;
 };
 
 #ifndef TCR_EMU
@@ -1813,14 +2091,78 @@ static int res2d_define(tcr_dscnn* d, Add& add) {
   return TCR_OK;
 }
 
+// Honk's ResNets as audio_nets/res.py builds them: f_conv (+ Res8's 4x3 / stride-1 pool), conv0 .. conv{L-1}, fc, all under the
+// scope "Res" with slim's default "Conv" sub-scope inside conv{k}; the weights in creation order, then each conv{k}_bn's moving
+// statistics.  Also each kernel's tile plan, and the refusals of what the kernels cannot run.
+template <class Add>
+static int res_define(tcr_dscnn* d, Add& add) {
+  const tcr_dscnn_config& c = d->cfg;
+  const bool r8 = c.size == TCR_RES8 || c.size == TCR_RES8_NARROW, narrow = c.size == TCR_RES8_NARROW || c.size == TCR_RES15_NARROW;
+  const int C = narrow ? 19 : 45, nl = r8 ? 6 : 13;
+  const size_t kSmemLimit = 227 * 1024;                            // sm_90's opt-in shared memory per block
+  const int64_t kGridX = 2147483647;
+  ResFconv& F0 = d->rfconv;
+  F0 = {c.height, c.width, r8 ? c.height - 3 : c.height, r8 ? c.width - 2 : c.width, C, r8 ? 4 : 1, r8 ? 3 : 1, 0, 0};
+  F0.w = add("Res/f_conv/weights", TCR_KIND_WEIGHT, {3, 3, 1, C});
+  int64_t wk[13];
+  for (int k = 0; k < nl; ++k) wk[k] = add("Res/conv" + std::to_string(k) + "/Conv/weights", TCR_KIND_WEIGHT, {3, 3, C, C});
+  d->rfc = add("Res/fc/weights", TCR_KIND_WEIGHT, {1, 1, C, c.num_classes});
+  ResBn bn[13];
+  for (int k = 0; k < nl; ++k) {
+    bn[k].mm = add("Res/conv" + std::to_string(k) + "_bn/moving_mean", TCR_KIND_MOVING_MEAN, {C});
+    bn[k].mv = add("Res/conv" + std::to_string(k) + "_bn/moving_variance", TCR_KIND_MOVING_VAR, {C});
+  }
+  auto layer = [&](int hin, int win, int hout, int wout, int cin) {
+    DsLayerDev L;
+    memset(&L, 0, sizeof(L));
+    L.type = kLayerRes; L.cin = cin; L.cout = C; L.hin = hin; L.win = win; L.hout = hout; L.wout = wout;
+    d->net.layer[d->net.nlayers++] = L;
+    d->act_floats = std::max(d->act_floats, (size_t)hout * wout * C);
+  };
+  // f_conv: up to 8 output rows per CTA, fewer where the staged conv rows pass 100 KB (wide log-mel maps)
+  F0.RH = std::min(F0.hout, 8);
+  while (F0.RH > 1 && res_fconv_smem_floats(F0) * 4 > 100 * 1024) --F0.RH;
+  if (res_fconv_smem_floats(F0) * 4 > kSmemLimit)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res_fconv needs %zu bytes of shared memory at width %d, the limit is %zu",
+                   res_fconv_smem_floats(F0) * 4, c.width, kSmemLimit);
+  if ((int64_t)c.max_batch * ((F0.hout + F0.RH - 1) / F0.RH) > kGridX)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res_fconv: max_batch %d x %d row tiles exceeds the grid's %lld CTAs", c.max_batch,
+                   (F0.hout + F0.RH - 1) / F0.RH, (long long)kGridX);
+  layer(c.height, c.width, F0.hout, F0.wout, 1);
+  d->flops += 2ll * c.height * c.width * 9 * C;
+  // conv{k}: tiles of TR whole rows, as many as the CTA's register tiles cover, then balanced so the last tile is not a sliver.  The
+  // plan depends on the geometry alone, so an utterance's bits do not depend on n.
+  const int H = F0.hout, W = F0.wout, npmax = narrow ? res_np_max<20>() : res_np_max<48>();
+  if (W > npmax)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res_conv tiles whole rows of at most %d positions; the blocks' map is %d wide", npmax, W);
+  int TR = std::min(H, npmax / W);
+  const int tpu = (H + TR - 1) / TR;
+  TR = (H + tpu - 1) / tpu;
+  const size_t smem = (narrow ? res_conv_smem_floats<20>(TR, W) : res_conv_smem_floats<48>(TR, W)) * 4;
+  if (smem > kSmemLimit)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res_conv needs %zu bytes of shared memory, the limit is %zu", smem, kSmemLimit);
+  if ((int64_t)c.max_batch * tpu > kGridX)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "res_conv: max_batch %d x %d row tiles exceeds the %lld tiles a launch walks", c.max_batch,
+                   tpu, (long long)kGridX);
+  for (int k = 0; k < nl; ++k) {
+    d->rconv[k] = {H, W, C, r8 ? 1 : 1 << (k / 3), TR, wk[k], bn[k]};   // Res15 dilates: rate 2^(k // 3), res.py:10
+    layer(H, W, H, W, C);
+    d->flops += 2ll * H * W * 9 * C * C;
+  }
+  d->flops += 2ll * C * c.num_classes;
+  return TCR_OK;
+}
+
 extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   if (!cfg || !out) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   *out = nullptr;
   const bool kws = cfg->size == TCR_KWS_TRAD_FPOOL3 || cfg->size == TCR_KWS_ONE_FSTRIDE4;
   const bool res2d = cfg->size == TCR_RES2D8 || cfg->size == TCR_RES2D8_POOL;
-  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws && !res2d) {
+  const bool res = cfg->size == TCR_RES8 || cfg->size == TCR_RES8_NARROW || cfg->size == TCR_RES15 || cfg->size == TCR_RES15_NARROW;
+  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws && !res2d && !res) {
     set_error("DS-CNN size must be 'S', 'M' or 'L', or a KWS baseline: 'P' (trad_fpool3) or 'F' (one_fstride4), or a 2-D ablation: "
-              "'R' (ResNet2D8) or 'A' (ResNet2D8Pool)");
+              "'R' (ResNet2D8) or 'A' (ResNet2D8Pool), or a Honk ResNet: 'E' (Res8), 'N' (Res8Narrow), 'D' (Res15) or 'T' "
+              "(Res15Narrow)");
     return TCR_ERR_INVALID;
   }
   if (!res2d && cfg->width_multiplier != 0.0)
@@ -1847,10 +2189,15 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   if (cfg->size == TCR_KWS_ONE_FSTRIDE4 && cfg->width < 8) {
     return ds_fail(TCR_ERR_UNSUPPORTED, "one_fstride4 needs width >= 8 (its T x 8 conv is VALID), got %d", cfg->width);
   }
+  if ((cfg->size == TCR_RES8 || cfg->size == TCR_RES8_NARROW) && (cfg->height < 4 || cfg->width < 3)) {
+    return ds_fail(TCR_ERR_UNSUPPORTED, "Res8 / Res8Narrow need height >= 4 and width >= 3 (res_fconv's 4x3 / stride 1 average pool "
+                   "is VALID), got %d x %d", cfg->height, cfg->width);
+  }
   tcr_dscnn* d = new tcr_dscnn();
   d->cfg = *cfg;
   d->kws = kws;
   d->res2d = res2d;
+  d->res = res;
   if (const char* e = getenv("TCR_DSCNN_TC")) { d->use_tc = e[0] != '0'; d->tc_ws = e[0] != '1'; }
   struct Def { int type, depth, kh, kw, sh, sw; const char* scope; };
   std::vector<Def> defs;
@@ -1923,6 +2270,11 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     h = d->net.layer[3].hout; w = d->net.layer[3].wout; cin = d->net.layer[3].cout;
     defs.clear();
   }
+  if (res) {
+    const int rc = res_define(d, add);
+    if (rc != TCR_OK) { delete d; return rc; }
+    defs.clear();
+  }
   for (const Def& df : defs) {
     DsLayerDev L;
     memset(&L, 0, sizeof(L));
@@ -1956,7 +2308,7 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     h = L.hout; w = L.wout; cin = df.depth;
   }
   d->net.classes = cfg->num_classes;
-  if (!kws && !res2d) {
+  if (!kws && !res2d && !res) {
     d->net.fcw = add("DSCNN/fc1/weights", TCR_KIND_WEIGHT, {cin, cfg->num_classes});
     d->net.fcb = add("DSCNN/fc1/biases", TCR_KIND_BETA, {cfg->num_classes});
     d->flops += 2ll * cin * cfg->num_classes;
@@ -2147,6 +2499,52 @@ static int res2d_launch(tcr_dscnn* d, int l, const float* params, const float* i
   return TCR_OK;
 }
 
+// conv{k} on res_conv_kernel: a persistent grid of as many CTAs as fit on the device, walking n x tpu row tiles.
+template <int CP, bool RES>
+static int res_launch_conv(tcr_dscnn* d, const ResConv& R, const float* params, const float* in, const float* res, float* out, int32_t n,
+                           cudaStream_t s) {
+  const size_t smem = res_conv_smem_floats<CP>(R.TR, R.w) * 4;
+  const int tiles = n * ((R.h + R.TR - 1) / R.TR);
+  auto kfn = res_conv_kernel<CP, RES>;
+  int per_sm = 1;
+#ifndef TCR_EMU
+  static SmemOptIn optin;
+  if (optin.ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res_conv: shared memory opt-in failed");
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kfn, kResConvThreads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+#endif
+  const int grid = std::min(tiles, d->sms * per_sm);
+  TCR_LAUNCH(RES ? "res_conv_res" : "res_conv", kfn, dim3(grid), dim3(kResConvThreads), smem, s, R, (int)n, params, in, res, out, 1e-3f);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res_conv launch failed");
+  return TCR_OK;
+}
+
+// A layer of Res8 / Res15: 0 is f_conv (+ pool) on res_fconv_kernel, l = k + 1 is conv{k} on res_conv_kernel, with the residual for
+// odd k (the second conv of a block).  The block input is layer l - 2's output, which both dscnn_forward and forward_partial leave
+// in act[l & 1]: in a full forward that is also `out`.
+template <bool WIN>
+static int res_launch(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s, WindowView win) {
+  if (l == 0) {
+    const ResFconv& L = d->rfconv;
+    const size_t smem = res_fconv_smem_floats(L) * 4;
+    auto kfn = res_fconv_kernel<WIN>;
+#ifndef TCR_EMU
+    static SmemOptIn optin;
+    if (optin.ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res_fconv: shared memory opt-in failed");
+#endif
+    const unsigned grid = (unsigned)((int64_t)n * ((L.hout + L.RH - 1) / L.RH));
+    TCR_LAUNCH(WIN ? "res_fconv:win" : "res_fconv", kfn, dim3(grid), dim3(256), smem, s, L, params, in, out, win);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res_fconv launch failed");
+    return TCR_OK;
+  }
+  const ResConv& R = d->rconv[l - 1];
+  const bool residual = (l - 1) & 1, narrow = R.c == 19;
+  const float* block_in = d->act[l & 1];
+  if (narrow) return residual ? res_launch_conv<20, true>(d, R, params, in, block_in, out, n, s)
+                              : res_launch_conv<20, false>(d, R, params, in, nullptr, out, n, s);
+  return residual ? res_launch_conv<48, true>(d, R, params, in, block_in, out, n, s)
+                  : res_launch_conv<48, false>(d, R, params, in, nullptr, out, n, s);
+}
+
 // Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC), or for l == 0 with `win` the windows it describes.
 // The kernel is chosen here, once for every entry point: wgmma where the layer's shape fits the tensor-core kernels
 // (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.  The warp-specialised block kernel reads its input through a TMA map
@@ -2162,6 +2560,10 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
   if (L.type == kLayerRes2d) {
     if (win) return res2d_launch<true>(d, l, params, in, out, n, s, *win);
     return res2d_launch<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
+  }
+  if (L.type == kLayerRes) {
+    if (win) return res_launch<true>(d, l, params, in, out, n, s, *win);
+    return res_launch<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
   }
   if (L.type == 0) {
     if (win) return ds_launch_conv<true>(d, L, params, in, out, n, s, *win);
@@ -2233,9 +2635,9 @@ int tcr::dscnn_forward(tcr_dscnn* d, const float* feat, const float* params, int
   }
   if (d->kws) return kws_head(d, params, in, n, logits, probs, s);
   const DsLayerDev& last = d->net.layer[d->net.nlayers - 1];
-  if (d->res2d) {
-    TCR_LAUNCH("res2d_head", res2d_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes, d->r2fc,
-               params, in, logits, probs);
+  if (d->res2d || d->res) {
+    TCR_LAUNCH("res2d_head", res2d_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes,
+               d->res ? d->rfc : d->r2fc, params, in, logits, probs);
     if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "res2d_head launch failed");
     return TCR_OK;
   }

@@ -1,7 +1,8 @@
 """DS-CNN forward (inference) on the CUDA path: the reference's 2-D-conv comparison model
 (audio_nets/ds_cnn.py; DSCNN{S,M,L}Model.build_inference in factory/audio_nets.py:298-358), and on the same handle the KWS
 baselines cnn-trad-fpool3 (size 'P') and cnn-one-fstride4 ('F') of audio_nets/kws.py, and the paper's 2-D ablations of TC-ResNet8,
-ResNet2D8 ('R') and ResNet2D8Pool ('A') of audio_nets/tc_resnet.py.  Training DS-CNN is out of scope
+ResNet2D8 ('R') and ResNet2D8Pool ('A') of audio_nets/tc_resnet.py, and Honk's ResNets of audio_nets/res.py, Res8 ('E'), Res8Narrow
+('N'), Res15 ('D') and Res15Narrow ('T'), with their dilated 3x3 convolutions.  Training DS-CNN is out of scope
 (SURVEY.md 2 #13): weights come from a checkpoint keyed by the TF variable names in `self.table`.
 
 With a front-end (set_frontend) the handle also takes audio: `mfcc`, `forward_input`, `eval_accumulate` and `listener` mirror
@@ -21,6 +22,8 @@ from .engine import Listener, frontend_config, frontend_shape
 KWS_SIZES = {"trad_fpool3": "P", "one_fstride4": "F"}
 # and of the 2-D ablations, by TF scope; they alone take a width multiplier
 RES2D_SIZES = {"ResNet2D8": "R", "ResNet2D8Pool": "A"}
+# and of Honk's ResNets, by model name (all four under the TF scope "Res")
+RES_SIZES = {"Res8": "E", "Res8Narrow": "N", "Res15": "D", "Res15Narrow": "T"}
 
 
 class DsCnn:

@@ -5,8 +5,8 @@ executing on the CUDA engine instead of building a TF graph.
 train_audio.py:32), call `Model(args, dataset)`, then `model.build(wavs, labels, is_training)` and hand the model
 to the trainer / evaluator, which touch only the attributes set here and `session.run`.  TCResNet8Model and
 TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model, KWSModel (--architecture trad_fpool3 / one_fstride4),
-ResNet2D8Model and ResNet2D8PoolModel are on it for evaluation, deployment and streaming (their training is out of scope and raises NotImplementedError); the other entries of `_available_nets` (baselines the north star
-does not name) are registered so the CLI accepts them but raise NotImplementedError when built.
+ResNet2D8Model, ResNet2D8PoolModel and Res{8,8Narrow,15,15Narrow}Model are on it for evaluation, deployment and streaming (their
+training is out of scope and raises NotImplementedError).
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ import torch
 from ..common import utils
 from ..common.model_loader import EMA_SUFFIX
 from ..datasets import preprocessor_factory
-from ..dscnn import KWS_SIZES, RES2D_SIZES, DsCnn
+from ..dscnn import KWS_SIZES, RES2D_SIZES, RES_SIZES, DsCnn
 from ..engine import OPTIMIZER_DEFAULTS, OPTIMIZER_SLOT_NAMES, Engine
 from ..runtime import InvalidArgumentError, Node
 from .base import TFModel
@@ -543,23 +543,6 @@ class TCResNet14Model(AudioNetModel):
     add_arguments = staticmethod(_tc_flags)
 
 
-def _baseline(name, flags):
-    def add_arguments(parser):
-        for flag, default in flags:
-            if isinstance(default, str):
-                parser.add_argument(flag, default=default, type=str)
-            else:
-                parser.add_argument(flag, default=default, type=float)
-    return type(name, (AudioNetModel,), {"add_arguments": staticmethod(add_arguments), "__doc__":
-                "Baseline of the reference registered for CLI compatibility; not on the accelerated path."})
-
-
-Res8Model = _baseline("Res8Model", [("--weight_decay", 0.00001)])
-Res8NarrowModel = _baseline("Res8NarrowModel", [("--weight_decay", 0.00001)])
-Res15Model = _baseline("Res15Model", [("--weight_decay", 0.00001)])
-Res15NarrowModel = _baseline("Res15NarrowModel", [("--weight_decay", 0.00001)])
-
-
 class DsCnnModel(AudioNetModel):
     """DSCNN{S,M,L}Model (factory/audio_nets.py:299-359, audio_nets/ds_cnn.py) in evaluation mode on dscnn.DsCnn: the handle runs the
     model's front-end (tcr_dscnn_set_frontend), the forward with the BatchNorm moving statistics held in its flat parameters
@@ -733,12 +716,18 @@ class _Res2dModel(DsCnnModel):
         return super().build_inference(inputs, is_training=False)
 
     def _regularization(self) -> float:
-        wd = float(self.args.weight_decay)
-        if not wd:
-            return 0.0
-        p = self.params.double()
-        return wd * 0.5 * sum(float((p[d["offset"]:d["offset"] + d["numel"]] ** 2).sum()) for d in self.engine.table
-                              if d["kind"] == "weight")
+        return _weights_l2(self)
+
+
+def _weights_l2(model: DsCnnModel) -> float:
+    """build_loss's L2 term, weight_decay * sum(tf.nn.l2_loss(w)) over the weights of the parameter table (every variable outside
+    BatchNorm)."""
+    wd = float(model.args.weight_decay)
+    if not wd:
+        return 0.0
+    p = model.params.double()
+    return wd * 0.5 * sum(float((p[d["offset"]:d["offset"] + d["numel"]] ** 2).sum()) for d in model.engine.table
+                          if d["kind"] == "weight")
 
 
 class ResNet2D8Model(_Res2dModel):
@@ -747,3 +736,47 @@ class ResNet2D8Model(_Res2dModel):
 
 class ResNet2D8PoolModel(_Res2dModel):
     scope = "ResNet2D8Pool"
+
+
+class _ResModel(DsCnnModel):
+    """Res8Model / Res8NarrowModel / Res15Model / Res15NarrowModel (factory/audio_nets.py:227-297, audio_nets/res.py): Honk's ResNets
+    in evaluation mode on the DS-CNN handle (size codes dscnn.RES_SIZES), Res15 with its dilated convolutions.  Variables are
+    restored by their TF names ("Res/conv0/Conv/weights", ...).  --weight_decay keeps the reference's 1e-5 default, and total_loss
+    adds build_loss's L2 term over the trainable variables, which are all weights.  Training is out of scope."""
+    net: str = ""
+
+    @staticmethod
+    def add_arguments(parser):
+        parser.add_argument("--weight_decay", default=0.00001, type=float)
+
+    @property
+    def dscnn_size(self) -> str:
+        return RES_SIZES[self.net]
+
+    def build_inference(self, inputs, is_training=True):
+        if is_training:
+            raise NotImplementedError(f"{type(self).__name__}: training Res8 / Res15 is out of scope on the CUDA path; evaluation "
+                                      "(evaluate_audio.py), the deployable model and the listener (listen_audio.py) are supported")
+        if getattr(self.args, "device_dataset", False):
+            raise NotImplementedError(f"{type(self).__name__}: --device_dataset serves the TC-ResNet models only; evaluate from the "
+                                      "dataset on disk")
+        return super().build_inference(inputs, is_training=False)
+
+    def _regularization(self) -> float:
+        return _weights_l2(self)
+
+
+class Res8Model(_ResModel):
+    net = "Res8"
+
+
+class Res8NarrowModel(_ResModel):
+    net = "Res8Narrow"
+
+
+class Res15Model(_ResModel):
+    net = "Res15"
+
+
+class Res15NarrowModel(_ResModel):
+    net = "Res15Narrow"
