@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 14
+#define TCR_ABI_VERSION 15
 
 enum {
   TCR_OK = 0,
@@ -345,6 +345,33 @@ int tcr_listener_history(const tcr_listener* L, float** history, int32_t* frames
 int tcr_eval_accumulate(tcr_handle* h, const float* scores, const float* onehot, int32_t n, int32_t topk, int64_t* counts,
                         tcr_stream stream);
 
+/* Ranking metrics on the device (ABI 15): the reference's MAPMetricOp (average_precision_score at macro, micro, weighted and
+ * samples) and APMetricOp (per-class AP), metrics/ops/non_tensor_ops.py:15-61, :296-343.  Scores stay on the device for the whole
+ * evaluation in a caller-owned store; one ranking pass at the end computes every AP.
+ *   tcr_eval_collect  appends rows [row_offset, row_offset + n) of the store: store_scores device fp32 [capacity, classes] <- scores,
+ *                     store_labels device int32 [capacity] <- the first maximum of each one-hot row (tcr_eval_accumulate's rule).
+ *                     scores MUST be the softmax outputs (tcr_forward's probs), as the reference ranks predictions_onehot: unlike
+ *                     the arg-max, a class's ranking across utterances differs between logits and softmax.
+ *                     TCR_ERR_INVALID unless capacity * classes <= 2^31 - 1 and the rows lie inside [0, capacity).
+ *   tcr_eval_rank     ranks the store's first n rows.  workspace == NULL is the query: *workspace_bytes <- the device bytes the
+ *                     pass needs, nothing runs.  Otherwise workspace (device, 256-byte aligned, *workspace_bytes of it) is scratch
+ *                     and result (device fp64 [2 * classes + 4]) receives:
+ *                       [0, classes)            AP of each class, sklearn's definition: the class's n scores sorted in descending
+ *                                               order, equal scores grouped, sum over groups of (R_g - R_{g-1}) * P_g; 0 for a
+ *                                               class without positives (sklearn 1.x);
+ *                       [classes, 2 * classes)  positives of each class (the support);
+ *                       [2 * classes + 0]       macro: the mean of the per-class APs;
+ *                       [2 * classes + 1]       micro: the AP of all n * classes (score, is-label) pairs ranked together;
+ *                       [2 * classes + 2]       weighted: the per-class APs weighted by their support;
+ *                       [2 * classes + 3]       samples: the mean over rows of 1 / |{c : p_c >= p_label}|.
+ *                     A NaN score makes every average it enters NaN.  The result is deterministic and depends only on the stored
+ *                     rows, not on how many rows each collect call wrote.  TCR_ERR_INVALID unless classes <= 32 and
+ *                     1 <= n with n * classes <= 2^31 - 1. */
+int tcr_eval_collect(tcr_handle* h, const float* scores, const float* onehot, int32_t n, int32_t row_offset, int32_t capacity,
+                     float* store_scores, int32_t* store_labels, tcr_stream stream);
+int tcr_eval_rank(tcr_handle* h, const float* store_scores, const int32_t* store_labels, int32_t n, void* workspace,
+                  int64_t* workspace_bytes, double* result, tcr_stream stream);
+
 /* Forward + backward + optimizer (momentum, Adam or RMSProp: tcr_step_args::optimizer) + BN moving-average update
  * (helper/trainer.py:171-222, slim.learning.create_train_op).  With a communicator attached (tcr_comm_init) gradients are
  * averaged over ranks with one ncclAllReduce (or the peer-memory exchange) before the update; every rank then applies the
@@ -495,6 +522,8 @@ int tcr_dscnn_forward_partial(tcr_dscnn* d, const float* features, const float* 
  *                          front-end into the handle's feature buffer, then the same forward, so the result equals
  *                          tcr_dscnn_forward on tcr_dscnn_mfcc_forward's features bit for bit.
  * tcr_dscnn_eval_accumulate  tcr_eval_accumulate's counts (same kernel, same layout) for num_classes of the DS-CNN handle.
+ * tcr_dscnn_eval_collect / tcr_dscnn_eval_rank  tcr_eval_collect / tcr_eval_rank (same kernels, same store, workspace and result
+ *                          layout, same softmax convention) for num_classes of the DS-CNN handle (ABI 15).
  * tcr_dscnn_listener_create  a tcr_listener (see above) on the DS-CNN handle and its front-end; tcr_listener_reset / _push / _history
  *                          / _destroy are shared, with the same four promises (tcr_dscnn_forward in place of tcr_forward).  Its
  *                          pushes pass moving = NULL.  TCR_ERR_INVALID without a front-end. */
@@ -504,6 +533,10 @@ int tcr_dscnn_forward_input(tcr_dscnn* d, const void* input, int32_t input_kind,
                             float* probs, tcr_stream stream);
 int tcr_dscnn_eval_accumulate(tcr_dscnn* d, const float* scores, const float* onehot, int32_t n, int32_t topk, int64_t* counts,
                               tcr_stream stream);
+int tcr_dscnn_eval_collect(tcr_dscnn* d, const float* scores, const float* onehot, int32_t n, int32_t row_offset, int32_t capacity,
+                           float* store_scores, int32_t* store_labels, tcr_stream stream);
+int tcr_dscnn_eval_rank(tcr_dscnn* d, const float* store_scores, const int32_t* store_labels, int32_t n, void* workspace,
+                        int64_t* workspace_bytes, double* result, tcr_stream stream);
 int tcr_dscnn_listener_create(tcr_dscnn* d, const tcr_listener_config* cfg, tcr_listener** out);
 
 /* Process-wide launch accounting (no reference counterpart; the reference only logs wall-clock per

@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libtcr_b200.so")
 
 TCR_MODEL_TCRESNET8 = 8
 TCR_MODEL_TCRESNET14 = 14
-ABI_VERSION = 14       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
+ABI_VERSION = 15       # TCR_ABI_VERSION of include/tcr_b200.h this binding was written against
 TCR_INPUT_WAV_F32, TCR_INPUT_FEATURES, TCR_INPUT_WAV_PCM16 = 0, 1, 2
 TCR_OPT_MOMENTUM, TCR_OPT_ADAM, TCR_OPT_RMSPROP = 0, 1, 2
 TCR_FEATURE_MFCC = 0
@@ -115,6 +115,10 @@ SYMBOLS = {
     "tcr_listener_destroy": (C.c_int, [C.c_void_p]),
     "tcr_listener_history": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int32)]),
     "tcr_eval_accumulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "tcr_eval_collect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_void_p]),
+    "tcr_eval_rank": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p,
+                                C.c_void_p]),
     "tcr_comm_set_sync_bn": (C.c_int, [C.c_void_p, C.c_int32]),
     "tcr_train_step": (C.c_int, [C.c_void_p, C.POINTER(TcrStepArgs), C.c_void_p]),
     "tcr_set_trainable": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
@@ -139,6 +143,10 @@ SYMBOLS = {
     "tcr_dscnn_mfcc_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
     "tcr_dscnn_forward_input": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "tcr_dscnn_eval_accumulate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "tcr_dscnn_eval_collect": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                         C.c_void_p, C.c_void_p]),
+    "tcr_dscnn_eval_rank": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int64), C.c_void_p,
+                                      C.c_void_p]),
     "tcr_dscnn_listener_create": (C.c_int, [C.c_void_p, C.POINTER(TcrListenerConfig), C.POINTER(C.c_void_p)]),
     "tcr_profile_enable": (C.c_int, [C.c_int]),
     "tcr_profile_read": (C.c_int, [C.POINTER(C.POINTER(TcrKernelStat)), C.POINTER(C.c_int32)]),

@@ -683,6 +683,32 @@ extern "C" int tcr_eval_accumulate(tcr_handle* h, const float* scores, const flo
   return TCR_OK;
 }
 
+extern "C" int tcr_eval_collect(tcr_handle* h, const float* scores, const float* onehot, int32_t n, int32_t row_offset, int32_t capacity,
+                                float* store_scores, int32_t* store_labels, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!h || !scores || !onehot || !store_scores || !store_labels) return fail(TCR_ERR_INVALID, "NULL argument");
+  if (const char* why = eval_rank_refusal(capacity, h->cfg.num_classes)) return fail(TCR_ERR_INVALID, "capacity %d: %s", capacity, why);
+  if (n <= 0 || row_offset < 0 || (int64_t)row_offset + n > capacity)
+    return fail(TCR_ERR_INVALID, "rows [%d, %lld) outside the store's %d rows", row_offset, (long long)row_offset + n, capacity);
+  eval_collect_launch(scores, onehot, n, h->cfg.num_classes, row_offset, store_scores, store_labels, (cudaStream_t)stream);
+  TCR_CUDA(cudaGetLastError());
+  return TCR_OK;
+}
+
+extern "C" int tcr_eval_rank(tcr_handle* h, const float* store_scores, const int32_t* store_labels, int32_t n, void* workspace,
+                             int64_t* workspace_bytes, double* result, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!h || !workspace_bytes) return fail(TCR_ERR_INVALID, "NULL argument");
+  if (const char* why = eval_rank_refusal(n, h->cfg.num_classes)) return fail(TCR_ERR_INVALID, "n %d: %s", n, why);
+  const int64_t need = eval_rank_workspace_bytes(n, h->cfg.num_classes);
+  if (!workspace) { *workspace_bytes = need; return TCR_OK; }
+  if (!store_scores || !store_labels || !result) return fail(TCR_ERR_INVALID, "NULL argument");
+  if (*workspace_bytes < need) return fail(TCR_ERR_INVALID, "workspace of %lld bytes, %lld needed", (long long)*workspace_bytes, (long long)need);
+  eval_rank_launch(store_scores, store_labels, n, h->cfg.num_classes, workspace, result, (cudaStream_t)stream);
+  TCR_CUDA(cudaGetLastError());
+  return TCR_OK;
+}
+
 // Front-end running ahead (tcr_step_args::input_resident): lazily created low-priority stream, second feature buffer, events.
 static int frontend_ahead_get(tcr_handle* h) {
   if (h->fe_stream) return TCR_OK;

@@ -2720,6 +2720,33 @@ extern "C" int tcr_dscnn_eval_accumulate(tcr_dscnn* d, const float* scores, cons
   return TCR_OK;
 }
 
+extern "C" int tcr_dscnn_eval_collect(tcr_dscnn* d, const float* scores, const float* onehot, int32_t n, int32_t row_offset,
+                                      int32_t capacity, float* store_scores, int32_t* store_labels, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !scores || !onehot || !store_scores || !store_labels) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  if (const char* why = eval_rank_refusal(capacity, d->cfg.num_classes)) return ds_fail(TCR_ERR_INVALID, "capacity %d: %s", capacity, why);
+  if (n <= 0 || row_offset < 0 || (int64_t)row_offset + n > capacity)
+    return ds_fail(TCR_ERR_INVALID, "rows [%d, %lld) outside the store's %d rows", row_offset, (long long)row_offset + n, capacity);
+  eval_collect_launch(scores, onehot, n, d->cfg.num_classes, row_offset, store_scores, store_labels, (cudaStream_t)stream);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "eval_collect launch failed");
+  return TCR_OK;
+}
+
+extern "C" int tcr_dscnn_eval_rank(tcr_dscnn* d, const float* store_scores, const int32_t* store_labels, int32_t n, void* workspace,
+                                   int64_t* workspace_bytes, double* result, tcr_stream stream) {
+  pdl_chain_reset();
+  if (!d || !workspace_bytes) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  if (const char* why = eval_rank_refusal(n, d->cfg.num_classes)) return ds_fail(TCR_ERR_INVALID, "n %d: %s", n, why);
+  const int64_t need = eval_rank_workspace_bytes(n, d->cfg.num_classes);
+  if (!workspace) { *workspace_bytes = need; return TCR_OK; }
+  if (!store_scores || !store_labels || !result) return ds_fail(TCR_ERR_INVALID, "NULL argument");
+  if (*workspace_bytes < need)
+    return ds_fail(TCR_ERR_INVALID, "workspace of %lld bytes, %lld needed", (long long)*workspace_bytes, (long long)need);
+  eval_rank_launch(store_scores, store_labels, n, d->cfg.num_classes, workspace, result, (cudaStream_t)stream);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "eval_rank launch failed");
+  return TCR_OK;
+}
+
 extern "C" int tcr_dscnn_forward_partial(tcr_dscnn* d, const float* features, const float* params, int32_t n, int32_t num_layers,
                                          float* act_out, tcr_stream stream) {
   pdl_chain_reset();

@@ -49,6 +49,14 @@ int augment_launch(const int16_t* pcm, int64_t pcm_stride, const tcr_augment_cli
 int dataset_batch_launch(const tcr_dataset& ds, int64_t position, int64_t epoch, uint64_t seed, float* out, float* onehot, int clip,
                          int classes, int n, cudaStream_t s);
 int eval_accumulate_launch(const float* scores, const float* onehot, int n, int classes, int topk, int64_t* counts, cudaStream_t s);
+// Ranking metrics (tcr_metrics.cu): append a batch to the score store at row_offset; the refusal of a ranking over n rows (nullptr
+// when accepted); its workspace bytes; the ranking pass writing result [2 * classes + 4] (layout in include/tcr_b200.h).
+int eval_collect_launch(const float* scores, const float* onehot, int n, int classes, int64_t row_offset, float* store_scores,
+                        int32_t* store_labels, cudaStream_t s);
+const char* eval_rank_refusal(int64_t n, int classes);
+int64_t eval_rank_workspace_bytes(int n, int classes);
+int eval_rank_launch(const float* store_scores, const int32_t* store_labels, int n, int classes, void* workspace, double* result,
+                     cudaStream_t s);
 int net_weight_transpose(tcr_handle* h, const float* params, cudaStream_t s);
 int sync_records(tcr_handle* h, const float* part, int gc, int cols, float* out, cudaStream_t s);   // SyncBN: sum records, all-reduce
 inline bool sync_bn_on(const tcr_handle* h) { return h->sync_bn && h->world > 1 && h->comm; }

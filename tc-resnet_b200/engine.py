@@ -360,6 +360,32 @@ class Engine:
                                                        self._stream), "tcr_eval_accumulate")
         return counts
 
+    def eval_collect(self, scores: torch.Tensor, onehot: torch.Tensor, store_scores: torch.Tensor, store_labels: torch.Tensor,
+                     row_offset: int) -> None:
+        """Appends one batch of SOFTMAX scores and its label indices to the ranking store (fp32 [capacity, C], int32 [capacity]) at
+        row_offset; see tcr_eval_collect in include/tcr_b200.h."""
+        L.check(self.lib, self.lib.tcr_eval_collect(self._h, self._ptr(scores), self._ptr(onehot), scores.shape[0], int(row_offset),
+                                                    store_scores.shape[0], self._ptr(store_scores), self._ptr(store_labels, torch.int32),
+                                                    self._stream), "tcr_eval_collect")
+
+    def eval_rank_workspace(self, n: int) -> torch.Tensor:
+        """The device workspace eval_rank needs for n stored rows (the tcr_eval_rank query)."""
+        nb = C.c_int64()
+        L.check(self.lib, self.lib.tcr_eval_rank(self._h, None, None, int(n), None, C.byref(nb), None, self._stream), "tcr_eval_rank")
+        return torch.empty(nb.value, dtype=torch.uint8, device=self.device)
+
+    def eval_rank(self, store_scores: torch.Tensor, store_labels: torch.Tensor, n: int,
+                  workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The ranking pass over the store's first n rows: fp64 [2C + 4] = per-class AP, per-class positives, then the macro,
+        micro, weighted and samples averages (tcr_eval_rank).  metrics.manager.ranking_metrics names them."""
+        ws = workspace if workspace is not None else self.eval_rank_workspace(n)
+        nb = C.c_int64(ws.numel())
+        out = torch.empty(2 * self.num_classes + 4, dtype=torch.float64, device=self.device)
+        L.check(self.lib, self.lib.tcr_eval_rank(self._h, self._ptr(store_scores), self._ptr(store_labels, torch.int32), int(n),
+                                                 self._ptr(ws, torch.uint8), C.byref(nb), self._ptr(out, torch.float64), self._stream),
+                "tcr_eval_rank")
+        return out
+
     def listener(self, streams: int, hop_frames: int, chunk_samples: int, params: Optional[torch.Tensor] = None,
                  moving: Optional[torch.Tensor] = None) -> "Listener":
         """A continuous-audio listener on this handle (tcr_listener_*): `streams` streams, a window every `hop_frames` frames,

@@ -50,6 +50,8 @@ class AudioNetModel(TFModel):
         self._feed_slots = []
         self._loss_ring, self._loss_pending, self._loss_submitted = [], [], 0   # --device_dataset: (device, pinned, event) loss slots
         self._counts = None                                        # device int64 [classes^2 + 2] (tcr_eval_accumulate)
+        self._rank = None                                          # (scores, labels, workspace) of the ranking store (tcr_eval_collect)
+        self._rank_rows = 0
 
     # ------------------------------------------------------------------ graph-construction API of the reference
     def build(self, wavs, labels, is_training):
@@ -293,6 +295,28 @@ class AudioNetModel(TFModel):
             self._counts.zero_()
         return out
 
+    def reserve_ranking(self, rows: int) -> None:
+        """Empties the device store of the ranking metrics and sizes it, with its workspace, for `rows` utterances: the scores of
+        every evaluation batch are collected there (tcr_eval_collect) until read_ranking()."""
+        if self._rank is None or self._rank[0].shape[0] < rows:
+            self._rank = None                                       # the old store goes before the new one is allocated
+            self._rank = (torch.empty(rows, self.args.num_classes, dtype=torch.float32, device=self.engine.device),
+                          torch.empty(rows, dtype=torch.int32, device=self.engine.device), self.engine.eval_rank_workspace(rows))
+        self._rank_rows = 0
+
+    def _collect(self, probs, onehot) -> None:
+        if self._rank is not None:
+            self.engine.eval_collect(probs, onehot, self._rank[0], self._rank[1], self._rank_rows)
+            self._rank_rows += probs.shape[0]
+
+    def read_ranking(self) -> Optional[np.ndarray]:
+        """The ranking pass over the utterances collected since reserve_ranking() (one D2H read of 2 * classes + 4 doubles, see
+        metrics.manager.ranking_metrics), or None when none were; empties the store."""
+        n, self._rank_rows = self._rank_rows, 0
+        if self._rank is None or n == 0:
+            return None
+        return self.engine.eval_rank(self._rank[0], self._rank[1], n, self._rank[2]).cpu().numpy()
+
     # ------------------------------------------------------------------ one session.run
     def _execute_train_fast(self, names: Set[str]) -> Optional[Dict[str, object]]:
         """session.run(train_op) through the host-buffer step of the C ABI (tcr_train_step_host via engine.HostFeed): the batch goes
@@ -419,6 +443,7 @@ class AudioNetModel(TFModel):
             if self._counts is None:
                 self._counts = torch.zeros(self.args.num_classes ** 2 + 2, dtype=torch.int64, device=self.engine.device)
             self.engine.eval_accumulate(out["probs"], self._d_hot, self._counts, topk=5)
+            self._collect(out["probs"], self._d_hot)
             vals["metric_counts"] = None
         losses = out["losses"].cpu().numpy()                    # the D2H read synchronises the step
         vals.update(total_loss=losses[0], model_loss=losses[1], global_step=np.int64(self.global_step))
@@ -625,6 +650,7 @@ class DsCnnModel(AudioNetModel):
             if self._counts is None:
                 self._counts = torch.zeros(self.args.num_classes ** 2 + 2, dtype=torch.int64, device=self.engine.device)
             self.engine.eval_accumulate(probs, self._d_hot, self._counts, topk=5)
+            self._collect(probs, self._d_hot)
             vals["metric_counts"] = None
         lg = logits.cpu().numpy().astype(np.float64)            # the D2H read synchronises the forward
         ls = float(getattr(self.args, "label_smoothing", 0.0) or 0.0)

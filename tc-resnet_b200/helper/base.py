@@ -38,6 +38,8 @@ class Base(ABC):
         fetch_ops = self.build_evaluation_fetch_ops(do_eval)
         agg = {k: [] for k in fetch_ops}
         agg.update(batch_infer_time=[], unit_infer_time=[])
+        if "metric_counts" in fetch_ops:                               # the scores of every batch stay on the device for the ranking
+            self.model.reserve_ranking(iters * self.args.batch_size)
         for _ in range(iters):
             try:
                 t0 = time.perf_counter()
@@ -57,6 +59,7 @@ class Base(ABC):
         out = {k: np.vstack(v) for k, v in agg.items() if v}
         if "metric_counts" in fetch_ops:                               # ONE device-to-host read per evaluation
             out["metric_counts"] = self.model.read_metric_counts(reset=True)
+            out["ranking"] = self.model.read_ranking()
         return out
 
     def run_evaluation(self, global_step: int, iters: int = None, is_training: bool = False):
@@ -96,4 +99,4 @@ class AudioBase(Base):
     def build_non_tensor_data_from_eval_dict(self, eval_dict, **kwargs):
         return {"dataset_split_name": self.dataset.dataset_split_name, "label_names": self.dataset.label_names,
                 "predictions_onehot": eval_dict.get("predictions_onehot"), "labels_onehot": eval_dict.get("labels_onehot"),
-                "metric_counts": eval_dict.get("metric_counts")}
+                "metric_counts": eval_dict.get("metric_counts"), "ranking": eval_dict.get("ranking")}
