@@ -207,26 +207,30 @@ class ResNet:
         return got[:n]
 
 
-def check_net(net, feat, layers=None):
+def check_net(net, feat, layers=None, rows=None):
     """Layers (1-based counts of forward_partial, all by default) on the path's own input to them, and for a block's second conv the
     path's own block input, against res_oracle.layer within 1e-5 of the layer's maximum; then logits against the fp64 oracle within
-    1e-4 and the softmax, with the arg-max equal wherever the oracle's top-2 margin exceeds the error."""
+    1e-4 and the softmax, with the arg-max equal wherever the oracle's top-2 margin exceeds the error.  rows: the utterances the
+    oracle checks (all by default; the NaN canary and the finiteness check cover the whole batch).  Returns the relative error of
+    each layer, and of the logits under "logits", and the logits of the whole batch."""
     spec, p = net.spec, net.p
     layers = range(1, spec.layers + 2) if layers is None else layers
-    outs = {0: feat.astype(np.float64)}
+    rows = slice(None) if rows is None else rows
+    outs = {0: feat[rows].astype(np.float64)}
     for k in sorted({j for k in layers for j in (k, k - 1, k - 2) if j >= 1}):
-        outs[k] = net.layer_output(feat, k).astype(np.float64)
+        outs[k] = net.layer_output(feat, k)[rows].astype(np.float64)
     errs = {k: rel_err(outs[k], R.layer(spec, p, k - 1, outs[k - 1], outs.get(k - 2) if k >= 3 else None)) for k in layers}
     assert max(errs.values()) <= 1e-5, errs
     logits, probs = net.forward(feat)
-    ref = R.forward(spec, p, feat.astype(np.float64))
-    err = np.abs(logits - ref).max()
+    ref = R.forward(spec, p, feat[rows].astype(np.float64))
+    err = np.abs(logits[rows] - ref).max()
     assert err <= 1e-4 * np.abs(ref).max(), err / np.abs(ref).max()
     e = np.exp(ref - ref.max(1, keepdims=True))
-    np.testing.assert_allclose(probs, e / e.sum(1, keepdims=True), atol=max(2e-5, 2 * err))
-    top2 = np.sort(ref, 1)[:, -2:]
+    np.testing.assert_allclose(probs[rows], e / e.sum(1, keepdims=True), atol=max(2e-5, 2 * err))
+    top2 = np.sort(ref, 1)[:, -2:]                                     # one column for a single class: no margin to check
     clear = top2[:, -1] - top2[:, 0] > 2 * err
-    assert np.array_equal(logits.argmax(1)[clear], ref.argmax(1)[clear])
+    assert np.array_equal(logits[rows].argmax(1)[clear], ref.argmax(1)[clear])
+    errs["logits"] = float(err / np.abs(ref).max())
     return errs, logits
 
 
