@@ -2065,9 +2065,10 @@ static int res2d_define(tcr_dscnn* d, Add& add) {
     if (B.down) { B.wd = convs[ci].w; B.bnd = convs[ci].bn; ++ci; }
     B.w0 = convs[ci].w; B.bn0 = convs[ci].bn; ++ci;
     B.w1 = convs[ci].w; B.bn1 = convs[ci].bn; ++ci;
-    // tile plan: up to 8 x 16 output positions and every output channel at once; filter slices of down to 32 channels keep it
-    // near 100 KB of shared memory (two CTAs per SM), and past 200 KB the tile shrinks.  Then balanced, so that the last tile
-    // of a row or column is not a sliver.  The plan depends on the geometry alone, so an utterance's bits do not depend on n.
+    // tile plan: up to 8 x 16 output positions and every output channel at once.  Past 100 KB of shared memory (two CTAs per
+    // SM) the filter slice COT halves, to a multiple of 4, until it is at most 32 channels: a sliced layer takes slices of 20 to
+    // 32 channels and a shorter last one.  Past 200 KB the tile shrinks.  Then balanced, so that the last tile of a row or
+    // column is not a sliver.  The plan depends on the geometry alone, so an utterance's bits do not depend on n.
     B.RH = std::min(B.hout, 8); B.WT = std::min(B.wout, 16); B.COT = r2_pad4(B.cout);
     auto bytes = [&] { return r2_block_smem(B).floats * 4; };
     while (bytes() > 100 * 1024 && B.COT > 32) B.COT = r2_pad4(B.COT / 2);

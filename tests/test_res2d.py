@@ -224,25 +224,30 @@ class Res2dNet:
         return got[:n]
 
 
-def check_net(net, feat):
+def check_net(net, feat, rows=None):
     """Each layer on the path's own input to it against res2d_oracle.layer, within 1e-5 of the layer's maximum, then logits against
-    the fp64 oracle within 1e-4 and the softmax, with the arg-max equal wherever the oracle's top-2 margin exceeds the error."""
+    the fp64 oracle within 1e-4 and the softmax, with the arg-max equal wherever the oracle's top-2 margin exceeds the error.  rows:
+    the utterances the oracle checks (all by default; the NaN canary and the finiteness check cover the whole batch).  Returns the
+    relative error of each layer (1-based, as forward_partial counts them) and of the logits under "logits", and the logits of the
+    whole batch."""
     spec, p = net.spec, net.p
-    errs, x = [], feat.astype(np.float64)
+    rows = slice(None) if rows is None else rows
+    errs, x = {}, feat[rows].astype(np.float64)
     for k in range(1, 5):
-        out = net.layer_output(feat, k)
-        errs.append(rel_err(out, R.layer(spec, p, k - 1, x)))
+        out = net.layer_output(feat, k)[rows]
+        errs[k] = rel_err(out, R.layer(spec, p, k - 1, x))
         x = out.astype(np.float64)
-    assert max(errs) <= 1e-5, errs
+    assert max(errs.values()) <= 1e-5, errs
     logits, probs = net.forward(feat)
-    ref = R.forward(spec, p, feat.astype(np.float64))
-    err = np.abs(logits - ref).max()
+    ref = R.forward(spec, p, feat[rows].astype(np.float64))
+    err = np.abs(logits[rows] - ref).max()
     assert err <= 1e-4 * np.abs(ref).max(), err / np.abs(ref).max()
     e = np.exp(ref - ref.max(1, keepdims=True))
-    np.testing.assert_allclose(probs, e / e.sum(1, keepdims=True), atol=max(2e-5, 2 * err))
-    top2 = np.sort(ref, 1)[:, -2:]
+    np.testing.assert_allclose(probs[rows], e / e.sum(1, keepdims=True), atol=max(2e-5, 2 * err))
+    top2 = np.sort(ref, 1)[:, -2:]                                     # one column for a single class: no margin to check
     clear = top2[:, -1] - top2[:, 0] > 2 * err
-    assert np.array_equal(logits.argmax(1)[clear], ref.argmax(1)[clear])
+    assert np.array_equal(logits[rows].argmax(1)[clear], ref.argmax(1)[clear])
+    errs["logits"] = float(err / np.abs(ref).max())
     return errs, logits
 
 
