@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TCR_ABI_VERSION 15
+#define TCR_ABI_VERSION 16
 
 enum {
   TCR_OK = 0,
@@ -450,6 +450,22 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
  * are [conv1 + pool, conv2] for 'P' and [conv] for 'F', each written NHWC ([n, hout, wout, cout], the pooled width for 'P''s
  * first), and, as for DS-CNN, the head is not among them.
  *
+ * And two of KWSModel's TensorFlow speech_commands nets (audio_nets/kws.py), evaluation mode (ABI 16); every layer has a bias:
+ *   size TCR_KWS_LOW_LATENCY_CONV ('C', --architecture low_latency_conv): height x 8 conv 1 -> 186, VALID, stride 1, + bias, ReLU,
+ *     then flatten and first_fc, second_fc, final_fc, each + bias with no nonlinearity, softmax.  With W = width - 7: variables
+ *     "first_weights" [height, 8, 1, 186], "first_bias" [186], "first_fc_weights" [W * 186, 128], "first_fc_bias" [128],
+ *     "second_fc_weights" [128, 128], "second_fc_bias" [128], "final_fc_weights" [128, classes], "final_fc_bias" [classes].
+ *     Needs width >= 8 and max_batch x W <= 2^31 - 1 (the conv's GEMM rows).
+ *   size TCR_KWS_TINY_CONV ('Y', --architecture tiny_conv): 10 x 8 conv 1 -> 8, TF SAME at stride 2 x 2, + bias, ReLU, then
+ *     flatten and final_fc + bias, softmax.  H = ceil(height / 2), W = ceil(width / 2); SAME pads pad_total = max((out - 1) * 2 + k
+ *     - in, 0) zeros, pad_total / 2 (rounded down) before (above / left) and the rest after.  Variables "first_weights" [10, 8, 1, 8],
+ *     "first_bias" [8], "final_fc_weights" [H * W * 8, classes], "final_fc_bias" [classes].  Takes any height; needs the conv's
+ *     staged rows, 4 * (648 + (2 * min(H, 8) + 8) * (2 W + 6)) bytes, within 227 KB of shared memory (width <= 2,388 from height 15 up).
+ *   Both: the flattened conv output K (W * 186, or H * W * 8) must be below 2^31, in at most 2^31 - 1 chunk x batch-group CTAs of
+ *   the split dense layer.  Weights have kind TCR_KIND_WEIGHT and biases TCR_KIND_BETA.  forward_flops counts 2 x multiply-adds
+ *   of the conv and the matmuls (tiny_conv: the full 80-tap kernel at every output), not the bias adds.  forward_partial's only
+ *   layer is the conv, NHWC [n, 1, W, 186] or [n, H, W, 8]; the dense head is not among them.
+ *
  * And the paper's 2-D ablations of TC-ResNet8 (audio_nets/tc_resnet.py ResNet2D8 / ResNet2D8Pool), evaluation mode (ABI 13):
  *   size TCR_RES2D8 ('R'): conv0 3x3 1 -> c0 + BN + ReLU, then three residual blocks of c1, c2, c3 channels: conv{i}_0 3x3 at stride
  *     s + BN + ReLU, conv{i}_1 3x3 + BN, plus the shortcut, then ReLU.  Where a block changes the channel count, s = 2 and the
@@ -481,6 +497,8 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
  * add and BN for conv{2i+1}): 7 layers for Res8, 14 for Res15. */
 #define TCR_KWS_TRAD_FPOOL3 'P'
 #define TCR_KWS_ONE_FSTRIDE4 'F'
+#define TCR_KWS_LOW_LATENCY_CONV 'C'
+#define TCR_KWS_TINY_CONV 'Y'
 #define TCR_RES2D8 'R'
 #define TCR_RES2D8_POOL 'A'
 #define TCR_RES8 'E'
@@ -489,8 +507,8 @@ int tcr_measure_fp32_peak(tcr_handle* h, double* tflops, tcr_stream stream);
 #define TCR_RES15_NARROW 'T'
 typedef struct tcr_dscnn tcr_dscnn;
 typedef struct tcr_dscnn_config {
-  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 | TCR_RES2D8 | TCR_RES2D8_POOL | TCR_RES8 |
-                            TCR_RES8_NARROW | TCR_RES15 | TCR_RES15_NARROW */
+  int32_t size;          /* 'S' | 'M' | 'L' | TCR_KWS_TRAD_FPOOL3 | TCR_KWS_ONE_FSTRIDE4 | TCR_KWS_LOW_LATENCY_CONV | TCR_KWS_TINY_CONV |
+                            TCR_RES2D8 | TCR_RES2D8_POOL | TCR_RES8 | TCR_RES8_NARROW | TCR_RES15 | TCR_RES15_NARROW */
   int32_t height;        /* frames, 49 */
   int32_t width;         /* coefficients, 40 (10 in the reference's DS-CNN recipes) */
   int32_t num_classes;   /* 12 */

@@ -10,7 +10,9 @@
 //   dscnn_head_kernel      global average pool + fully connected (+bias) + softmax
 // and the KWS baselines of audio_nets/kws.py on the same handle (sizes 'P' trad_fpool3, 'F' one_fstride4): kws_conv_kernel (FMA
 // first layers), kws_bsplit_kernel + kws_conv2_tc_kernel (trad_fpool3's 64 -> 64 conv on wgmma), kws_lin_kernel + kws_head_kernel
-// (the dense head); and the 2-D ablations of TC-ResNet8 ('R' ResNet2D8, 'A' ResNet2D8Pool): res2d_conv0_kernel (conv0, the pool
+// (the dense head); KWSModel's speech_commands nets ('C' low_latency_conv, 'Y' tiny_conv): kws_llconv_kernel (the T x 8 conv as an
+// FMA implicit GEMM), kws_tinyconv_kernel (10 x 8 SAME / stride 2), kws_fcs_kernel + kws_fcb_head_kernel (dense head with biases);
+// and the 2-D ablations of TC-ResNet8 ('R' ResNet2D8, 'A' ResNet2D8Pool): res2d_conv0_kernel (conv0, the pool
 // fused), res2d_block_kernel (one fused residual block), res2d_head_kernel (dscnn_head without the bias); and Honk's ResNets of
 // audio_nets/res.py ('E' Res8, 'N' Res8Narrow, 'D' Res15, 'T' Res15Narrow): res_fconv_kernel (f_conv, Res8's pool fused),
 // res_conv_kernel (one dilated 3x3 conv, its residual add and BatchNorm in the epilogue), and res2d_head_kernel.
@@ -35,7 +37,8 @@ namespace tcr {
 struct DsLayerDev {
   int type;                 // 0 conv, 1 separable, 2 (kLayerKws) VALID bias-free conv + ReLU of the KWS baselines, 3 (kLayerRes2d)
                             // a layer of the 2-D ablations (its R2Conv0 / R2Block is in the handle), 4 (kLayerRes) a layer of
-                            // Res8 / Res15 (its ResFconv / ResConv is in the handle)
+                            // Res8 / Res15 (its ResFconv / ResConv is in the handle), 5 (kLayerKwsB) the conv of low_latency_conv or
+                            // tiny_conv (its KwsLlConv / KwsTinyConv is in the handle)
   int cin, cout, kh, kw, sh, sw, hin, win, hout, wout, pt, pl;
   int64_t w, b, beta, mm, mv;                // conv / depthwise
   int64_t pw, pb, pbeta, pmm, pmv;           // pointwise (separable only)
@@ -45,6 +48,7 @@ constexpr int kDsMaxLayers = 16;      // Res15: f_conv and 13 convs (DsNet is ho
 constexpr int kLayerKws = 2;
 constexpr int kLayerRes2d = 3;
 constexpr int kLayerRes = 4;
+constexpr int kLayerKwsB = 5;
 struct DsNet {
   int nlayers, n, classes;
   DsLayerDev layer[kDsMaxLayers];
@@ -1410,6 +1414,245 @@ __global__ void __launch_bounds__(128) kws_head_kernel(KwsHead H, int n, const f
   }
 }
 
+// ---- KWSModel's speech_commands nets (audio_nets/kws.py): low_latency_conv ('C') and tiny_conv ('Y'), evaluation mode ----
+// Every layer has a bias.  low_latency_conv: T x 8 VALID conv 1 -> 186 + bias + ReLU, then fc 128, fc 128, fc classes (each + bias,
+// no nonlinearity: the training dropouts are the identity).  tiny_conv: 10 x 8 TF-SAME conv at stride 2 x 2, 1 -> 8 + bias + ReLU,
+// then fc classes + bias.  Both flatten NHWC.
+
+// low_latency_conv's conv as an implicit GEMM on the FMA pipe: rows m = (utterance, output column), M = n * wout, K = T * 8 taps,
+// N = 186 channels padded to 192.  A CTA computes kLlBM rows x 192 channels; a thread 8 rows x 12 channels.  The K loop walks one
+// filter row (8 taps) per step: its 8 x kLlBM im2col slice and 8 x 192 weights are staged in shared memory, the next step's loaded
+// into registers while the current one is multiplied.  Every output is one fmaf chain in tap order whatever tile it falls in, so
+// an utterance's bits do not depend on its batch.  WIN: utterance u is a listener window (ds_window).
+constexpr int kLlBM = 128, kLlBN = 192, kLlCout = 186, kLlThreads = 256;
+constexpr size_t kLlSmem = (size_t)2 * 8 * (kLlBM + kLlBN) * 4;
+struct KwsLlConv { int hin, win, wout, M; int64_t w, b; };
+template <bool WIN>
+__global__ void __launch_bounds__(kLlThreads, 1) kws_llconv_kernel(KwsLlConv L, const float* __restrict__ params,
+                                                                 const float* __restrict__ in, float* __restrict__ out, WindowView win) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* as = reinterpret_cast<float*>(smem_raw);                 // [2][8][kLlBM]
+  float* bs = as + 2 * 8 * kLlBM;                                 // [2][8][kLlBN]
+  const int tid = threadIdx.x, m0 = blockIdx.x * kLlBM;
+  // staging: A row am, taps aj0 .. aj0 + 3; B elements tid + 256 q of the step's [8][192] slice (channels past 186 are zeros)
+  const int am = tid & (kLlBM - 1), aj0 = (tid >> 7) * 4;
+  const int mrow = imin(m0 + am, L.M - 1), u = mrow / L.wout, col = mrow - u * L.wout;
+  const float* arow = (WIN ? ds_window(in, u, win) : in + (int64_t)u * L.hin * L.win) + col + aj0;
+  int boff[6];
+#pragma unroll
+  for (int q = 0; q < 6; ++q) {
+    const int e = tid + kLlThreads * q, j = e / kLlBN, c = e - j * kLlBN;
+    boff[q] = c < kLlCout ? j * kLlCout + c : -1;
+  }
+  float ra[4], rb[6];
+  auto load = [&](int i) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) ra[k] = arow[(int64_t)i * L.win + k];
+    const float* wr = params + L.w + (int64_t)i * 8 * kLlCout;
+#pragma unroll
+    for (int q = 0; q < 6; ++q) rb[q] = boff[q] >= 0 ? __ldg(wr + boff[q]) : 0.f;
+  };
+  auto store = [&](int buf) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) as[(buf * 8 + aj0 + k) * kLlBM + am] = ra[k];
+#pragma unroll
+    for (int q = 0; q < 6; ++q) bs[buf * 8 * kLlBN + tid + kLlThreads * q] = rb[q];
+  };
+  const int tx = tid & 15, ty = tid >> 4;                         // channels 12 tx .. 12 tx + 11, rows 8 ty .. 8 ty + 7
+  float acc[8][12];
+#pragma unroll
+  for (int r = 0; r < 8; ++r)
+#pragma unroll
+    for (int c = 0; c < 12; ++c) acc[r][c] = 0.f;
+  load(0);
+  store(0);
+  __syncthreads();
+  for (int i = 0; i < L.hin; ++i) {
+    const int cur = i & 1;
+    if (i + 1 < L.hin) load(i + 1);
+    const float* ab = as + cur * 8 * kLlBM + 8 * ty;
+    const float* bb = bs + cur * 8 * kLlBN + 12 * tx;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float4 a0 = ld4(ab + j * kLlBM), a1 = ld4(ab + j * kLlBM + 4);
+      const float4 b0 = ld4(bb + j * kLlBN), b1 = ld4(bb + j * kLlBN + 4), b2 = ld4(bb + j * kLlBN + 8);
+      const float a[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+      const float b[12] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w, b2.x, b2.y, b2.z, b2.w};
+#pragma unroll
+      for (int r = 0; r < 8; ++r)
+#pragma unroll
+        for (int c = 0; c < 12; ++c) acc[r][c] = fmaf(a[r], b[c], acc[r][c]);
+    }
+    if (i + 1 < L.hin) store(cur ^ 1);
+    __syncthreads();
+  }
+#pragma unroll
+  for (int c = 0; c < 12; ++c) {
+    const int ch = 12 * tx + c;
+    if (ch >= kLlCout) break;
+    const float bias = __ldg(params + L.b + ch);
+#pragma unroll
+    for (int r = 0; r < 8; ++r) {
+      const int m = m0 + 8 * ty + r;
+      if (m < L.M) out[(int64_t)m * kLlCout + ch] = fmaxf(acc[r][c] + bias, 0.f);
+    }
+  }
+}
+
+// tiny_conv's conv: 10 x 8, TF SAME at stride 2 x 2 (pt rows above, pl columns left: the smaller half of each total), 1 -> 8 +
+// bias + ReLU.  One CTA per (utterance, tile of RH output rows), blockIdx.x = n * tiles + tile.  The tile's 2 RH + 8 input rows
+// are staged with the padding as zeros (xw = 2 wout + 6 columns), and the taps and bias; a thread computes all 8 channels of one
+// output position.  WIN: utterance n is a listener window, padded with zeros at the window's edges like any other input: the
+// history frames before it are not read.
+struct KwsTinyConv { int hin, win, hout, wout, pt, pl, RH, xw; int64_t w, b; };
+TCR_HD inline size_t kws_tiny_smem_floats(const KwsTinyConv& L) { return 648 + (size_t)(2 * L.RH + 8) * L.xw; }
+template <bool WIN>
+__global__ void __launch_bounds__(256) kws_tinyconv_kernel(KwsTinyConv L, const float* __restrict__ params, const float* __restrict__ in,
+                                                           float* __restrict__ out, WindowView win) {
+  pdl_wait();
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* ws = reinterpret_cast<float*>(smem_raw);                 // [80 taps][8]
+  float* bs = ws + 640;                                           // [8]
+  float* xs = ws + 648;                                           // [2 RH + 8][xw]
+  const int tpu = (L.hout + L.RH - 1) / L.RH, tid = threadIdx.x;
+  const int n = blockIdx.x / tpu, h0 = (blockIdx.x - n * tpu) * L.RH, rh = imin(L.RH, L.hout - h0);
+  const float* src = WIN ? ds_window(in, n, win) : in + (int64_t)n * L.hin * L.win;
+  const int r0 = 2 * h0 - L.pt, staged = (2 * rh + 8) * L.xw;
+  for (int i = tid; i < staged; i += blockDim.x) {
+    const int r = i / L.xw, gr = r0 + r, gc = i - r * L.xw - L.pl;
+    xs[i] = gr >= 0 && gr < L.hin && gc >= 0 && gc < L.win ? src[(int64_t)gr * L.win + gc] : 0.f;
+  }
+  for (int i = tid; i < 648; i += blockDim.x) ws[i] = __ldg(params + (i < 640 ? L.w + i : L.b + i - 640));
+  __syncthreads();
+  for (int p = tid; p < rh * L.wout; p += blockDim.x) {
+    const int r = p / L.wout, q = p - r * L.wout;
+    const float* x = xs + 2 * r * L.xw + 2 * q;
+    float acc[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) acc[c] = 0.f;
+    for (int i = 0; i < 10; ++i)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float v = x[i * L.xw + j];
+        const float4 w0 = ld4(ws + (i * 8 + j) * 8), w1 = ld4(ws + (i * 8 + j) * 8 + 4);
+        acc[0] = fmaf(v, w0.x, acc[0]); acc[1] = fmaf(v, w0.y, acc[1]); acc[2] = fmaf(v, w0.z, acc[2]); acc[3] = fmaf(v, w0.w, acc[3]);
+        acc[4] = fmaf(v, w1.x, acc[4]); acc[5] = fmaf(v, w1.y, acc[5]); acc[6] = fmaf(v, w1.z, acc[6]); acc[7] = fmaf(v, w1.w, acc[7]);
+      }
+    float* o = out + (((int64_t)n * L.hout + h0 + r) * L.wout + q) * 8;
+    st4(o, make_float4(fmaxf(acc[0] + bs[0], 0.f), fmaxf(acc[1] + bs[1], 0.f), fmaxf(acc[2] + bs[2], 0.f), fmaxf(acc[3] + bs[3], 0.f)));
+    st4(o + 4, make_float4(fmaxf(acc[4] + bs[4], 0.f), fmaxf(acc[5] + bs[5], 0.f), fmaxf(acc[6] + bs[6], 0.f), fmaxf(acc[7] + bs[7], 0.f)));
+  }
+}
+
+// Their dense heads.  The first matmul (K = the flattened conv output) is split over K: CTA (utterance group, K chunk s) stages KC
+// rows of the weights ([K, N], N <= 32 NQ columns, zero-padded) once for 64 utterances and writes partial sums part[s][u][32 NQ].
+// kws_fcb_head_kernel adds the chunks in order and the bias, applies the remaining matrices (+ bias) one at a time, and the
+// softmax, so the logits of an utterance do not depend on the batch it is in.  low_latency_conv: first_fc (N = 128, NQ = 4), then
+// second_fc and final_fc in the head kernel; tiny_conv: final_fc is the split matmul (N = classes, NQ = 1).
+struct KwsFcb { int K, N0, nsplit, nmid, classes; int64_t w0, b0, mid, midb, out, outb; };
+template <int NQ, int KC>
+constexpr size_t kws_fcs_smem() { return (size_t)(KC * 32 * NQ + 64 * (KC + 1)) * 4; }
+template <int NQ, int KC>
+__global__ void __launch_bounds__(256) kws_fcs_kernel(KwsFcb H, int n, const float* __restrict__ params, const float* __restrict__ in,
+                                                      float* __restrict__ part) {
+  pdl_wait();
+  constexpr int NP = 32 * NQ;
+  TCR_DYNAMIC_SMEM(smem_raw);
+  float* ws = reinterpret_cast<float*>(smem_raw);                 // [KC][NP]
+  float* xs = ws + KC * NP;                                       // [64][KC + 1]
+  const int s = blockIdx.x % H.nsplit, u0 = (blockIdx.x / H.nsplit) * 64, tid = threadIdx.x;
+  const int k0 = s * KC, kc = imin(KC, H.K - k0), nu = imin(64, n - u0);
+  for (int i = tid; i < kc * NP; i += blockDim.x) {
+    const int k = i / NP, c = i - k * NP;
+    ws[i] = c < H.N0 ? __ldg(params + H.w0 + (int64_t)(k0 + k) * H.N0 + c) : 0.f;
+  }
+  for (int i = tid; i < nu * kc; i += blockDim.x) {
+    const int u = i / kc, k = i - u * kc;
+    xs[u * (KC + 1) + k] = in[(int64_t)(u0 + u) * H.K + k0 + k];
+  }
+  __syncthreads();
+  const int lane = tid & 31, warp = tid >> 5;                     // columns lane + 32 q, utterances warp + 8 i
+  float acc[8][NQ];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) acc[i][q] = 0.f;
+  for (int k = 0; k < kc; ++k) {
+    float w[NQ];
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) w[q] = ws[k * NP + lane + 32 * q];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float x = xs[(warp + 8 * i) * (KC + 1) + k];
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) acc[i][q] = fmaf(x, w[q], acc[i][q]);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+    if (warp + 8 * i < nu)
+#pragma unroll
+      for (int q = 0; q < NQ; ++q) part[((int64_t)s * n + u0 + warp + 8 * i) * NP + lane + 32 * q] = acc[i][q];
+}
+
+// kKwsHeadU utterances per CTA of 128 threads; the partial sums' row stride is N0 rounded up to 32.
+__global__ void __launch_bounds__(128) kws_fcb_head_kernel(KwsFcb H, int n, const float* __restrict__ params, const float* __restrict__ part,
+                                                           float* __restrict__ logits, float* __restrict__ probs) {
+  pdl_wait();
+  __shared__ float h[2][kKwsHeadU][128];
+  __shared__ float s_logit[kKwsHeadU][kMaxClasses];
+  const int u0 = blockIdx.x * kKwsHeadU, nu = imin(kKwsHeadU, n - u0), tid = threadIdx.x, C = H.classes;
+  const int NP = (H.N0 + 31) & ~31;
+  for (int i = tid; i < kKwsHeadU * H.N0; i += blockDim.x) {
+    const int u = i / H.N0, j = i - u * H.N0;
+    float a = 0.f;
+    if (u < nu) {
+      for (int s = 0; s < H.nsplit; ++s) a += part[((int64_t)s * n + u0 + u) * NP + j];
+      a += __ldg(params + H.b0 + j);
+    }
+    h[0][u][j] = a;
+  }
+  __syncthreads();
+  int cur = 0;
+  for (int m = 0; m < H.nmid; ++m, cur ^= 1) {                    // 128 -> 128 (+ bias)
+    const float* W = params + H.mid;
+    float acc[kKwsHeadU];
+#pragma unroll
+    for (int u = 0; u < kKwsHeadU; ++u) acc[u] = 0.f;
+    for (int k = 0; k < 128; ++k) {
+      const float w = __ldg(W + k * 128 + tid);
+#pragma unroll
+      for (int u = 0; u < kKwsHeadU; ++u) acc[u] = fmaf(h[cur][u][k], w, acc[u]);
+    }
+    const float b = __ldg(params + H.midb + tid);
+#pragma unroll
+    for (int u = 0; u < kKwsHeadU; ++u) h[cur ^ 1][u][tid] = acc[u] + b;
+    __syncthreads();
+  }
+  for (int i = tid; i < nu * C; i += blockDim.x) {
+    const int u = i / C, c = i - u * C;
+    float a = h[cur][u][c];                                       // tiny_conv: the split matmul's output are the logits
+    if (H.out >= 0) {
+      a = 0.f;
+      for (int k = 0; k < 128; ++k) a = fmaf(h[cur][u][k], __ldg(params + H.out + k * C + c), a);
+      a += __ldg(params + H.outb + c);
+    }
+    s_logit[u][c] = a;
+    if (logits) logits[(int64_t)(u0 + u) * C + c] = a;
+  }
+  __syncthreads();
+  if (!probs) return;
+  for (int i = tid; i < nu * C; i += blockDim.x) {
+    const int u = i / C, c = i - u * C;
+    float mx = -3.0e38f;
+    for (int k = 0; k < C; ++k) mx = fmaxf(mx, s_logit[u][k]);
+    float se = 0.f;
+    for (int k = 0; k < C; ++k) se += expf(s_logit[u][k] - mx);
+    probs[(int64_t)(u0 + u) * C + c] = expf(s_logit[u][c] - mx) / se;
+  }
+}
+
 // ---- ResNet2D8 / ResNet2D8Pool: the paper's 2-D ablations of TC-ResNet8 (audio_nets/tc_resnet.py:6-54, 73-101, debug_2d) ----
 // Evaluation mode.  No conv has a bias, and BatchNorm has gamma (TCResNet_arg_scope: center and scale):
 // (beta, gamma, moving mean, moving variance) fold into scale = gamma / sqrt(var + eps) and shift = beta - mean * scale.
@@ -1951,6 +2194,11 @@ struct tcr_dscnn {
   ResFconv rfconv = {};
   ResConv rconv[13] = {};
   int64_t rfc = 0;
+  // low_latency_conv / tiny_conv ('C', 'Y'): the conv's plan and the dense head (its partial sums in `part`)
+  bool kwsb = false;
+  KwsLlConv llconv = {};
+  KwsTinyConv tiny = {};
+  KwsFcb fcb = {};
 };
 
 #ifndef TCR_EMU
@@ -2154,16 +2402,88 @@ static int res_define(tcr_dscnn* d, Add& add) {
   return TCR_OK;
 }
 
+// low_latency_conv / tiny_conv as audio_nets/kws.py builds them (create_low_latency_conv_model 293-405, create_tiny_conv_model
+// 681-757): top-level TF variables in creation order, each weight followed by its bias.  FLOPs count tiny_conv's full 80-tap kernel
+// at every output, padding included.  Also each kernel's plan, and the refusals of what the kernels cannot run.
+template <class Add>
+static int kwsb_define(tcr_dscnn* d, Add& add) {
+  const tcr_dscnn_config& c = d->cfg;
+  const bool ll = c.size == TCR_KWS_LOW_LATENCY_CONV;
+  const size_t kSmemLimit = 227 * 1024;                            // sm_90's opt-in shared memory per block
+  const int64_t kIntMax = 2147483647;
+  DsLayerDev L;
+  memset(&L, 0, sizeof(L));
+  L.type = kLayerKwsB; L.cin = 1; L.hin = c.height; L.win = c.width;
+  KwsFcb& H = d->fcb;
+  H = {};
+  H.classes = c.num_classes;
+  H.out = H.outb = -1;
+  int64_t K;
+  if (ll) {
+    if (c.width < 8) return ds_fail(TCR_ERR_UNSUPPORTED, "low_latency_conv needs width >= 8 (its T x 8 conv is VALID), got %d", c.width);
+    L.cout = kLlCout; L.kh = c.height; L.kw = 8; L.sh = L.sw = 1; L.hout = 1; L.wout = c.width - 7;
+    if ((int64_t)c.max_batch * L.wout > kIntMax)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "kws_llconv: max_batch %d x %d output columns exceeds the %lld GEMM rows it indexes",
+                     c.max_batch, L.wout, (long long)kIntMax);
+    K = (int64_t)L.wout * kLlCout;
+  } else {
+    L.cout = 8; L.kh = 10; L.kw = 8; L.sh = L.sw = 2;
+    ds_same(c.height, 10, 2, &L.hout, &L.pt);
+    ds_same(c.width, 8, 2, &L.wout, &L.pl);
+    KwsTinyConv& T = d->tiny;
+    T = {c.height, c.width, L.hout, L.wout, L.pt, L.pl, std::min(L.hout, 8), 2 * L.wout + 6, 0, 0};
+    if (kws_tiny_smem_floats(T) * 4 > kSmemLimit)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "kws_tinyconv needs %zu bytes of shared memory at width %d, the limit is %zu",
+                     kws_tiny_smem_floats(T) * 4, c.width, kSmemLimit);
+    if ((int64_t)c.max_batch * ((T.hout + T.RH - 1) / T.RH) > kIntMax)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "kws_tinyconv: max_batch %d x %d row tiles exceeds the grid's %lld CTAs", c.max_batch,
+                     (T.hout + T.RH - 1) / T.RH, (long long)kIntMax);
+    K = (int64_t)L.hout * L.wout * 8;
+  }
+  const int KC = ll ? 128 : 256;                                   // kws_fcs_kernel's K chunk
+  if (K > kIntMax || (K + KC - 1) / KC * ((c.max_batch + 63) / 64) > kIntMax)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "kws_fcs: K = %lld flattened values in chunks of %d for max_batch %d exceeds the grid's %lld CTAs",
+                   (long long)K, KC, c.max_batch, (long long)kIntMax);
+  H.K = (int)K;
+  H.nsplit = (H.K + KC - 1) / KC;
+  L.w = add("first_weights", TCR_KIND_WEIGHT, {L.kh, 8, 1, L.cout});
+  L.b = add("first_bias", TCR_KIND_BETA, {L.cout});
+  d->flops += 2ll * L.hout * L.wout * L.kh * 8 * L.cout;
+  if (ll) {
+    d->llconv = {c.height, c.width, L.wout, 0, L.w, L.b};
+    H.N0 = 128;
+    H.nmid = 1;
+    H.w0 = add("first_fc_weights", TCR_KIND_WEIGHT, {H.K, 128});
+    H.b0 = add("first_fc_bias", TCR_KIND_BETA, {128});
+    H.mid = add("second_fc_weights", TCR_KIND_WEIGHT, {128, 128});
+    H.midb = add("second_fc_bias", TCR_KIND_BETA, {128});
+    H.out = add("final_fc_weights", TCR_KIND_WEIGHT, {128, c.num_classes});
+    H.outb = add("final_fc_bias", TCR_KIND_BETA, {c.num_classes});
+    d->flops += 2ll * H.K * 128 + 2ll * 128 * 128 + 2ll * 128 * c.num_classes;
+  } else {
+    d->tiny.w = L.w;
+    d->tiny.b = L.b;
+    H.N0 = c.num_classes;
+    H.w0 = add("final_fc_weights", TCR_KIND_WEIGHT, {H.K, c.num_classes});
+    H.b0 = add("final_fc_bias", TCR_KIND_BETA, {c.num_classes});
+    d->flops += 2ll * H.K * c.num_classes;
+  }
+  d->net.layer[d->net.nlayers++] = L;
+  d->act_floats = (size_t)L.hout * L.wout * L.cout;
+  return TCR_OK;
+}
+
 extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   if (!cfg || !out) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   *out = nullptr;
   const bool kws = cfg->size == TCR_KWS_TRAD_FPOOL3 || cfg->size == TCR_KWS_ONE_FSTRIDE4;
   const bool res2d = cfg->size == TCR_RES2D8 || cfg->size == TCR_RES2D8_POOL;
   const bool res = cfg->size == TCR_RES8 || cfg->size == TCR_RES8_NARROW || cfg->size == TCR_RES15 || cfg->size == TCR_RES15_NARROW;
-  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws && !res2d && !res) {
-    set_error("DS-CNN size must be 'S', 'M' or 'L', or a KWS baseline: 'P' (trad_fpool3) or 'F' (one_fstride4), or a 2-D ablation: "
-              "'R' (ResNet2D8) or 'A' (ResNet2D8Pool), or a Honk ResNet: 'E' (Res8), 'N' (Res8Narrow), 'D' (Res15) or 'T' "
-              "(Res15Narrow)");
+  const bool kwsb = cfg->size == TCR_KWS_LOW_LATENCY_CONV || cfg->size == TCR_KWS_TINY_CONV;
+  if (cfg->size != 'S' && cfg->size != 'M' && cfg->size != 'L' && !kws && !res2d && !res && !kwsb) {
+    set_error("DS-CNN size must be 'S', 'M' or 'L', or a KWS baseline: 'P' (trad_fpool3) or 'F' (one_fstride4), or 'C' "
+              "(low_latency_conv) or 'Y' (tiny_conv), or a 2-D ablation: 'R' (ResNet2D8) or 'A' (ResNet2D8Pool), or a Honk ResNet: "
+              "'E' (Res8), 'N' (Res8Narrow), 'D' (Res15) or 'T' (Res15Narrow)");
     return TCR_ERR_INVALID;
   }
   if (!res2d && cfg->width_multiplier != 0.0)
@@ -2199,6 +2519,7 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   d->kws = kws;
   d->res2d = res2d;
   d->res = res;
+  d->kwsb = kwsb;
   if (const char* e = getenv("TCR_DSCNN_TC")) { d->use_tc = e[0] != '0'; d->tc_ws = e[0] != '1'; }
   struct Def { int type, depth, kh, kw, sh, sw; const char* scope; };
   std::vector<Def> defs;
@@ -2276,6 +2597,11 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     if (rc != TCR_OK) { delete d; return rc; }
     defs.clear();
   }
+  if (kwsb) {
+    const int rc = kwsb_define(d, add);
+    if (rc != TCR_OK) { delete d; return rc; }
+    defs.clear();
+  }
   for (const Def& df : defs) {
     DsLayerDev L;
     memset(&L, 0, sizeof(L));
@@ -2309,7 +2635,7 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     h = L.hout; w = L.wout; cin = df.depth;
   }
   d->net.classes = cfg->num_classes;
-  if (!kws && !res2d && !res) {
+  if (!kws && !res2d && !res && !kwsb) {
     d->net.fcw = add("DSCNN/fc1/weights", TCR_KIND_WEIGHT, {cin, cfg->num_classes});
     d->net.fcb = add("DSCNN/fc1/biases", TCR_KIND_BETA, {cfg->num_classes});
     d->flops += 2ll * cin * cfg->num_classes;
@@ -2334,6 +2660,12 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
       set_error("cudaMalloc failed for the KWS head / filter buffers");
       return TCR_ERR_CUDA;
     }
+  }
+  if (kwsb && cudaMalloc((void**)&d->part, (size_t)d->fcb.nsplit * cfg->max_batch * ((d->fcb.N0 + 31) & ~31) * sizeof(float)) !=
+                  cudaSuccess) {
+    tcr_dscnn_destroy(d);
+    set_error("cudaMalloc failed for the KWS head's partial sums");
+    return TCR_ERR_CUDA;
   }
   *out = d;
   return TCR_OK;
@@ -2471,6 +2803,49 @@ static int kws_head(tcr_dscnn* d, const float* params, const float* in, int n, f
   return TCR_OK;
 }
 
+// The conv of low_latency_conv (kws_llconv_kernel) or tiny_conv (kws_tinyconv_kernel); the emulator build runs the same kernels.
+template <bool WIN>
+static int kwsb_launch_conv(tcr_dscnn* d, const float* params, const float* in, float* out, int32_t n, cudaStream_t s, WindowView win) {
+  if (d->cfg.size == TCR_KWS_LOW_LATENCY_CONV) {
+    KwsLlConv L = d->llconv;
+    L.M = n * L.wout;
+    auto kfn = kws_llconv_kernel<WIN>;
+    TCR_LAUNCH(WIN ? "kws_llconv:win" : "kws_llconv", kfn, dim3((L.M + kLlBM - 1) / kLlBM), dim3(kLlThreads), kLlSmem, s, L, params,
+               in, out, win);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_llconv launch failed");
+    return TCR_OK;
+  }
+  const KwsTinyConv& L = d->tiny;
+  const size_t smem = kws_tiny_smem_floats(L) * 4;
+  auto kfn = kws_tinyconv_kernel<WIN>;
+#ifndef TCR_EMU
+  static SmemOptIn optin;
+  if (optin.ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_tinyconv: shared memory opt-in failed");
+#endif
+  const unsigned grid = (unsigned)((int64_t)n * ((L.hout + L.RH - 1) / L.RH));
+  TCR_LAUNCH(WIN ? "kws_tinyconv:win" : "kws_tinyconv", kfn, dim3(grid), dim3(256), smem, s, L, params, in, out, win);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_tinyconv launch failed");
+  return TCR_OK;
+}
+
+// flatten -> the first matmul split over K (kws_fcs: 128 columns for low_latency_conv, the classes for tiny_conv) -> the chunks
+// summed in order, the biases, the remaining matrices, logits, softmax (kws_fcb_head)
+static int kwsb_head(tcr_dscnn* d, const float* params, const float* in, int n, float* logits, float* probs, cudaStream_t s) {
+  const KwsFcb& H = d->fcb;
+  const bool ll = d->cfg.size == TCR_KWS_LOW_LATENCY_CONV;
+  auto kfn = ll ? kws_fcs_kernel<4, 128> : kws_fcs_kernel<1, 256>;
+  const size_t smem = ll ? kws_fcs_smem<4, 128>() : kws_fcs_smem<1, 256>();
+#ifndef TCR_EMU
+  static SmemOptIn optin4, optin1;
+  if ((ll ? optin4 : optin1).ensure(kfn, smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "kws_fcs: shared memory opt-in failed");
+#endif
+  TCR_LAUNCH("kws_fcs", kfn, dim3(H.nsplit * ((n + 63) / 64)), dim3(256), smem, s, H, n, params, in, d->part);
+  TCR_LAUNCH("kws_fcb_head", kws_fcb_head_kernel, dim3((n + kKwsHeadU - 1) / kKwsHeadU), dim3(128), 0, s, H, n, params, d->part, logits,
+             probs);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "KWS head launch failed");
+  return TCR_OK;
+}
+
 // A layer of the 2-D ablations: 0 is conv0 (+ pool) on res2d_conv0_kernel, 1-3 the residual blocks on res2d_block_kernel.
 template <bool WIN>
 static int res2d_launch(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s, WindowView win) {
@@ -2566,6 +2941,10 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
     if (win) return res_launch<true>(d, l, params, in, out, n, s, *win);
     return res_launch<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
   }
+  if (L.type == kLayerKwsB) {
+    if (win) return kwsb_launch_conv<true>(d, params, in, out, n, s, *win);
+    return kwsb_launch_conv<false>(d, params, in, out, n, s, WindowView{0, 0, 0});
+  }
   if (L.type == 0) {
     if (win) return ds_launch_conv<true>(d, L, params, in, out, n, s, *win);
     return ds_launch_conv<false>(d, L, params, in, out, n, s, WindowView{0, 0, 0});
@@ -2635,6 +3014,7 @@ int tcr::dscnn_forward(tcr_dscnn* d, const float* feat, const float* params, int
     in = out;
   }
   if (d->kws) return kws_head(d, params, in, n, logits, probs, s);
+  if (d->kwsb) return kwsb_head(d, params, in, n, logits, probs, s);
   const DsLayerDev& last = d->net.layer[d->net.nlayers - 1];
   if (d->res2d || d->res) {
     TCR_LAUNCH("res2d_head", res2d_head_kernel, dim3(n), dim3(256), 0, s, last.hout * last.wout, last.cout, d->net.classes,

@@ -1,6 +1,7 @@
 """DS-CNN forward (inference) on the CUDA path: the reference's 2-D-conv comparison model
 (audio_nets/ds_cnn.py; DSCNN{S,M,L}Model.build_inference in factory/audio_nets.py:298-358), and on the same handle the KWS
-baselines cnn-trad-fpool3 (size 'P') and cnn-one-fstride4 ('F') of audio_nets/kws.py, and the paper's 2-D ablations of TC-ResNet8,
+baselines cnn-trad-fpool3 (size 'P') and cnn-one-fstride4 ('F') of audio_nets/kws.py and its speech_commands nets low_latency_conv
+('C') and tiny_conv ('Y'), and the paper's 2-D ablations of TC-ResNet8,
 ResNet2D8 ('R') and ResNet2D8Pool ('A') of audio_nets/tc_resnet.py, and Honk's ResNets of audio_nets/res.py, Res8 ('E'), Res8Narrow
 ('N'), Res15 ('D') and Res15Narrow ('T'), with their dilated 3x3 convolutions.  Training DS-CNN is out of scope
 (SURVEY.md 2 #13): weights come from a checkpoint keyed by the TF variable names in `self.table`.
@@ -19,7 +20,7 @@ from . import _lib as L
 from .engine import Listener, frontend_config, frontend_shape
 
 # tcr_dscnn_config.size of the KWS baselines (include/tcr_b200.h): KWSModel --architecture -> size code
-KWS_SIZES = {"trad_fpool3": "P", "one_fstride4": "F"}
+KWS_SIZES = {"trad_fpool3": "P", "one_fstride4": "F", "low_latency_conv": "C", "tiny_conv": "Y"}
 # and of the 2-D ablations, by TF scope; they alone take a width multiplier
 RES2D_SIZES = {"ResNet2D8": "R", "ResNet2D8Pool": "A"}
 # and of Honk's ResNets, by model name (all four under the TF scope "Res")
@@ -91,8 +92,8 @@ class DsCnn:
 
     def new_variables(self, seed: int = 0) -> torch.Tensor:
         """Flat variables as the reference initialises them before a restore: Xavier-uniform weights (slim's default), zero biases /
-        beta / moving mean, unit moving variance, unit gamma (the 2-D ablations' BatchNorm); the KWS baselines ('P', 'F') draw every weight from
-        truncated_normal(stddev=0.01) (audio_nets/kws.py), values past two sigma redrawn.  Host-side RNG, not TF's."""
+        beta / moving mean, unit moving variance, unit gamma (the 2-D ablations' BatchNorm); the KWS nets (KWS_SIZES) draw every weight from
+        truncated_normal(stddev=0.01) (audio_nets/kws.py), values past two sigma redrawn, and zero biases.  Host-side RNG, not TF's."""
         rng = np.random.default_rng(seed)
         flat = np.zeros(self.num_params, np.float32)
         for d in self.table:

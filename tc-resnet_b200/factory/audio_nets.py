@@ -4,7 +4,7 @@ executing on the CUDA engine instead of building a TF graph.
 `train_audio.py` / `evaluate_audio.py` look the class up by NAME (`eval(f"audio_nets.{args.model}")`,
 train_audio.py:32), call `Model(args, dataset)`, then `model.build(wavs, labels, is_training)` and hand the model
 to the trainer / evaluator, which touch only the attributes set here and `session.run`.  TCResNet8Model and
-TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model, KWSModel (--architecture trad_fpool3 / one_fstride4),
+TCResNet14Model are on the accelerated path; DSCNN{S,M,L}Model, KWSModel (--architecture trad_fpool3 / one_fstride4 / low_latency_conv / tiny_conv),
 ResNet2D8Model, ResNet2D8PoolModel and Res{8,8Narrow,15,15Narrow}Model are on it for evaluation, deployment and streaming (their
 training is out of scope and raises NotImplementedError).
 """
@@ -679,16 +679,17 @@ class DSCNNLModel(DsCnnModel):
     dscnn_size = "L"
 
 
-# KWSModel --architecture choices (factory/audio_nets.py:222-224); KWS_SIZES names the two on the CUDA path
+# KWSModel --architecture choices (factory/audio_nets.py:222-224); KWS_SIZES names the four on the CUDA path
 KWS_ARCHITECTURES = ["single_fc", "conv", "low_latency_conv", "low_latency_svdf", "tiny_conv", "one_fstride4", "trad_fpool3"]
 
 
 class KWSModel(DsCnnModel):
     """KWSModel (factory/audio_nets.py:205-224, audio_nets/kws.py) for --architecture trad_fpool3 and one_fstride4, the two Sainath &
-    Parada CNNs of the reference's recipes, in evaluation mode on the DS-CNN handle (size codes 'P' / 'F', dscnn.KWS_SIZES).  The
-    variables are top-level TF names ("first_weights", ...).  --weight_decay keeps TFModel's default of 1e-4, and total_loss adds
-    the reference's L2 term over every weight (build_loss: weight_decay * sum(tf.nn.l2_loss(w))).  The other five architectures and
-    training are out of scope."""
+    Parada CNNs of the reference's recipes, and low_latency_conv and tiny_conv, two of TensorFlow's speech_commands nets, in
+    evaluation mode on the DS-CNN handle (size codes 'P' / 'F' / 'C' / 'Y', dscnn.KWS_SIZES).  The variables are top-level TF names
+    ("first_weights", "first_bias", ...).  --weight_decay keeps TFModel's default of 1e-4, and total_loss adds the reference's L2
+    term over every variable, biases included (build_loss: weight_decay * sum(tf.nn.l2_loss(v))).  single_fc, conv and
+    low_latency_svdf, and training, are out of scope."""
 
     @staticmethod
     def add_arguments(parser):
