@@ -787,8 +787,9 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
       cudaStream_t f = (cudaStream_t)h->fe_stream;
       if (input_event) TCR_CUDA(cudaStreamWaitEvent(f, (cudaEvent_t)input_event, 0));
       if (h->fe_count > 2) TCR_CUDA(cudaStreamWaitEvent(f, (cudaEvent_t)h->fe_free[fe_buf], 0));   // the step two calls back has read it
-      // not before the previous step's weight gradients are launched-and-done: the front-end then shares the GPU with the small,
-      // latency-bound tail kernels (grad_finalize, update and its cross-GPU arrival wait) instead of time-slicing with the FMA-bound ones
+      // not before the previous step's backward-data pass is done: the front-end's persistent CTAs then take the SMs the weight-gradient
+      // chunks free and run beside grad_finalize / update, instead of starting only when the weight gradients are done and leaving the
+      // next forward waiting for the front-end alone (TCResNet8-1.0, N = 512 on an H100: 0.320 ms per step instead of 0.330)
       if (h->fe_gate_valid) TCR_CUDA(cudaStreamWaitEvent(f, (cudaEvent_t)h->fe_gate, 0));
       fs = (tcr_stream)f;
       featbuf = h->fe_feat[fe_buf];
@@ -838,14 +839,14 @@ static int train_step_impl(tcr_handle* h, const tcr_step_args* a, tcr_stream str
   rc = resident == kResidentFwdBwdData && h->bwd_phases > 0 ? resident_backward_data(h, feat, a, s)
                                                             : net_backward_data(h, a->params, a->n, s);
   if (rc) return fail_wrap(rc, "backward launch failed");
-  rc = net_weight_gradients(h, feat, a->n, s);
-  if (rc) return fail_wrap(rc, "weight-gradient launch failed");
 #ifndef TCR_EMU
   if (h->fe_gate) {                   // the gate of the NEXT step's front-end (see above)
     TCR_CUDA(cudaEventRecord((cudaEvent_t)h->fe_gate, s));
     h->fe_gate_valid = 1;
   }
 #endif
+  rc = net_weight_gradients(h, feat, a->n, s);
+  if (rc) return fail_wrap(rc, "weight-gradient launch failed");
   rc = net_update(h, a, s);
   if (rc) return fail_wrap(rc, "update launch failed");
   TCR_CUDA(cudaGetLastError());

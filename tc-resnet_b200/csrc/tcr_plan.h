@@ -63,8 +63,8 @@ struct tcr_handle {
   float* fe_aug = nullptr;           // the ahead path's own decoded-wav buffer (device input stage)
   float* fe_hot[2] = {nullptr, nullptr};   // one-hot labels of a resident-dataset step, one per feature buffer of the ahead path
   float* d_hot = nullptr;            // the same for a resident-dataset step ordered on the caller's stream
-  void* fe_gate = nullptr; int fe_gate_valid = 0;   // recorded on the step's stream once the weight gradients are launched: the next
-                                     // step's front-end starts behind it, i.e. next to grad_finalize / update, not next to the FMA-bound kernels
+  void* fe_gate = nullptr; int fe_gate_valid = 0;   // recorded on the step's stream once the backward-data pass is launched: the next
+                                     // step's front-end starts behind it, next to the weight-gradient launch and grad_finalize / update
   float* feat_last = nullptr;
   int sync_bn = 0;                   // BatchNorm statistics over the global batch (per-layer kernels + NCCL; tcr_comm_set_sync_bn)        // feature buffer the library filled last ("features" of tcr_workspace_tensor)
   float* d_logits = nullptr; float* d_probs = nullptr;
