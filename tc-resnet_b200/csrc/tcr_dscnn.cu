@@ -2162,9 +2162,16 @@ __global__ void __launch_bounds__(kResConvThreads) res_conv_kernel(ResConv L, in
 // ------------------------------------------------------------------------------------------------
 using namespace tcr;
 
+// How a layer of DS-CNN S / M / L runs, worked out once by ds_plan_layer in tcr_dscnn_create: the kernel, its tile rows (RHt of the
+// wgmma kernels, RH of dscnn_dsblock; 0 for dscnn_conv, which stages a whole utterance), dscnn_dsblock's output-channel slice COT,
+// and the dynamic shared memory of the launch.
+enum DsKernel { kDsConv, kDsConvTc, kDsConvWs, kDsBlock, kDsBlockTc, kDsBlockWs };
+struct DsPlan { int kernel, RH, COT; size_t smem; };
+
 struct tcr_dscnn {
   tcr_dscnn_config cfg;
   DsNet net;
+  DsPlan plan[kDsMaxLayers] = {};   // DS-CNN S / M / L: each layer's kernel, tile and shared memory
   std::vector<tcr_param_desc> table;
   int64_t n_params = 0, flops = 0;
   float* act[2] = {nullptr, nullptr};
@@ -2473,6 +2480,72 @@ static int kwsb_define(tcr_dscnn* d, Add& add) {
   return TCR_OK;
 }
 
+// Tile rows of the wgmma kernels: at most 128 accumulator rows (RH * wout) per tile, balanced (25 rows -> 5 tiles of 5).
+static int ds_tile_rows(const DsLayerDev& L) {
+  const int cap = std::max(1, std::min(L.hout, 128 / std::max(1, std::min(L.wout, 128))));
+  const int tiles = (L.hout + cap - 1) / cap;
+  return (L.hout + tiles - 1) / tiles;
+}
+
+// The plan of layer l of DS-CNN S / M / L (d->plan[l]), and the refusal of a layer no kernel can run.  wgmma where the layer's shape
+// fits the tensor-core kernels (use_tc, TCR_DSCNN_TC; never in the emulator build, which has no wgmma), the register-tiled FMA
+// kernels otherwise.  dscnn_conv stages a whole utterance, so its bytes grow with height x width, up to sm_90's 227 KB opt-in;
+// dscnn_dsblock shrinks its output-channel slice, then its tile of rows, and stops at 200 KB.  The plan depends on the geometry
+// alone, so an utterance's bits do not depend on n.
+static int ds_plan_layer(tcr_dscnn* d, int l, const char* scope) {
+  const DsLayerDev& L = d->net.layer[l];
+  DsPlan& P = d->plan[l];
+  if (L.type == 0) {
+#ifndef TCR_EMU
+    const int RHt = ds_tile_rows(L);
+    // implicit GEMM on wgmma (3xTF32), where the kernel's per-thread im2col walk covers the tile
+    if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && im2col_walk_fits(L, RHt, kTcThreads)) {
+      const size_t smem_ws = conv_tc_smem<64>(L, RHt, 2).floats * 4;
+      if (d->tc_ws && smem_ws <= 220 * 1024 && im2col_walk_fits(L, RHt, kWsProducers) && (L.kh * L.kw / 4) % 2 == 0)
+        P = {kDsConvWs, RHt, 0, smem_ws};
+      else
+        P = {kDsConvTc, RHt, 0, conv_tc_smem<64>(L, RHt, 1).floats * 4};
+      return TCR_OK;
+    }
+#endif
+    const size_t kSmemLimit = 227 * 1024;                          // sm_90's opt-in shared memory per block
+    P = {kDsConv, 0, 0, conv_smem(L).floats * 4};
+    if (P.smem > kSmemLimit)
+      return ds_fail(TCR_ERR_UNSUPPORTED, "dscnn_conv (%s) needs %zu bytes of shared memory at %d x %d, the limit is %zu", scope, P.smem,
+                     d->cfg.height, d->cfg.width, kSmemLimit);
+    return TCR_OK;
+  }
+  // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage.  The
+  // warp-specialised kernel where its input tile and producers fit, the lock-step kernel where its fetch walk does.
+#ifndef TCR_EMU
+  if (d->use_tc && L.cin == 64 && L.cout == 64 && L.kh == 3 && L.kw == 3 && L.sh == 1 && L.sw == 1 && L.wout <= 64) {
+    const int RHt = ds_tile_rows(L);
+    const size_t smem_ws = dsblock_ws_smem<64, 64>(L, RHt).floats * 4;
+    if (d->tc_ws && smem_ws <= 226 * 1024 && L.cin / 4 * L.wout <= kWsProducers && L.wout + 2 <= 256 && RHt + 2 <= 256) {
+      P = {kDsBlockWs, RHt, 0, smem_ws};
+      return TCR_OK;
+    }
+    const size_t smem_tc = dsblock_tc_smem<64, 64>(L, RHt).floats * 4;
+    if (smem_tc <= 200 * 1024 && (RHt + 2) * (L.wout + 2) <= kDwCells * (kTcThreads / (L.cin / 4))) {
+      P = {kDsBlockTc, RHt, 0, smem_tc};
+      return TCR_OK;
+    }
+  }
+#endif
+  // the whole pointwise bank in shared memory when it fits next to a useful tile; else (DS-CNN-L: 276 x 276 fp32 = 305 KB) output-
+  // channel tiles of COT, the depthwise output of the tile being reused for every slice
+  int COT = L.cout;
+  while (COT > 32 && dsblock_smem(L, 1, COT).floats * 4 > 96 * 1024) COT = ((COT / 2) + 3) & ~3;
+  int RH = std::min(L.hout, 8);
+  while (RH > 1 && dsblock_smem(L, RH, COT).floats * 4 > 100 * 1024) --RH;
+  const size_t kBlockLimit = 200 * 1024;
+  P = {kDsBlock, RH, COT, dsblock_smem(L, RH, COT).floats * 4};
+  if (P.smem > kBlockLimit)
+    return ds_fail(TCR_ERR_UNSUPPORTED, "dscnn_dsblock (%s) needs %zu bytes of shared memory at %d x %d, the limit is %zu", scope, P.smem,
+                   d->cfg.height, d->cfg.width, kBlockLimit);
+  return TCR_OK;
+}
+
 extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
   if (!cfg || !out) { set_error("NULL argument"); return TCR_ERR_INVALID; }
   *out = nullptr;
@@ -2631,6 +2704,8 @@ extern "C" int tcr_dscnn_create(const tcr_dscnn_config* cfg, tcr_dscnn** out) {
     }
     if (df.depth % 4) { delete d; set_error("DS-CNN depth must be a multiple of 4"); return TCR_ERR_UNSUPPORTED; }
     d->net.layer[d->net.nlayers++] = L;
+    const int rc = ds_plan_layer(d, d->net.nlayers - 1, df.scope);
+    if (rc != TCR_OK) { delete d; return rc; }
     d->act_floats = std::max(d->act_floats, (size_t)L.hout * L.wout * df.depth);
     h = L.hout; w = L.wout; cin = df.depth;
   }
@@ -2693,47 +2768,42 @@ extern "C" int tcr_dscnn_param_table(const tcr_dscnn* d, const tcr_param_desc** 
   return TCR_OK;
 }
 
-// Tile rows of the wgmma kernels: at most 128 accumulator rows (RH * wout) per tile, balanced (25 rows -> 5 tiles of 5).
-static int ds_tile_rows(const DsLayerDev& L) {
-  const int cap = std::max(1, std::min(L.hout, 128 / std::max(1, std::min(L.wout, 128))));
-  const int tiles = (L.hout + cap - 1) / cap;
-  return (L.hout + tiles - 1) / tiles;
-}
-
-// The first layer (cin == 1).  WIN: utterance u is the window `win` describes (tcr_listener.cu); the kernel choice is the same.
+// The first layer (cin == 1) on the kernel of its plan (ds_plan_layer).  WIN: utterance u is the window `win` describes
+// (tcr_listener.cu); the kernel choice is the same.
 template <bool WIN>
-static int ds_launch_conv(tcr_dscnn* d, const DsLayerDev& L, const float* params, const float* in, float* out, int32_t n, cudaStream_t s,
+static int ds_launch_conv(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s,
                           WindowView win) {
+  const DsLayerDev& L = d->net.layer[l];
+  const DsPlan& P = d->plan[l];
   const float eps = 1e-3f;
 #ifndef TCR_EMU
-  const int RHt = ds_tile_rows(L), grid = std::min(ds_tiles_per_utt(L, RHt) * n, d->sms);
-  // implicit GEMM on wgmma (3xTF32), where the kernel's per-thread im2col walk covers the tile
-  if (d->use_tc && L.cin == 1 && L.cout == 64 && (L.kh * L.kw) % 8 == 0 && L.wout <= 64 && im2col_walk_fits(L, RHt, kTcThreads)) {
-    const size_t smem_ws = conv_tc_smem<64>(L, RHt, 2).floats * 4;
-    if (d->tc_ws && smem_ws <= 220 * 1024 && im2col_walk_fits(L, RHt, kWsProducers) && (L.kh * L.kw / 4) % 2 == 0) {
-      auto kws = dscnn_conv_ws_kernel<64, WIN>;
-      static SmemOptIn optin_ws;
-      if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
-      TCR_LAUNCH(WIN ? "dscnn_conv_ws:win" : "dscnn_conv_ws", kws, dim3(grid), dim3(kTcThreads), smem_ws, s, L, RHt, n, params, in, out, eps,
-                 win);
-      return TCR_OK;
-    }
-    const size_t smem_tc = conv_tc_smem<64>(L, RHt, 1).floats * 4;
+  const int grid = P.RH ? std::min(ds_tiles_per_utt(L, P.RH) * n, d->sms) : 0;   // wgmma only: dscnn_conv has P.RH = 0
+  if (P.kernel == kDsConvWs) {
+    auto kws = dscnn_conv_ws_kernel<64, WIN>;
+    static SmemOptIn optin_ws;
+    if (optin_ws.ensure(kws, P.smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_conv_ws: shared memory opt-in failed");
+    TCR_LAUNCH(WIN ? "dscnn_conv_ws:win" : "dscnn_conv_ws", kws, dim3(grid), dim3(kTcThreads), P.smem, s, L, P.RH, n, params, in, out, eps,
+               win);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_conv_ws launch failed");
+    return TCR_OK;
+  }
+  if (P.kernel == kDsConvTc) {
     auto ktc = dscnn_conv_tc_kernel<64, WIN>;
     static SmemOptIn optin_tc;
-    if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-    TCR_LAUNCH(WIN ? "dscnn_conv_tc:win" : "dscnn_conv_tc", ktc, dim3(grid), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps,
+    if (optin_tc.ensure(ktc, P.smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_conv_tc: shared memory opt-in failed");
+    TCR_LAUNCH(WIN ? "dscnn_conv_tc:win" : "dscnn_conv_tc", ktc, dim3(grid), dim3(kTcThreads), P.smem, s, L, P.RH, n, params, in, out, eps,
                win);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_conv_tc launch failed");
     return TCR_OK;
   }
 #endif
-  const size_t smem = conv_smem(L).floats * 4;
   auto kfn = dscnn_conv_kernel<WIN>;
 #ifndef TCR_EMU
   static SmemOptIn optin;
-  if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
+  if (optin.ensure(kfn, P.smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_conv: shared memory opt-in failed");
 #endif
-  TCR_LAUNCH(WIN ? "dscnn_conv:win" : "dscnn_conv", kfn, dim3(n), dim3(256), smem, s, L, params, in, out, eps, win);
+  TCR_LAUNCH(WIN ? "dscnn_conv:win" : "dscnn_conv", kfn, dim3(n), dim3(256), P.smem, s, L, params, in, out, eps, win);
+  if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_conv launch failed");
   return TCR_OK;
 }
 
@@ -2922,9 +2992,9 @@ static int res_launch(tcr_dscnn* d, int l, const float* params, const float* in,
 }
 
 // Launches layer l: in [n, hin, win, cin] -> out [n, hout, wout, cout] (NHWC), or for l == 0 with `win` the windows it describes.
-// The kernel is chosen here, once for every entry point: wgmma where the layer's shape fits the tensor-core kernels
-// (TCR_DSCNN_TC), the register-tiled FMA kernels otherwise.  The warp-specialised block kernel reads its input through a TMA map
-// over max_batch utterances, so only from an activation buffer of the handle.
+// DS-CNN S / M / L run the kernel of the layer's plan, chosen once in tcr_dscnn_create (ds_plan_layer) for every entry point.  The
+// warp-specialised block kernel reads its input through a TMA map over max_batch utterances, so only from an activation buffer of
+// the handle, which is where every entry point leaves a block's input.
 static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float* in, float* out, int32_t n, cudaStream_t s,
                            const WindowView* win = nullptr) {
   const DsLayerDev& L = d->net.layer[l];
@@ -2946,60 +3016,50 @@ static int ds_launch_layer(tcr_dscnn* d, int l, const float* params, const float
     return kwsb_launch_conv<false>(d, params, in, out, n, s, WindowView{0, 0, 0});
   }
   if (L.type == 0) {
-    if (win) return ds_launch_conv<true>(d, L, params, in, out, n, s, *win);
-    return ds_launch_conv<false>(d, L, params, in, out, n, s, WindowView{0, 0, 0});
-  } else {
+    if (win) return ds_launch_conv<true>(d, l, params, in, out, n, s, *win);
+    return ds_launch_conv<false>(d, l, params, in, out, n, s, WindowView{0, 0, 0});
+  }
+  const DsPlan& P = d->plan[l];
 #ifndef TCR_EMU
-    // pointwise conv on the tensor cores (wgmma, 3xTF32): the 64 -> 64 channel blocks with a 3x3 / stride-1 depthwise stage
-    if (d->use_tc && L.cin == 64 && L.cout == 64 && L.kh == 3 && L.kw == 3 && L.sh == 1 && L.sw == 1 && L.wout <= 64) {
-      const int RHt = ds_tile_rows(L), grid = std::min(ds_tiles_per_utt(L, RHt) * n, d->sms);
-      const size_t smem_ws = dsblock_ws_smem<64, 64>(L, RHt).floats * 4;
-      if (d->tc_ws && smem_ws <= 226 * 1024 && L.cin / 4 * L.wout <= kWsProducers && L.wout + 2 <= 256 && RHt + 2 <= 256 &&
-          (in == d->act[0] || in == d->act[1])) {
-        auto kws = dscnn_dsblock_ws_kernel<64, 64>;
-        static SmemOptIn optin_ws;
-        if (optin_ws.ensure(kws, smem_ws) != cudaSuccess) return TCR_ERR_CUDA;
-        if ((int)d->in_maps.size() < d->net.nlayers) d->in_maps.resize(d->net.nlayers);
-        tcr_dscnn::InMap& im = d->in_maps[l];
-        if (im.ptr != in || im.rh != RHt) {                    // the activations ping-pong between two buffers: encoded once per layer
-          const int rc = ds_encode_in_map(&im.map, in, L.cin, L.win, L.hin, d->cfg.max_batch, L.wout + 2, RHt + 2);
-          if (rc != TCR_OK) return rc;
-          im.ptr = in;
-          im.rh = RHt;
-        }
-        TCR_LAUNCH("dscnn_dsblock_ws", kws, dim3(grid), dim3(kTcThreads), smem_ws, s, im.map, L, RHt, n, params, out, eps);
-        return TCR_OK;
+  if (P.kernel == kDsBlockWs || P.kernel == kDsBlockTc) {
+    const int grid = std::min(ds_tiles_per_utt(L, P.RH) * n, d->sms);
+    if (P.kernel == kDsBlockWs) {
+      if (in != d->act[0] && in != d->act[1])
+        return ds_fail(TCR_ERR_INVALID, "dscnn_dsblock_ws reads its input through a TMA map over the handle's activation buffers");
+      auto kws = dscnn_dsblock_ws_kernel<64, 64>;
+      static SmemOptIn optin_ws;
+      if (optin_ws.ensure(kws, P.smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_dsblock_ws: shared memory opt-in failed");
+      if ((int)d->in_maps.size() < d->net.nlayers) d->in_maps.resize(d->net.nlayers);
+      tcr_dscnn::InMap& im = d->in_maps[l];
+      if (im.ptr != in || im.rh != P.RH) {                     // the activations ping-pong between two buffers: encoded once per layer
+        const int rc = ds_encode_in_map(&im.map, in, L.cin, L.win, L.hin, d->cfg.max_batch, L.wout + 2, P.RH + 2);
+        if (rc != TCR_OK) return rc;
+        im.ptr = in;
+        im.rh = P.RH;
       }
-      const size_t smem_tc = dsblock_tc_smem<64, 64>(L, RHt).floats * 4;
-      if (smem_tc <= 200 * 1024 && (RHt + 2) * (L.wout + 2) <= kDwCells * (kTcThreads / (L.cin / 4))) {   // the kernel's fetch walk
-        auto ktc = dscnn_dsblock_tc_kernel<64, 64>;
-        static SmemOptIn optin_tc;
-        if (optin_tc.ensure(ktc, smem_tc) != cudaSuccess) return TCR_ERR_CUDA;
-        TCR_LAUNCH("dscnn_dsblock_tc", ktc, dim3(grid), dim3(kTcThreads), smem_tc, s, L, RHt, n, params, in, out, eps);
-        return TCR_OK;
-      }
+      TCR_LAUNCH("dscnn_dsblock_ws", kws, dim3(grid), dim3(kTcThreads), P.smem, s, im.map, L, P.RH, n, params, out, eps);
+      if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_dsblock_ws launch failed");
+      return TCR_OK;
     }
+    auto ktc = dscnn_dsblock_tc_kernel<64, 64>;
+    static SmemOptIn optin_tc;
+    if (optin_tc.ensure(ktc, P.smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_dsblock_tc: shared memory opt-in failed");
+    TCR_LAUNCH("dscnn_dsblock_tc", ktc, dim3(grid), dim3(kTcThreads), P.smem, s, L, P.RH, n, params, in, out, eps);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_dsblock_tc launch failed");
+    return TCR_OK;
+  }
 #endif
-    // the whole pointwise bank in shared memory when it fits next to a useful tile; else (DS-CNN-L: 276 x 276 fp32 = 305 KB) output-
-    // channel tiles of COT, the depthwise output of the tile being reused for every slice
-    int COT = L.cout;
-    while (COT > 32 && dsblock_smem(L, 1, COT).floats * 4 > 96 * 1024) COT = ((COT / 2) + 3) & ~3;
-    int RH = std::min(L.hout, 8);
-    while (RH > 1 && dsblock_smem(L, RH, COT).floats * 4 > 100 * 1024) --RH;
-    const size_t smem = dsblock_smem(L, RH, COT).floats * 4;
-    if (smem > 200 * 1024) { set_error("DS-CNN layer does not fit in shared memory"); return TCR_ERR_UNSUPPORTED; }
-    auto kfn = dscnn_dsblock_kernel;
+  auto kfn = dscnn_dsblock_kernel;
 #ifndef TCR_EMU
-    static SmemOptIn optin;
-    if (optin.ensure(kfn, smem) != cudaSuccess) return TCR_ERR_CUDA;
+  static SmemOptIn optin;
+  if (optin.ensure(kfn, P.smem) != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_dsblock: shared memory opt-in failed");
 #endif
-    // one utterance per blockIdx.y: batches past kMaxGridRows run as several launches over consecutive utterances
-    const size_t in_utt = (size_t)L.hin * L.win * L.cin, out_utt = (size_t)L.hout * L.wout * L.cout;
-    for (int first = 0; first < n; first += kMaxGridRows) {
-      TCR_LAUNCH("dscnn_dsblock", kfn, dim3(ds_tiles_per_utt(L, RH), std::min(n - first, kMaxGridRows)), dim3(256), smem, s, L, RH, COT,
-                 params, in + first * in_utt, out + first * out_utt, eps);
-      if (cudaGetLastError() != cudaSuccess) { set_error("DS-CNN block launch failed"); return TCR_ERR_CUDA; }
-    }
+  // one utterance per blockIdx.y: batches past kMaxGridRows run as several launches over consecutive utterances
+  const size_t in_utt = (size_t)L.hin * L.win * L.cin, out_utt = (size_t)L.hout * L.wout * L.cout;
+  for (int first = 0; first < n; first += kMaxGridRows) {
+    TCR_LAUNCH("dscnn_dsblock", kfn, dim3(ds_tiles_per_utt(L, P.RH), std::min(n - first, kMaxGridRows)), dim3(256), P.smem, s, L, P.RH,
+               P.COT, params, in + first * in_utt, out + first * out_utt, eps);
+    if (cudaGetLastError() != cudaSuccess) return ds_fail(TCR_ERR_CUDA, "dscnn_dsblock launch failed");
   }
   return TCR_OK;
 }

@@ -52,7 +52,8 @@ def check_ds_push(ds, lis, off, samples):
 
 
 def run_case(b, size, case, S, hop, K, pushes=None, reset_at=(), pcm_every=3, seed=0):
-    ds = Ds(b, size, FRONTENDS[case], S * K, seed=seed)
+    """case: a key of FRONTENDS, or a dict of front-end flags."""
+    ds = Ds(b, size, FRONTENDS[case] if isinstance(case, str) else case, S * K, seed=seed)
     lis = DsListener(ds, S, hop, K * hop * ds.cfg.window_stride_samples)
     try:
         off = Offline(ds, S, hop)
