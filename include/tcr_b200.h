@@ -340,8 +340,12 @@ int tcr_listener_history(const tcr_listener* L, float** history, int32_t* frames
  *   scores  device [n, classes]: logits or softmax outputs of tcr_forward (arg-max and ranks are the same for both)
  *   onehot  device [n, classes]
  *   counts  device int64 [classes*classes + 2], ACCUMULATED (zero it before the first batch):
- *           [y*classes + p] confusion matrix (true row, predicted column; first maximum wins like np.argmax),
- *           [classes*classes] utterances whose true class is among the `topk` best scores, [classes*classes + 1] utterances */
+ *           [y*classes + p] confusion matrix (true row, predicted column), y and p the np.argmax of the one-hot and score rows:
+ *                           the first NaN if the row has one, else the first maximum (+0 and -0 are equal),
+ *           [classes*classes] utterances whose true class is among the first `topk` of np.argsort(-scores, kind="stable"): a
+ *                           numeric true score ranks after the greater scores and the equal ones at lower class indices, a NaN
+ *                           true score after every number and the NaNs at lower indices; topk >= classes counts every row,
+ *           [classes*classes + 1] utterances */
 int tcr_eval_accumulate(tcr_handle* h, const float* scores, const float* onehot, int32_t n, int32_t topk, int64_t* counts,
                         tcr_stream stream);
 

@@ -4,8 +4,8 @@
 // (helper/base.py:52-143, metrics/parser.py:135-147) and computes accuracy / top-5 / precision / recall / F1 / the classification
 // report with sklearn (metrics/ops/non_tensor_ops.py:64-142, :146-295, :346-).  All of these are functions of the confusion
 // matrix plus one top-k counter, so the batch is reduced to classes^2 + 2 integers where the scores already are:
-//   counts[y * C + p] += 1     y = arg-max of the one-hot label row, p = arg-max of the score row (first maximum, like np.argmax)
-//   counts[C * C]     += 1     when the true class ranks among the top k scores (ties broken by the lower class index)
+//   counts[y * C + p] += 1     y = arg-max of the one-hot label row, p = arg-max of the score row (first_argmax: np.argmax's rule)
+//   counts[C * C]     += 1     when the true class ranks among the top k scores (true_rank: np.argsort(-scores, kind="stable"))
 //   counts[C * C + 1] += 1     per utterance
 // Integer atomics: exact and order-independent, so the result is bit-identical to the host computation.
 #include "tcr_device.cuh"
@@ -16,24 +16,41 @@
 
 namespace tcr {
 
+// np.argmax of one row: the first NaN if the row has one, else the first maximum
+__device__ __forceinline__ int first_argmax(const float* v, int C) {
+  int p = 0;
+  float best = v[0];
+  if (best != best) return 0;
+  for (int c = 1; c < C; ++c) {
+    const float x = v[c];
+    if (x != x) return c;
+    if (x > best) { best = x; p = c; }
+  }
+  return p;
+}
+
+// Classes ahead of class y in the stable descending sort np.argsort(-s, kind="stable"), which puts every NaN after every number:
+// a number is preceded by the greater scores and the equal ones at lower indices; a NaN by every number and the NaNs at lower indices.
+__device__ __forceinline__ int true_rank(const float* s, int C, int y) {
+  const float sy = s[y];
+  int rank = 0;
+  if (sy == sy) {
+    for (int c = 0; c < C; ++c) rank += (s[c] > sy || (s[c] == sy && c < y)) ? 1 : 0;
+  } else {
+    for (int c = 0; c < C; ++c) rank += (s[c] == s[c] || c < y) ? 1 : 0;
+  }
+  return rank;
+}
+
 __global__ void __launch_bounds__(256) eval_accumulate_kernel(const float* __restrict__ scores, const float* __restrict__ onehot, int n, int C,
                                                               int topk, unsigned long long* counts) {
   pdl_wait();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float* s = scores + (size_t)i * C;
-  const float* l = onehot + (size_t)i * C;
-  int y = 0, p = 0;
-  float ly = l[0], sp = s[0];
-  for (int c = 1; c < C; ++c) {
-    if (l[c] > ly) { ly = l[c]; y = c; }
-    if (s[c] > sp) { sp = s[c]; p = c; }
-  }
-  const float sy = s[y];
-  int rank = 0;                       // classes ranked before the true one by a stable descending sort
-  for (int c = 0; c < C; ++c) rank += (s[c] > sy || (s[c] == sy && c < y)) ? 1 : 0;
+  const int y = first_argmax(onehot + (size_t)i * C, C), p = first_argmax(s, C);
   atomicAdd(counts + (size_t)y * C + p, 1ull);
-  if (rank < topk) atomicAdd(counts + (size_t)C * C, 1ull);
+  if (true_rank(s, C, y) < topk) atomicAdd(counts + (size_t)C * C, 1ull);
   atomicAdd(counts + (size_t)C * C + 1, 1ull);
 }
 
@@ -96,12 +113,7 @@ __global__ void __launch_bounds__(256) eval_collect_kernel(const float* __restri
   if (e >= (int64_t)n * C) return;
   store[e] = scores[e];
   if (e % C) return;
-  const float* l = onehot + e;
-  int y = 0;
-  float ly = l[0];
-  for (int c = 1; c < C; ++c)
-    if (l[c] > ly) { ly = l[c]; y = c; }
-  labels[e / C] = y;
+  labels[e / C] = first_argmax(onehot + e, C);
 }
 
 __global__ void __launch_bounds__(256) rank_items_kernel(const float* __restrict__ store, const int* __restrict__ labels, int64_t L, int C,

@@ -13,7 +13,9 @@ import numpy as np
 
 
 def topn_accuracy(labels_onehot, predictions, n=5):
-    top = np.argsort(-predictions, axis=1)[:, :n]
+    """The reference's topN_accuracy (metrics/funcs.py:4-19) with a stable sort: equal scores keep the lower class first, as on
+    the device (tcr_eval_accumulate), at every class count.  NaN scores rank after every number."""
+    top = np.argsort(-predictions, axis=1, kind="stable")[:, :n]
     return float(np.mean(np.any(top == labels_onehot.argmax(1)[:, None], axis=1)))
 
 
@@ -43,7 +45,7 @@ def ranking_vector(labels_onehot, predictions) -> np.ndarray:
             return 0.0
         order = np.argsort(-score, kind="stable")
         score, pos = score[order], pos[order]
-        ends = np.r_[np.nonzero(np.diff(score))[0], score.size - 1]      # last item of each group of equal scores
+        ends = np.r_[np.nonzero(score[1:] != score[:-1])[0], score.size - 1]   # last item of each group of equal scores (inf too)
         tp = np.cumsum(pos)[ends]
         return float(np.sum(np.diff(np.r_[0, tp]) * tp / (ends + 1.0)) / tp[-1])
 

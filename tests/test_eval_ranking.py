@@ -40,6 +40,10 @@ def case(rng, n, classes, kind="plain"):
             scores[:, 2] = np.where(np.arange(n) % 2, 1.0, 0.0).astype(np.float32)
     if kind == "absent" and classes > 1:
         labels[labels == classes - 1] = 0
+    if kind == "edges":                                  # +-inf, +-0 (one group) and subnormals (not flushed to zero)
+        edge = np.array([np.inf, -np.inf, 0.0, -0.0, 1e-45, 2e-45, -1e-45, 1e-40, np.inf, 0.0], np.float32)
+        pick = rng.random((n, classes)) < 0.4
+        scores[pick] = edge[rng.integers(0, edge.size, pick.sum())]
     return scores, labels
 
 
@@ -109,7 +113,10 @@ def check_against_sklearn(r, n, classes, kind, seed=0, splits=None):
     rng = np.random.default_rng(seed)
     scores, labels = case(rng, n, classes, kind)
     got = r.run(scores, labels, splits)
-    ref = sklearn_vector(scores, labels, classes, samples=n <= 10_000)
+    # sklearn refuses infinite scores; AP depends only on the order and the ties, so it gets each score's rank among the distinct
+    # values (np.unique merges +0 and -0 as the device does)
+    ranked = np.unique(scores, return_inverse=True)[1].reshape(scores.shape).astype(np.float64) if kind == "edges" else scores
+    ref = sklearn_vector(ranked, labels, classes, samples=n <= 10_000)
     assert np.abs(got - ref).max() <= 1e-12, (n, classes, kind, got, ref)
     assert np.abs(ranking_vector(np.eye(classes)[labels], scores) - ref).max() <= 1e-12
     return scores, labels, got
@@ -162,7 +169,7 @@ def emu():
 
 @pytest.mark.parametrize("classes", [1, 2, 12, 32])
 @pytest.mark.parametrize("n", [1, 3, 39, 5000])
-@pytest.mark.parametrize("kind", ["plain", "ties", "absent"])
+@pytest.mark.parametrize("kind", ["plain", "ties", "absent", "edges"])
 def test_emulated_rank_matches_sklearn(emu, classes, n, kind):
     if n == 5000 and kind != "ties" and classes != 32:
         pytest.skip("n = 5000 runs the heaviest cases only: ties at every class count, every kind at 32 classes")
@@ -245,7 +252,7 @@ def cuda():
 @pytest.mark.gpu
 @pytest.mark.parametrize("classes", [1, 2, 12, 32])
 @pytest.mark.parametrize("n", [1, 3, 39, 5000])
-@pytest.mark.parametrize("kind", ["plain", "ties", "absent"])
+@pytest.mark.parametrize("kind", ["plain", "ties", "absent", "edges"])
 def test_cuda_rank_matches_sklearn(cuda, classes, n, kind):
     r = Ranker(cuda, classes, dscnn=kind == "absent")
     try:
