@@ -17,6 +17,7 @@ index block of BlockHandles, 48-byte footer with the table magic 0xdb4775248b80f
 """
 from __future__ import annotations
 
+import functools
 import os
 import struct
 from pathlib import Path
@@ -49,10 +50,43 @@ def _make_table():
 
 _CRC_TABLE = _make_table()
 _CRC_LIST = [int(x) for x in _CRC_TABLE]
+_CHUNK = 32                   # bytes per chunk of the chunk-parallel path
+
+
+def _shift(tables: np.ndarray, regs: np.ndarray) -> np.ndarray:
+    return tables[0][regs & 0xFF] ^ tables[1][(regs >> 8) & 0xFF] ^ tables[2][(regs >> 16) & 0xFF] ^ tables[3][regs >> 24]
+
+
+@functools.lru_cache(maxsize=None)
+def _zeros_tables(n: int) -> np.ndarray:
+    """The CRC register after n zero bytes (n = _CHUNK * 2^k), as lookup tables [4, 256] on the bytes of the starting register
+    (the map is linear over GF(2)); 2n is n applied twice."""
+    if n > _CHUNK:
+        half = _zeros_tables(n // 2)
+        return _shift(half, half)
+    regs = (np.arange(256, dtype=np.uint32)[None, :] << (8 * np.arange(4, dtype=np.uint32))[:, None]).ravel()
+    for _ in range(n):
+        regs = _CRC_TABLE[regs & 0xFF] ^ (regs >> 8)
+    return regs.reshape(4, 256)
 
 
 def crc32c(data: bytes, crc: int = 0) -> int:
     c = crc ^ 0xFFFFFFFF
+    n = len(data) // _CHUNK
+    if n >= 64:               # large inputs (audio summaries): every chunk's register in one NumPy pass, then folded pairwise
+        levels = (n - 1).bit_length()
+        regs = np.zeros(1 << levels, np.uint32)
+        first = (1 << levels) - n                            # leading all-zero registers leave the result unchanged
+        regs[first] = c
+        cols = np.frombuffer(data, np.uint8, n * _CHUNK).reshape(n, _CHUNK).T
+        for col in cols:
+            regs[first:] = _CRC_TABLE[(regs[first:] ^ col) & 0xFF] ^ (regs[first:] >> 8)
+        size = _CHUNK
+        while regs.size > 1:
+            regs = _shift(_zeros_tables(size), regs[0::2]) ^ regs[1::2]
+            size *= 2
+        c = int(regs[0])
+        data = data[n * _CHUNK:]
     tab = _CRC_LIST
     for b in data:
         c = tab[(c ^ b) & 0xFF] ^ (c >> 8)

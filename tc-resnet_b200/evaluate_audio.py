@@ -39,15 +39,18 @@ def main(args, loop_timeout=None):
     evaluator = SingleLabelAudioEvaluator(model, session, args, dataset, dataset_name)
     log = utils.get_logger("EvaluateAudio")
     results = []
-    if args.valid_type == "once":
-        results.append(evaluator.evaluate_once(ckpt.resolve_checkpoint_path(args.checkpoint_path)))
-    elif args.valid_type == "loop":
-        log.info(f"Start Loop: watching {evaluator.watch_path}")
-        for path in ckpt.checkpoints_iterator(evaluator.watch_path, timeout=loop_timeout):
-            log.info(f"[watch] {path}")
-            results.append(evaluator.evaluate_once(path))
-    else:
-        raise ValueError(f"Undefined valid_type: {args.valid_type}")
+    try:
+        if args.valid_type == "once":
+            results.append(evaluator.evaluate_once(ckpt.resolve_checkpoint_path(args.checkpoint_path)))
+        elif args.valid_type == "loop":
+            log.info(f"Start Loop: watching {evaluator.watch_path}")
+            for path in ckpt.checkpoints_iterator(evaluator.watch_path, timeout=loop_timeout):
+                log.info(f"[watch] {path}")
+                results.append(evaluator.evaluate_once(path))
+        else:
+            raise ValueError(f"Undefined valid_type: {args.valid_type}")
+    finally:
+        evaluator.metric_manager.close_summaries()
     return results
 
 

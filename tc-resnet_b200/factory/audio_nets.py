@@ -10,6 +10,7 @@ training is out of scope and raises NotImplementedError).
 """
 from __future__ import annotations
 
+import collections
 from typing import Dict, Optional, Set
 
 import numpy as np
@@ -52,6 +53,8 @@ class AudioNetModel(TFModel):
         self._counts = None                                        # device int64 [classes^2 + 2] (tcr_eval_accumulate)
         self._rank = None                                          # (scores, labels, workspace) of the ranking store (tcr_eval_collect)
         self._rank_rows = 0
+        self.reported_losses = collections.deque(maxlen=256)      # (global step, total_loss, model_loss) of each finished step
+        self._clip_request, self._clips = 0, None                   # audio summaries: clips kept from the next training step
 
     # ------------------------------------------------------------------ graph-construction API of the reference
     def build(self, wavs, labels, is_training):
@@ -341,6 +344,7 @@ class AudioNetModel(TFModel):
             slot[0].copy_(torch.from_numpy(wav_np.reshape(n, -1)))
             slot[1].copy_(torch.from_numpy(hot_np))
             pinned = slot
+        self._keep_clips(pinned[0])
         if self._feed is None:
             from ..engine import HostFeed
             self._feed = HostFeed(self.engine, lag=lag)
@@ -352,7 +356,7 @@ class AudioNetModel(TFModel):
         self.global_step += 1
         self._feed_steps.append(self.global_step)
         if r is not None:
-            self._feed_last = (self._feed_steps.pop(0), np.float32(r[1]), np.float32(r[2]))
+            self._report_loss(self._feed_steps.pop(0), r[1], r[2])
             if not np.isfinite(r[1]):
                 raise InvalidArgumentError(f"non-finite loss at step {self._feed_last[0]} (malformed input batch?)")
         step, total, model = self._feed_last
@@ -378,6 +382,8 @@ class AudioNetModel(TFModel):
                                dataset=ds.device_data.desc, position=position, epoch=epoch, seed=ds.draw_seed, n=self.args.batch_size)
         slot[1].copy_(slot[0], non_blocking=True)
         slot[2].record()
+        if self._clip_request:
+            self._keep_clips(ds.device_data.batch(position, epoch, ds.draw_seed, min(self._clip_request, self.args.batch_size))[0])
         self._advance_optimizer()
         self.global_step += 1
         self._feed_steps.append(self.global_step)
@@ -391,15 +397,44 @@ class AudioNetModel(TFModel):
     def _collect_loss(self):
         _, host, event = self._loss_pending.pop(0)
         event.synchronize()
-        self._feed_last = (self._feed_steps.pop(0), np.float32(host[0]), np.float32(host[1]))
+        self._report_loss(self._feed_steps.pop(0), host[0], host[1])
         if not np.isfinite(self._feed_last[1]):
             raise InvalidArgumentError(f"non-finite loss at step {self._feed_last[0]}")
+
+    def _report_loss(self, step, total, model):
+        self._feed_last = (step, np.float32(total), np.float32(model))
+        self.reported_losses.append(self._feed_last)
+
+    def capture_clips(self, k: int):
+        """The next training step keeps the first k clips of its batch for an audio summary (take_clips).  A batch built on the
+        device is regenerated for those rows and copied to pinned memory behind the step, so nothing waits for it here."""
+        self._clip_request = int(k)
+
+    def take_clips(self):
+        """The clips kept by the last training step since capture_clips, as (host tensor [k, samples], event or None), or None.
+        The tensor is valid once the event (the step's copy) has completed."""
+        clips, self._clips, self._clip_request = self._clips, None, 0
+        return clips
+
+    def _keep_clips(self, wav):
+        k = min(self._clip_request, wav.shape[0])
+        if k <= 0:
+            return
+        if isinstance(wav, np.ndarray) or not wav.is_cuda:
+            self._clips = (torch.as_tensor(wav[:k]).reshape(k, -1).clone(), None)
+        else:
+            host = torch.empty((k, wav.shape[1]), dtype=torch.float32).pin_memory()
+            host.copy_(wav[:k], non_blocking=True)
+            event = torch.cuda.Event()
+            event.record()
+            self._clips = (host, event)
+        self._clip_request = 0
 
     def flush_feed(self):
         """Drain the host-feed pipeline (before anything reads the variables: checkpoints, evaluation, get_variables)."""
         if self._feed is not None:
             for r in self._feed.flush():
-                self._feed_last = (self._feed_steps.pop(0), np.float32(r[1]), np.float32(r[2]))
+                self._report_loss(self._feed_steps.pop(0), r[1], r[2])
         while self._loss_pending:
             self._collect_loss()
 
@@ -447,6 +482,10 @@ class AudioNetModel(TFModel):
             vals["metric_counts"] = None
         losses = out["losses"].cpu().numpy()                    # the D2H read synchronises the step
         vals.update(total_loss=losses[0], model_loss=losses[1], global_step=np.int64(self.global_step))
+        if "train_op" in names:
+            self.reported_losses.append((self.global_step, losses[0], losses[1]))
+            if self._clip_request:
+                self._keep_clips(wav_np if device_data is None else self._d_wav)
         if device_data is None:
             vals.update(labels=hot_np, audio_original=wav_np)
         else:                                                   # copied to the host only when fetched

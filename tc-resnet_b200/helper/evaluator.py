@@ -11,7 +11,7 @@ from pathlib import Path
 from ..common import checkpoint as ckpt
 from ..common import model_loader
 from ..common.utils import get_logger
-from ..metrics.manager import AudioMetricManager
+from ..metrics.manager import KEY_TYPES, AudioMetricManager, Summaries, summary_directory
 from .base import AudioBase
 
 
@@ -50,6 +50,7 @@ class Evaluator:
         keep = self.metric_manager.filter_best_keep_metric(metrics)
         if self.args.save_best_keeper:
             self.keep_best(keep, str(checkpoint_path), step)
+        self.metric_manager.write_evaluation_summaries(step, [KEY_TYPES.DEFAULT])
         self.metric_manager.log_metrics(step, self.log.info)
         self.log.info("Evaluation finished")
         if step >= self.args.max_step_from_restore:
@@ -90,8 +91,11 @@ class SingleLabelAudioEvaluator(Evaluator, AudioBase):
         super().__init__(model, session, args, dataset, dataset_name, "SingleLabelAudioEvaluator")
         assert len(self.dataset.label_names) == self.args.num_classes
         self.use_class_metrics = len(self.dataset.label_names) < self.args.maximum_num_labels_for_metric
+        summary = Summaries(summary_directory(self.watch_path, False, self.dataset.dataset_split_name), self.args.max_outputs,
+                            self.args.sample_rate)
+        summary.setup_experiment(self.args)
         self.metric_manager = AudioMetricManager(is_training=False, use_class_metrics=self.use_class_metrics,
-                                                 exclude_metric_names=self.args.exclude_metric_names)
+                                                 exclude_metric_names=self.args.exclude_metric_names, summary=summary)
         self.metric_tf_op = self.metric_manager.build_metric_ops({
             "dataset_split_name": self.dataset_name, "label_names": self.dataset.label_names,
             "losses": self.build_basic_loss_ops(), "learning_rate": None, "wavs": self.model.audio_original})

@@ -17,7 +17,7 @@ from pathlib import Path
 from ..common import checkpoint as ckpt
 from ..common import model_loader
 from ..common import utils
-from ..metrics.manager import AudioMetricManager
+from ..metrics.manager import KEY_TYPES, AudioMetricManager, Summaries, summary_collections, summary_directory
 from ..runtime import InvalidArgumentError, Node, no_op
 from .base import AudioBase
 
@@ -164,14 +164,55 @@ class TrainerBase:
             dist.barrier()
         return path
 
+    # ---- step summaries ----------------------------------------------------------------------
+    def prepare_step_summaries(self):
+        """Before a step: the collections it writes (summary_collections, on the step_from_restore it will report), and with an
+        audio summary among them the model is asked to keep its clips.  Returns (global step, collections, learning rate)."""
+        self.model.take_clips()                        # nothing left from a step that raised
+        step = self.model.global_step + 1
+        a = self.args
+        keys = summary_collections(step - self.global_step_from_checkpoint, a.step_min_summaries, a.step_save_summaries,
+                                   a.step_save_verbose_summaries, a.step_save_first_n_summaries)
+        if not keys or self.metric_manager.summary is None or not self.metric_manager.step_summary_tags(keys):
+            return None
+        if self.metric_manager.wants_clips(keys):
+            self.model.capture_clips(a.max_outputs)
+        return step, keys, float(self.model.lr_schedule(step - 1))
+
+    def write_step_summaries(self, final: bool = False):
+        """Writes the pending step summaries whose losses the model has reported (the host-feed pipeline reports a step's losses
+        `feed_lag` steps later, from pinned memory, so no step waits for a summary).  final: the rest too, without losses."""
+        for step, total, model in list(self.model.reported_losses):
+            entry = self._pending_summaries.pop(int(step), None)
+            if entry is not None:
+                self._write_step_summary(step, entry, {"total_loss": total, "model_loss": model})
+        self.model.reported_losses.clear()
+        if final:
+            for step in sorted(self._pending_summaries):
+                self._write_step_summary(step, self._pending_summaries.pop(step), {})
+
+    def _write_step_summary(self, step, entry, losses):
+        keys, lr, clips = entry
+        if clips is not None:
+            host, event = clips
+            if event is not None:
+                event.synchronize()            # the step's copy: complete by now, its losses (copied after it) have arrived
+            clips = host.numpy()
+        self.metric_manager.write_step_summaries(step, keys, losses, lr, clips)
+
     def train(self, name: str = "Training"):
         self.log.info(f"{name} started")
         global_step, step_from_restore, epoch_from_restore = 0, 0, 0
+        self._pending_summaries = {}
         while True:
             try:
                 feed_dict = self.get_feed_dict(is_training=True)
                 metric_ops = self.metric_tf_op if step_from_restore % self.args.step_evaluation == 0 else None
+                summary = self.prepare_step_summaries()
                 _, global_step, step_from_restore, epoch_from_restore = self.run_with_logging(None, metric_ops, feed_dict)
+                if summary is not None:
+                    self._pending_summaries[summary[0]] = (summary[1], summary[2], self.model.take_clips())
+                self.write_step_summaries()
                 if step_from_restore % self.args.step_save_checkpoint == 0:
                     self.save_checkpoint(global_step)
                 if step_from_restore % self.args.step_evaluation == 0:
@@ -186,6 +227,10 @@ class TrainerBase:
                 self.log.error(f"Invalid instance is detected: {e}")
                 continue
         self.save_checkpoint(global_step)
+        if self.metric_manager.summary is not None:
+            self.model.flush_feed()
+            self.write_step_summaries(final=True)
+            self.metric_manager.close_summaries()
         self.log.info(f"{name} finished")
 
     def evaluate(self, epoch_from_restore, step_from_restore, global_step, dataset_name, iters=None):
@@ -196,6 +241,8 @@ class TrainerBase:
             data = self.build_non_tensor_data_from_eval_dict(eval_dict)
             self.metric_manager.evaluate_and_aggregate_metrics(step=global_step, non_tensor_data=data, eval_dict=eval_dict)
         if self.is_chief:
+            self.write_step_summaries()                # the evaluation drained the pipeline: keep the file in step order
+            self.metric_manager.write_evaluation_summaries(global_step, [KEY_TYPES.DEFAULT])
             self.metric_manager.log_metrics(global_step, self.log.info)
 
     @staticmethod
@@ -244,12 +291,17 @@ class SingleLabelAudioTrainer(TrainerBase, AudioBase):
         assert len(self.label_names) == self.args.num_classes
         self.use_class_metrics = len(self.label_names) < self.args.maximum_num_labels_for_metric
         self.setup_trainer()
+        # rank 0 alone writes summaries; the other ranks open no writer (DESIGN.md section 4m)
+        summary = Summaries(summary_directory(self.args.train_dir, True, self.dataset_name), self.args.max_outputs,
+                            self.args.sample_rate) if self.is_chief else None
         self.metric_manager = AudioMetricManager(is_training=True, use_class_metrics=self.use_class_metrics,
-                                                 exclude_metric_names=self.args.exclude_metric_names)
+                                                 exclude_metric_names=self.args.exclude_metric_names, summary=summary)
         self.metric_tf_op = self.metric_manager.build_metric_ops({
             "dataset_split_name": self.dataset_name, "label_names": self.dataset.label_names,
             "losses": self.build_basic_loss_ops(), "learning_rate": self.learning_rate_placeholder,
             "wavs": self.model.audio_original})
+        if summary is not None:
+            summary.setup_experiment(self.args)
         self.log.info(f"--checkpoint_path {self.train_dir_name}")
 
     def build_evaluate_iterations(self, iters):

@@ -1,15 +1,70 @@
-"""Host-side metrics on the aggregated [num_samples, num_classes] arrays the hot path returns.
+"""Host-side metrics on the aggregated [num_samples, num_classes] arrays the hot path returns, and their TensorBoard summaries.
 
-The reference routes these through a metric-op registry + TensorBoard summaries (metrics/, ~1.26 kLoC, sklearn);
-that observability layer is out of scope (SURVEY.md 2 #16).  What the trainer / evaluator loops need is kept:
-the flag surface of MetricManagerBase.add_arguments (metrics/base.py:250-260), accuracy / top-5 / per-class
-precision-recall-F1 / mAP computed with NumPy, `get_best_keep_metric_with_modes`, and a log line per evaluation.
+The reference routes these through a metric-op registry + TensorBoard summaries (metrics/, ~1.26 kLoC, sklearn).  What the
+trainer / evaluator loops need is kept: the flag surface of MetricManagerBase.add_arguments (metrics/base.py:250-260),
+accuracy / top-5 / per-class precision-recall-F1 / mAP computed with NumPy, `get_best_keep_metric_with_modes`, a log line
+per evaluation, and the summaries of metrics/summaries.py:11-202 written by common/tf_events (DESIGN.md section 4m):
+`summary_table` restates which op registers which tag in which collection, `summary_collections` the trainer's schedule.
 """
 from __future__ import annotations
 
-from typing import Dict, List
+from pathlib import Path
+from types import SimpleNamespace
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
+
+from ..common.tf_events import EventWriter, audio_values, scalar_value, text_value
+
+# metrics/summaries.py:12-23
+KEY_TYPES = SimpleNamespace(DEFAULT="SUMMARY_DEFAULT", VERBOSE="SUMMARY_VERBOSE", FIRST_N="SUMMARY_FIRST_N")
+VALUE_TYPES = SimpleNamespace(SCALAR="SCALAR", PLACEHOLDER="PLACEHOLDER", AUDIO="AUDIO")
+
+
+def summary_collections(step_from_restore: int, step_min_summaries: int, step_save_summaries: int,
+                        step_save_verbose_summaries: int, step_save_first_n_summaries: int) -> List[str]:
+    """The collections a training step writes (helper/trainer.py:374-385): DEFAULT from step_min_summaries on, every
+    step_save_summaries steps; VERBOSE every step_save_verbose_summaries steps; FIRST_N up to step_save_first_n_summaries."""
+    keys = []
+    if step_from_restore >= step_min_summaries and step_from_restore % max(1, step_save_summaries) == 0:
+        keys.append(KEY_TYPES.DEFAULT)
+    if step_from_restore % max(1, step_save_verbose_summaries) == 0:
+        keys.append(KEY_TYPES.VERBOSE)
+    if step_from_restore <= step_save_first_n_summaries:
+        keys.append(KEY_TYPES.FIRST_N)
+    return keys
+
+
+def summary_directory(train_dir, is_training: bool, base_name: str) -> Path:
+    """metrics/summaries.py:130-142: the training directory itself, or `<dir>/<split>` for an evaluator (the directory of a
+    checkpoint path that is a file)."""
+    if is_training:
+        return Path(train_dir)
+    return (Path(train_dir) if Path(train_dir).is_dir() else Path(train_dir).parent) / base_name
+
+
+class Summaries:
+    """One event-file writer (metrics/summaries.py:BaseSummaries): the `config` text once, then Summary events by step."""
+
+    def __init__(self, directory, max_outputs: int, sample_rate: int = 16000):
+        self.writer = EventWriter(directory)
+        self.max_outputs, self.sample_rate = int(max_outputs), int(sample_rate)
+
+    def setup_experiment(self, config):
+        """The sorted (flag, str(value)) table as tf.summary.text("config") (metrics/summaries.py:47-59).  There is no graph to
+        add: the step is one fused CUDA launch sequence, not a TF graph."""
+        rows = [(k, str(v)) for k, v in sorted(vars(config).items(), key=lambda x: x[0])]
+        self.writer.add(0, [text_value("config", rows)])
+        self.writer.flush()
+
+    def write(self, step: int, values: Sequence[bytes]):
+        self.writer.add(step, values)
+
+    def flush(self):
+        self.writer.flush()
+
+    def close(self):
+        self.writer.close()
 
 
 def topn_accuracy(labels_onehot, predictions, n=5):
@@ -103,14 +158,50 @@ class MetricManagerBase:
 
 
 class AudioMetricManager(MetricManagerBase):
-    def __init__(self, is_training: bool, use_class_metrics: bool, exclude_metric_names: List[str], summary=None):
+    def __init__(self, is_training: bool, use_class_metrics: bool, exclude_metric_names: List[str],
+                 summary: Optional[Summaries] = None):
         self.is_training, self.use_class_metrics = is_training, use_class_metrics
         self.exclude = set(exclude_metric_names or [])
         self.results: Dict[int, Dict[str, float]] = {}
+        self.summary = summary
+        self.summary_table: List[tuple] = []
 
     def build_metric_ops(self, data):          # tensor metrics (losses / learning rate) are fetched with the step
+        """Registers the step summaries of metrics/manager.py:20-37 as (op, tag, value type, collection) rows: LossesMetricOp
+        (metric_loss/<split>/<loss>), and in training LearningRateSummaryOp (learning_rate/<split>) and WavSummaryOp
+        (wav/<split>), each in DEFAULT as the reference registers them; an op named in --exclude_metric_names is left out.
+        The evaluation metrics are written under their result keys (write_evaluation_summaries)."""
         self.label_names = data["label_names"]
+        split = self.split = data["dataset_split_name"]
+        rows = [("LossesMetricOp", f"metric_loss/{split}/{name}", VALUE_TYPES.SCALAR, KEY_TYPES.DEFAULT) for name in data["losses"]]
+        if self.is_training:
+            if data.get("learning_rate") is not None:
+                rows.append(("LearningRateSummaryOp", f"learning_rate/{split}", VALUE_TYPES.SCALAR, KEY_TYPES.DEFAULT))
+            rows.append(("WavSummaryOp", f"wav/{split}", VALUE_TYPES.AUDIO, KEY_TYPES.DEFAULT))
+        self.summary_table = [r for r in rows if r[0] not in self.exclude]
         return {}
+
+    def step_summary_tags(self, collection_keys) -> List[tuple]:
+        return [r for r in self.summary_table if r[3] in collection_keys]
+
+    def wants_clips(self, collection_keys) -> bool:
+        return self.summary is not None and any(r[2] == VALUE_TYPES.AUDIO for r in self.step_summary_tags(collection_keys))
+
+    def write_step_summaries(self, step, collection_keys, losses: Dict[str, float], learning_rate=None, clips=None):
+        """The step summaries of `collection_keys` at `step`: the step's losses by name, its learning rate and its first
+        --max_outputs clips [n, samples] (tf.summary.audio at 16 kHz).  Values that are None are skipped."""
+        if self.summary is None:
+            return
+        values = []
+        for op, tag, kind, _ in self.step_summary_tags(collection_keys):
+            loss = losses.get(tag[len(f"metric_loss/{self.split}/"):]) if op == "LossesMetricOp" else None
+            if loss is not None:
+                values.append(scalar_value(tag, loss))
+            elif op == "LearningRateSummaryOp" and learning_rate is not None:
+                values.append(scalar_value(tag, learning_rate))
+            elif kind == VALUE_TYPES.AUDIO and clips is not None:
+                values += audio_values(tag, clips, self.summary.sample_rate, self.summary.max_outputs)
+        self.summary.write(step, values)
 
     def get_best_keep_metric_with_modes(self):
         return {"accuracy": "max"}
@@ -152,5 +243,15 @@ class AudioMetricManager(MetricManagerBase):
         scalars = {k: round(v, 5) for k, v in self.results[int(step)].items() if np.isscalar(v)}
         log(f"[step {step}] " + " / ".join(f"{k}: {v}" for k, v in scalars.items() if "/" not in k or k.startswith("mAP/")))
 
-    def write_evaluation_summaries(self, step, collection_keys=None):
-        pass   # TensorBoard plumbing is out of scope
+    def write_evaluation_summaries(self, step, collection_keys=(KEY_TYPES.DEFAULT,)):
+        """Every scalar result of the evaluation at `step` (the keys of the log line and the per-class ones), in DEFAULT as the
+        reference's non-tensor metric ops; the file is flushed."""
+        if self.summary is None or KEY_TYPES.DEFAULT not in collection_keys:
+            return
+        res = self.results[int(step)]
+        self.summary.write(int(step), [scalar_value(k, v) for k, v in res.items() if np.isscalar(v)])
+        self.summary.flush()
+
+    def close_summaries(self):
+        if self.summary is not None:
+            self.summary.close()
